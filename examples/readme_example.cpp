@@ -1,5 +1,5 @@
 // The reference README's 3-vertex example (README.md:105-139 of ethz-asl/mav_trajectory_generation), unchanged
-// apart from the include root: solveLinear() runs on the B200 behind include/mtg_b200.h.
+// apart from the include root: solveLinear() runs on the H100 behind include/mtg_b200.h.
 //
 //   g++ -std=c++17 -I mav_trajectory_generation_b200/host/include -I include examples/readme_example.cpp \
 //       -L mav_trajectory_generation_b200 -lmtg_host -lmtg_b200 -Wl,-rpath,$PWD/mav_trajectory_generation_b200 -o readme_example

@@ -1,5 +1,5 @@
 /*
- * mtg_b200.h -- C-ABI of the B200-native batched linear min-derivative solver.
+ * mtg_b200.h -- C-ABI of the H100-native batched linear min-derivative solver.
  *
  * Drop-in boundary for ONE path of ethz-asl/mav_trajectory_generation:
  * PolynomialOptimization<N>::solveLinear() and the per-segment assembly feeding it.
@@ -33,7 +33,7 @@
  *     trouble is reported in status[] and never stops the batch.
  *   - a handle is bound to one CUDA device and is single-caller (the reference object is not
  *     thread-safe either); use one handle per host thread / per GPU.
- *   - there is NO CPU fallback: every compute entry point launches sm_100a kernels or fails.
+ *   - there is NO CPU fallback: every compute entry point launches sm_90a kernels or fails.
  */
 #ifndef MTG_B200_H_
 #define MTG_B200_H_
@@ -50,7 +50,7 @@ extern "C" {
 #define MTG_OK 0
 #define MTG_ERR_BAD_ARG (-1)      /* null pointer, odd N, r out of [0, N/2-1], K < 1, D < 1 ... */
 #define MTG_ERR_CUDA (-2)         /* CUDA runtime error; see mtg_last_error() */
-#define MTG_ERR_NO_DEVICE (-3)    /* no sm_100 device / extension cannot run */
+#define MTG_ERR_NO_DEVICE (-3)    /* no sm_90 device / extension cannot run */
 #define MTG_ERR_ALLOC (-4)
 
 /* per-trajectory status bits (status[b] == 0 means solved) */
@@ -91,13 +91,13 @@ const char* mtg_last_error(const mtg_handle* h);
 /* number of kernels this handle has launched so far (bench.py's gpu_launches) */
 int64_t mtg_launch_count(const mtg_handle* h);
 /* 1 when the visible device of the handle is compute capability 10.x */
-int mtg_device_is_sm100(const mtg_handle* h);
+int mtg_device_is_sm90(const mtg_handle* h);
 
 /* tuning knobs (results are identical to rounding; used by tests and profiles)
  *   MTG_OPT_WAYPOINT_VARIANT: 0 = default (6 where it applies, else 4 for K <= 8, 3 while the factor fits on chip at
  *                                 two CTAs per SM, 5 beyond),
  *                             1 = one thread per trajectory, 2 = twisted (state in shared memory),
- *                             3 = twisted with the sweep state in tensor memory + TMA tensor stores,
+ *                             3 = twisted with the sweep state in shared memory + TMA tensor stores,
  *                             4 = persistent version of 3 with deep input prefetch,
  *                             5 = chunked (checkpoint + recompute) kernel, any K (default for K too large for 3),
  *                             6 = 4 with the inputs moved by TMA bulk copies (B % 16 == 0, 16-byte aligned inputs, K

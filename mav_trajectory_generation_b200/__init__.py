@@ -1,4 +1,4 @@
-"""B200-native batched minimum-derivative trajectory solve (drop-in for
+"""H100-native batched minimum-derivative trajectory solve (drop-in for
 mav_trajectory_generation::PolynomialOptimization<N>::solveLinear()).
 
 Python here is plumbing for tests and benchmarks; the product is the C-ABI library

@@ -1,4 +1,4 @@
-"""In-tree build of the native libraries (nvcc for sm_100a, g++ for the host mirror).
+"""In-tree build of the native libraries (nvcc for sm_90a, g++ for the host mirror).
 
   libmtg_b200.so   CUDA kernels + the C-ABI of include/mtg_b200.h          (csrc/*.cu)
   libmtg_host.so   C++ mirror of the reference's Vertex/Segment/Polynomial/
@@ -18,7 +18,7 @@ HOST = os.path.join(PKG, "host")
 LIB_CUDA = os.path.join(PKG, "libmtg_b200.so")
 LIB_HOST = os.path.join(PKG, "libmtg_host.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-shared", "-Wall"]
 

@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI (include/mtg_b200.h) for tests, bench.py and smoke().
 
 This is plumbing only: device memory comes from torch tensors (data_ptr), streams from
-torch.cuda.  There is NO fallback: if libmtg_b200.so is missing or no sm_100 device is present
+torch.cuda.  There is NO fallback: if libmtg_b200.so is missing or no sm_90 device is present
 every entry point raises.
 """
 import ctypes as C
@@ -22,7 +22,7 @@ OPT_TMA_INPUTS = 9
 OPT_EARLY_REFILL = 10
 
 EXPORTED_SYMBOLS = [
-    "mtg_create", "mtg_destroy", "mtg_last_error", "mtg_launch_count", "mtg_device_is_sm100",
+    "mtg_create", "mtg_destroy", "mtg_last_error", "mtg_launch_count", "mtg_device_is_sm90",
     "mtg_problem_layout", "mtg_solve_linear_batch_f64", "mtg_coeffs_from_constraints_batch_f64",
     "mtg_compute_cost_batch_f64", "mtg_solve_linear_batch_host_f64",
     "mtg_coeffs_from_constraints_batch_host_f64", "mtg_compute_cost_batch_host_f64",
@@ -66,7 +66,7 @@ def load():
     L.mtg_last_error.argtypes = [vp]
     L.mtg_launch_count.restype = i64
     L.mtg_launch_count.argtypes = [vp]
-    L.mtg_device_is_sm100.argtypes = [vp]
+    L.mtg_device_is_sm90.argtypes = [vp]
     L.mtg_problem_layout.argtypes = [C.POINTER(MtgProblem), C.POINTER(MtgLayout), vp]
     L.mtg_solve_linear_batch_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dp, dp, dp, vp]
     L.mtg_coeffs_from_constraints_batch_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dp, dp, vp]

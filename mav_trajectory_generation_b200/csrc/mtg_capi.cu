@@ -1,6 +1,6 @@
 // mtg_capi.cu -- the C-ABI (include/mtg_b200.h): handle, host-side constraint layout,
 // kernel routing and the pipelined host-buffer entry points.  No CPU compute path exists
-// here: every mtg_*_batch_* call launches sm_100a kernels or returns an error.
+// here: every mtg_*_batch_* call launches sm_90a kernels or returns an error.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -75,11 +75,11 @@ struct mtg_handle {
   Arena pack[kPipe + 1];     // times + d_fixed produced by nfabian_pack_kernel; Mellinger expansion
   Arena counters[kPipe + 1]; // dynamic tile counter of the persistent kernels (event-ordered like the scratch arenas: two
                              // launches of one slot on different caller streams must not share a live counter)
-  // cached launch plans of the TMEM kernel (per waypoint entry and K): attributes are set once
+  // cached launch plans of the v3 kernel (per waypoint entry and K): attributes are set once
   struct TmemPlan {
     const void* entry = nullptr;
     int K = 0;
-    int cols = 0, ntm = 0, ctas = 0;
+    int ctas = 0;
     size_t smem = 0;
     bool attr_plain = false, attr_fused = false;
   };
@@ -179,9 +179,9 @@ struct WaypointEntry {
   int N, R, D, slots;
   WaypointKernel fn;          // one thread per trajectory
   WaypointKernel fn_twisted;  // two lanes per trajectory (twisted factorisation)
-  void (*fn_tmem)(const mtg::WaypointParams, const mtg::TmemLaunch, const CUtensorMap);  // + TMEM state, TMA stores
+  void (*fn_tmem)(const mtg::WaypointParams, const CUtensorMap);  // + shared-memory state, TMA stores
   int stage_bytes_per_warp;
-  void (*fn_tmem_fused)(const mtg::WaypointParams, const mtg::TmemLaunch, const CUtensorMap);  // + fused Nfabian
+  void (*fn_tmem_fused)(const mtg::WaypointParams, const CUtensorMap);  // + fused Nfabian
   void (*fn_chunked)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap);  // any K (K3)
 };
 #define MTG_WP(N_, R_, D_)                                                                   \
@@ -207,7 +207,7 @@ const WaypointEntry kWaypointKernels[] = {
 };
 
 // ---- cost-only kernels (computeCost of the solution without writing coefficients; Mellinger expansion on the fly)
-typedef void (*TmemKernel)(const mtg::WaypointParams, const mtg::TmemLaunch, const CUtensorMap);
+typedef void (*TmemKernel)(const mtg::WaypointParams, const CUtensorMap);
 struct CostEntry {
   int N, R, D;
   TmemKernel fn;
@@ -222,8 +222,7 @@ const CostEntry* find_cost(const mtg_problem* p) {
 }
 
 // ---- v4 (persistent, deep input prefetch) kernels: the default for short trajectories (K <= 8), where the per-tile
-// prologue of the per-tile kernel is a large share of a tile (profiles/r02_k1_variants.json: C2 +11 %, C4 +18 %;
-// at K = 16 the per-tile kernel is 5 % faster and stays the default)
+// prologue of the per-tile kernel is a large share of a tile
 typedef void (*V4Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV4, const CUtensorMap);
 struct V4Entry {
   int N, R, D;
@@ -238,10 +237,9 @@ const V4Entry kV4Kernels[] = {MTG_V4(10, 4, 3, 2), MTG_V4(8, 3, 3, 3), MTG_V4(10
                               MTG_V4(10, 2, 3, 2), MTG_V4(12, 5, 3, 2)};
 constexpr int kV4MaxK = 8;
 
-// ---- v5: v4 with the inputs moved by TMA bulk copies (whole 16-trajectory tiles, double buffered); K <= 8
+// ---- v5: v4 with the inputs moved by TMA bulk copies (whole 16-trajectory tiles, double buffered when two fit)
 typedef void (*V5Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV5, const CUtensorMap);
-// lead (outward-sweep steps) of the single-buffer tile refill: measured on C3 / C5-on-one-GPU / K = 14 with E = off, 1, 2, 3,
-// 4 -> 0.625 / 0.638 / 0.646 / 0.641 / 0.639 (C3), 0.657 / 0.679 / 0.690 / 0.671 / 0.663 (C5x1)  [tools/early_refill_sweep.py]
+// lead (outward-sweep steps) of the single-buffer tile refill
 constexpr int kV5Early = 2;
 struct V5Entry {
   int N, R, D;
@@ -422,6 +420,16 @@ struct FusedInput {
   double* times_out;
 };
 
+// shared memory of an SM that resident CTAs share (H100: 228 KB; every CTA also reserves 1 KB of it)
+constexpr int kSmemPerSm = 228 * 1024;
+
+// dynamic shared memory of the v3 kernel (and its cost-only instantiation): staging tiles, prefetch ring, time
+// history and the sweep state of nmax eliminated vertices (the state block also keeps the vertex position)
+size_t v3_smem_bytes(const WaypointEntry* e, int D, int nmax) {
+  return size_t(4) * e->stage_bytes_per_warp + size_t(2) * (1 + D) * mtg::kTmemThreads * 8 +
+         size_t(nmax + 1) * mtg::kTmemThreads * 8 + size_t(nmax) * (e->slots + D) * mtg::kTmemThreads * sizeof(double);
+}
+
 // K3: the chunked (checkpoint + recompute) twisted kernel -- any K, fixed on-chip footprint.
 int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, const mtg::WaypointParams& prm,
                    double* coeffs, int64_t B, cudaStream_t stream, int slot) {
@@ -434,43 +442,29 @@ int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, 
     if (rc_regs != MTG_OK) return rc_regs;
   }
   const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
-  auto smem_of = [&](int C, int ntm) {
-    return size_t(mtg::kTmemHeaderBytes) + size_t(4) * e->stage_bytes_per_warp +
-           size_t(rd * (1 + D) + (C + 1) + (D + 1) + (1 + 2 * D) + (C - ntm) * kslots) * mtg::kTmemThreads * 8;
+  auto smem_of = [&](int C) {
+    return size_t(4) * e->stage_bytes_per_warp +
+           size_t(rd * (1 + D) + (C + 1) + (D + 1) + (1 + 2 * D) + C * kslots) * mtg::kTmemThreads * 8;
   };
-  int best_ctas = 0, best_C = 0, best_cols = 0, best_ntm = 0;
+  int best_ctas = 0, best_C = 0;
   size_t best_smem = 0;
   const int cmax = std::max(1, std::min(nmax, 24));
-  const int col_options[] = {256, 512, 128, 64, 0};
-  for (int cols : col_options)
-    for (int C = cmax; C >= 1; --C) {
-      if (h->chunk_blocks > 0 && C != std::min(h->chunk_blocks, cmax)) continue;
-      const int ntm = cols ? std::min(C, cols / (2 * kslots)) : 0;
-      const size_t smem = smem_of(C, ntm);
-      if (smem > h->smem_optin) continue;
-      int ctas = std::min<int>(by_regs, int((228 * 1024) / (smem + 1024)));
-      if (cols) ctas = std::min(ctas, 512 / cols);
-      ctas = std::min(ctas, 8);
-      // More resident CTAs first.  Then: when the sweep needs several rounds anyway, the chunk that fits tensor memory
-      // entirely (no shared-memory blocks: 60 KB per CTA instead of 114 KB leaves ~100 KB of L1 for the re-read
-      // inputs and checkpoints -- measured at K = 50: 0.376 of the HBM roofline with C = 4 vs 0.255 with C = 7);
-      // a single round (C >= nmax) always wins over recomputation.
-      const bool single = C >= nmax, best_single = best_C >= nmax && best_C > 0;
-      const bool all_tmem = ntm == C, best_all_tmem = best_ntm == best_C;
-      bool better = ctas > best_ctas;
-      if (ctas == best_ctas && ctas > 0) {
-        if (single != best_single) better = single;
-        else if (!single && all_tmem != best_all_tmem) better = all_tmem;
-        else better = C > best_C;
-      }
-      if (better) {
-        best_ctas = ctas;
-        best_C = C;
-        best_cols = cols;
-        best_ntm = ntm;
-        best_smem = smem;
-      }
+  for (int C = cmax; C >= 1; --C) {
+    if (h->chunk_blocks > 0 && C != std::min(h->chunk_blocks, cmax)) continue;
+    const size_t smem = smem_of(C);
+    if (smem > h->smem_optin) continue;
+    int ctas = std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024)));
+    ctas = std::min(ctas, 8);
+    // More resident CTAs first; then a single round (C >= nmax) wins over recomputation; then the larger chunk.
+    const bool single = C >= nmax, best_single = best_C >= nmax && best_C > 0;
+    bool better = ctas > best_ctas;
+    if (ctas == best_ctas && ctas > 0) better = single != best_single ? single : C > best_C;
+    if (better) {
+      best_ctas = ctas;
+      best_C = C;
+      best_smem = smem;
     }
+  }
   if (best_ctas == 0) {
     h->error = "chunked kernel: no launch configuration fits";
     return MTG_ERR_ALLOC;
@@ -480,8 +474,6 @@ int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, 
   const int nc = nmax > 0 ? (nmax + best_C - 1) / best_C : 1;
   mtg::ChunkedLaunch cl;
   cl.chunk = best_C;
-  cl.n_tmem_blocks = best_ntm;
-  cl.tmem_cols = best_cols;
   cl.ckpt = nullptr;
   mtg_handle::Arena& ar = h->scratch[slot];
   if (nc > 1) {
@@ -583,28 +575,9 @@ int launch_cost_fused(mtg_handle* h, const mtg_problem* p, CachedTopology* topo,
     if (rc_regs != MTG_OK) return rc_regs;
   }
   const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
-  int best_ctas = 0, best_cols = 0, best_ntm = 0;
-  size_t best_smem = 0;
-  const int col_options[] = {512, 256, 128, 64, 32, 0};
-  for (int cols : col_options) {
-    const int tslots = e->slots + e->D;
-    const int ntm = cols ? std::min(nmax, cols / (2 * tslots)) : 0;
-    if (cols && ntm == 0) continue;
-    const size_t smem = mtg::kTmemHeaderBytes + size_t(4) * e->stage_bytes_per_warp +
-                        size_t(2) * (1 + p->D) * mtg::kTmemThreads * 8 + size_t(nmax + 1) * mtg::kTmemThreads * 8 +
-                        size_t(nmax - ntm) * tslots * mtg::kTmemThreads * sizeof(double);
-    if (smem > h->smem_optin) continue;
-    int ctas = std::min<int>(by_regs, int((228 * 1024) / (smem + 1024)));
-    ctas = std::min(ctas, 16);
-    if (cols) ctas = std::min(ctas, 512 / cols);
-    if (ctas > best_ctas || (ctas == best_ctas && smem < best_smem)) {
-      best_ctas = ctas;
-      best_cols = cols;
-      best_ntm = ntm;
-      best_smem = smem;
-    }
-  }
-  if (best_ctas < 2) return MTG_ERR_ALLOC;  // large K: unfused path (chunked kernel + cost kernel)
+  const size_t smem = v3_smem_bytes(e, p->D, nmax);
+  const int ctas = smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024))), 16);
+  if (ctas < 2) return MTG_ERR_ALLOC;  // large K: unfused path (chunked kernel + cost kernel)
   mtg::WaypointParams prm;
   prm.K = p->K;
   prm.n_fixed = L.n_fixed;
@@ -621,16 +594,13 @@ int launch_cost_fused(mtg_handle* h, const mtg_problem* p, CachedTopology* topo,
   prm.mel_k1 = mel_k1;
   prm.mel_inc = inc;
   prm.mel_lower = lower;
-  mtg::TmemLaunch tl;
-  tl.n_tmem_blocks = best_ntm;
-  tl.tmem_cols = best_cols;
   {
-        const int rc_smem = ensure_dyn_smem(h, (const void*)ce->fn, size_t(best_smem));
+        const int rc_smem = ensure_dyn_smem(h, (const void*)ce->fn, smem);
         if (rc_smem != MTG_OK) return rc_smem;
       }
   CUtensorMap tmap;
   std::memset(&tmap, 0, sizeof(tmap));  // unused by the cost-only instantiation
-  ce->fn<<<(unsigned)((nx + 63) / 64), mtg::kTmemThreads, best_smem, stream>>>(prm, tl, tmap);
+  ce->fn<<<(unsigned)((nx + 63) / 64), mtg::kTmemThreads, smem, stream>>>(prm, tmap);
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
   return MTG_OK;
@@ -694,44 +664,38 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
           if (rc_regs != MTG_OK) return rc_regs;
         }
         const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
-        int best_ctas = 0, best_cols = 0, best_nbuf = 0;
+        int best_ctas = 0, best_nbuf = 0;
         size_t best_smem = 0;
-        const int col_options[] = {256, 128, 64, 32, 512};
-        for (int nbuf = 2; nbuf >= 1; --nbuf)
-          for (int cols : col_options) {
-            const int tslots = cols / 2;
-            const int spill = std::max(0, total_state - tslots);
-            const size_t tile_doubles = fused ? size_t(16) * (p->K + 1) * p->D : size_t(16) * (p->K + p->D * L.n_fixed);
-            const size_t smem = mtg::kTmemHeaderBytes + size_t(4) * e->stage_bytes_per_warp + 128 +
-                                size_t(4) * nbuf * tile_doubles * 8 +
-                                size_t(spill + (fused ? nmax + 1 : 0)) * mtg::kTmemThreads * 8;
-            if (smem > h->smem_optin) continue;
-            int ctas = std::min<int>(by_regs, int((228 * 1024) / (smem + 1024)));
-            ctas = std::min(std::min(ctas, 512 / cols), 8);
-            // more resident CTAs first; then double buffering; then less shared memory
-            if (ctas > best_ctas || (ctas == best_ctas && ctas > 0 && (nbuf > best_nbuf || (nbuf == best_nbuf && smem < best_smem)))) {
-              best_ctas = ctas;
-              best_cols = cols;
-              best_nbuf = nbuf;
-              best_smem = smem;
-            }
+        for (int nbuf = 2; nbuf >= 1; --nbuf) {
+          const size_t tile_doubles = fused ? size_t(16) * (p->K + 1) * p->D : size_t(16) * (p->K + p->D * L.n_fixed);
+          const size_t smem = size_t(4) * e->stage_bytes_per_warp + 128 + size_t(4) * nbuf * tile_doubles * 8 +
+                              size_t(total_state + (fused ? nmax + 1 : 0)) * mtg::kTmemThreads * 8;
+          if (smem > h->smem_optin) continue;
+          const int ctas = std::min(std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024))), 8);
+          // more resident CTAs first; then double buffering
+          if (ctas > best_ctas) {
+            best_ctas = ctas;
+            best_nbuf = nbuf;
+            best_smem = smem;
           }
-        const bool take = best_ctas >= 2 && (h->waypoint_variant == 6 || best_nbuf == 2 || h->tma_inputs == 2);
+        }
+        // default routing wants two resident CTAs per SM (otherwise the chunked kernel keeps more warps in flight);
+        // a forced v5 runs whenever one CTA fits
+        const bool take = best_ctas >= (h->waypoint_variant == 6 ? 1 : 2) &&
+                          (h->waypoint_variant == 6 || best_nbuf == 2 || h->tma_inputs == 2);
         if (take) {
           mtg::TmemLaunchV5 tl;
-          tl.tmem_slots = best_cols / 2;
-          tl.tmem_cols = best_cols;
           tl.n_buffers = best_nbuf;
           tl.tile_counter = nullptr;
           V5Kernel launch_fn = fn5;
           if (best_nbuf == 1 && h->early_steps >= 0) {
             // early refill of the single tile buffer (EARLY instantiation): both lanes must own >= E vertices and the
-            // parking area must lie in tensor memory behind the state blocks still needed
+            // parking area must lie inside the sweep state, behind the state blocks still needed
             const int E = kV5Early;
             const int own_min = p->K - (p->K + 1) / 2 - 1;
             const int stash = (p->D + 1) * E + p->D + mm * p->D + 1;
             const V5Kernel fe = fused ? e5->fn_fused_early : e5->fn_early;
-            if (fe != nullptr && E <= own_min && E <= nmax && E * kslots + stash <= best_cols / 2) {
+            if (fe != nullptr && E <= own_min && E <= nmax && E * kslots + stash <= total_state) {
               int regs_e = 0;
               const int rc_regs = kernel_regs(h, (const void*)fe, &regs_e);
               if (rc_regs != MTG_OK) return rc_regs;
@@ -739,9 +703,8 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
             }
           }
           const int64_t blocks = std::min<int64_t>((B + 63) / 64, int64_t(best_ctas) * h->sm_count);
-          // dynamic tile counter for long tiles with several tiles per warp (balances the tail: C3 0.618 vs 0.605,
-          // C5 on one GPU 0.655 vs 0.630); static round-robin for short trajectories, where the atomic's round trip is
-          // not small against a tile (C2 0.581 vs 0.529, C4 0.812 vs 0.797)  [profiles/r02_k1_variants.json]
+          // dynamic tile counter for long tiles with several tiles per warp (balances the tail); static round-robin for
+          // short trajectories, where the atomic's round trip is not small against a tile
           const int64_t tiles_per_warp = (B / 16) / std::max<int64_t>(1, blocks * 4);
           if (h->dynamic_tiles == 1 || (h->dynamic_tiles == 0 && tiles_per_warp >= 8 && p->K > kV4MaxK)) {
             const int rc_ctr = tile_counter_acquire(h, slot, stream, &tl.tile_counter);
@@ -778,32 +741,15 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
           if (rc_regs != MTG_OK) return rc_regs;
         }
         const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
-        int best_ctas = 0, best_cols = 0, best_ntm = 0;
-        size_t best_smem = 0;
-        const int col_options[] = {512, 256, 128, 64, 32, 0};
-        for (int cols : col_options) {
-          const int ntm = cols ? std::min(nmax, cols / (2 * kslots)) : 0;
-          if (cols && ntm == 0 && nmax > 0) continue;
-          const int spill = std::max(0, nmax - ntm) * kslots;
-          const size_t smem = mtg::kTmemHeaderBytes + size_t(4) * e->stage_bytes_per_warp +
-                              size_t(rd * (1 + p->D) + (nmax + 1) + p->D + std::max(spill, kpro)) * mtg::kTmemThreads * 8;
-          if (smem > h->smem_optin) continue;
-          int ctas = std::min<int>(by_regs, int((228 * 1024) / (smem + 1024)));
-          if (cols) ctas = std::min(ctas, 512 / cols);
-          ctas = std::min(ctas, 8);
-          if (ctas > best_ctas || (ctas == best_ctas && smem < best_smem)) {
-            best_ctas = ctas;
-            best_cols = cols;
-            best_ntm = ntm;
-            best_smem = smem;
-          }
-        }
-        if (best_ctas > 0) {
+        const size_t best_smem = size_t(4) * e->stage_bytes_per_warp +
+                                 size_t(rd * (1 + p->D) + (nmax + 1) + p->D + std::max(nmax * kslots, kpro)) *
+                                     mtg::kTmemThreads * 8;
+        int best_ctas =
+            best_smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (best_smem + 1024))), 8);
+        if (best_ctas >= (h->waypoint_variant == 4 ? 1 : 2)) {  // as for v5: a forced v4 runs whenever one CTA fits
           const bool per_tile = h->ctas_per_sm == 9;
           if (h->ctas_per_sm > 0 && !per_tile) best_ctas = std::min(best_ctas, h->ctas_per_sm);
           mtg::TmemLaunchV4 tl;
-          tl.n_tmem_blocks = best_ntm;
-          tl.tmem_cols = best_cols;
           tl.region_slots = 0;
           tl.tile_counter = nullptr;
           // dynamic tile counter when every warp has many tiles to draw (balances the tail); static round-robin for
@@ -839,8 +785,8 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
     if (want_default && (coeffs_aligned || fused)) {
       if (!coeffs_aligned) return MTG_ERR_ALLOC;  // fused entry: caller falls back to pack + solve
       const int nmax = (p->K + 1) / 2 - 1;
-      // ---- launch plan (TMEM column count / spill split maximising resident CTAs per SM): computed and
-      // the function attributes set ONCE per (kernel, K); a B = 1 solveLinear() call pays none of it again.
+      // ---- launch plan (resident CTAs per SM): computed and the function attributes set ONCE per (kernel, K);
+      // a B = 1 solveLinear() call pays none of it again.
       mtg_handle::TmemPlan* plan = nullptr;
       for (auto& pl : h->plans)
         if (pl.entry == (const void*)e && pl.K == p->K) plan = &pl;
@@ -854,34 +800,14 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
         mtg_handle::TmemPlan np;
         np.entry = (const void*)e;
         np.K = p->K;
-        const int col_options[] = {512, 256, 128, 64, 32, 0};
-        for (int cols : col_options) {
-          const int tslots = e->slots + e->D;  // TMEM kernel also keeps the vertex position in the state block
-          const int ntm = cols ? std::min(nmax, cols / (2 * tslots)) : 0;
-          if (cols && ntm == 0) continue;
-          const size_t smem = mtg::kTmemHeaderBytes + size_t(4) * e->stage_bytes_per_warp +
-                              size_t(2) * (1 + p->D) * mtg::kTmemThreads * 8 + size_t(nmax + 1) * mtg::kTmemThreads * 8 +
-                              size_t(nmax - ntm) * tslots * mtg::kTmemThreads * sizeof(double);
-          if (smem > h->smem_optin) continue;
-          int ctas = std::min<int>(by_regs, int((228 * 1024) / (smem + 1024)));
-          ctas = std::min(ctas, 16);
-          if (cols) ctas = std::min(ctas, 512 / cols);
-          if (ctas > np.ctas || (ctas == np.ctas && smem < np.smem)) {
-            np.ctas = ctas;
-            np.cols = cols;
-            np.ntm = ntm;
-            np.smem = smem;
-          }
-        }
+        np.smem = v3_smem_bytes(e, p->D, nmax);
+        np.ctas = np.smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (np.smem + 1024))), 16);
         h->plans.push_back(np);
         plan = &h->plans.back();
       }
       if (plan->ctas < 2 && fused) return MTG_ERR_ALLOC;  // caller falls back to pack + solve
       if (plan->ctas < 2)  // the whole factor does not fit on chip at two CTAs per SM: checkpoint + recompute (K3)
         return launch_chunked(h, p, e, prm, coeffs, B, stream, slot);
-      mtg::TmemLaunch tl;
-      tl.n_tmem_blocks = plan->ntm;
-      tl.tmem_cols = plan->cols;
       const int64_t blocks = (B + 63) / 64;
       auto fn = fused ? e->fn_tmem_fused : e->fn_tmem;
       {
@@ -903,7 +829,7 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
         h->tmap_key.D = p->D;
         h->tmap_key.N = p->N;
       }
-      fn<<<(unsigned)blocks, mtg::kTmemThreads, plan->smem, stream>>>(prm, tl, h->tmap_cached);
+      fn<<<(unsigned)blocks, mtg::kTmemThreads, plan->smem, stream>>>(prm, h->tmap_cached);
     } else if (use_v1) {
       {
         const int rc_smem = ensure_dyn_smem(h, (const void*)e->fn, size_t(smem_v1));
@@ -1017,8 +943,8 @@ int mtg_create(int device, mtg_handle** out) {
     g_create_error = std::string("cudaGetDeviceProperties: ") + cudaGetErrorString(e);
     return MTG_ERR_CUDA;
   }
-  if (prop.major != 10) {
-    g_create_error = "this library contains sm_100a code only; device is sm_" + std::to_string(prop.major) +
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_error = "this library contains sm_90a code only; device is sm_" + std::to_string(prop.major) +
                      std::to_string(prop.minor);
     return MTG_ERR_NO_DEVICE;
   }
@@ -1057,7 +983,7 @@ const char* mtg_last_error(const mtg_handle* h) { return h ? h->error.c_str() : 
 
 int64_t mtg_launch_count(const mtg_handle* h) { return h ? h->launches : 0; }
 
-int mtg_device_is_sm100(const mtg_handle* h) { return h && h->cc_major == 10; }
+int mtg_device_is_sm90(const mtg_handle* h) { return h && h->cc_major == 9; }
 
 int mtg_set_option(mtg_handle* h, int key, int value) {
   if (!h) return MTG_ERR_BAD_ARG;
@@ -1112,7 +1038,7 @@ int mtg_problem_layout(const mtg_problem* p, mtg_layout* out, int32_t* slot_col)
   out->n_all = L.n_all;
   out->n_fixed = L.n_fixed;
   out->n_free = L.n_free;
-  // routing without a device: assume the B200 opt-in shared memory limit (227 KB)
+  // routing without a device: assume the H100 opt-in shared memory limit (227 KB)
   mtg_handle fake;
   fake.smem_optin = 227 * 1024;
   out->kernel = route(&fake, p, L);

@@ -24,13 +24,8 @@
 // The factor (L_v: h(h+1)/2, y_v: h*D doubles per vertex; W_v is recomputed from T_v on the way back) is a LIFO in
 // global memory, [vertex][slot][resident thread] so that every access is coalesced; it is written once and read
 // once (8*(K+1)*(h(h+1)/2 + h*D)*2 bytes per trajectory -- for N = 10, D = 3, K = 16: 8.2 KB next to 4.9 KB of
-// algorithmic traffic), which bounds this kernel at ~0.37 of the HBM roofline.  Dimensions are processed in
+// algorithmic traffic), which bounds this kernel well below the HBM roofline.  Dimensions are processed in
 // groups of DG <= 4 (template), larger D re-runs the sweep per group.
-// Measured and rejected on the bench mask (N = 10, D = 3, K = 16, velocity fixed at every vertex; tools/k1_variants.py):
-// storing only the free part of L_v (15-21 instead of 30 doubles per vertex, runtime prefix-sum slot offsets) 0.173 vs
-// 0.191 of the HBM roofline -- the predicated pushes / pops with computed offsets cost more issue slots than the bytes
-// saved; additionally prefetching the next vertex's slots with cp.async into a double-buffered 61 KB shared-memory
-// window 0.156 (0.089 vs 0.155 at N = 12, where the window drops the kernel to one CTA per SM).
 #pragma once
 
 #include "mtg_generic_kernel.cuh"

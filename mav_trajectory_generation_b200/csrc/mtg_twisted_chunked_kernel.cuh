@@ -2,11 +2,10 @@
 // on-chip footprint (large-K kernel; the reference's own timing program runs K = 50 and K = 100,
 // src/polynomial_timing_evaluation.cpp:114-129, its test-suite K = 50, test/test_polynomial_optimization.cpp:822-828).
 //
-// The headline kernels keep the factor of every eliminated vertex on chip (TMEM + shared memory), which caps
-// them at K <= 34 for N = 10, D = 3 before occupancy collapses (K = 50 ran one warp per SM on the shared-memory
-// kernel: 0.12 of the HBM roofline; K = 100 fell to the generic kernel: 0.009).  Here only a CHUNK of C vertex
-// blocks per lane is ever resident -- the same 7 blocks (5 in tensor memory, 2 in shared memory) that give the
-// headline kernel two CTAs per SM -- and the rest is RECOMPUTED (checkpointing):
+// The resident kernels keep the factor of every eliminated vertex in shared memory, which caps the number of
+// trajectories in flight per SM as K grows (25 doubles per lane and eliminated vertex at N = 10, D = 3).  Here
+// only a CHUNK of C vertex blocks per lane is ever resident -- the host picks C for the most resident CTAs per
+// SM -- and the rest is RECOMPUTED (checkpointing):
 //
 //   round 0   forward sweep over all own vertices 1..n (n = ceil(K/2)-1); only the innermost chunk (n-C, n] is
 //             stored; the loop-carried state (W, y: m*m + m*D doubles) is checkpointed to global memory at the
@@ -19,12 +18,7 @@
 // the inputs -- against 2.2x the algorithmic traffic if the whole factor were spilled to HBM.
 // CTAs are persistent (static tile assignment) so that the checkpoint area is bounded by the number of resident
 // threads, not by the batch.  Arithmetic per vertex is exactly the v3/v4 sequence: results are bitwise equal to
-// the headline kernels where both run (tests force tiny chunks on K = 16 to prove it).
-//
-// Measured and rejected (profiles/r02_k1_variants.json): staging the next round's checkpoint and restart inputs in
-// shared memory with cp.async during the current round's back-substitution (K = 50: 0.352 vs 0.383 of the HBM
-// roofline, K = 100: 0.294 vs 0.337) -- the extra 28 KB of shared memory per CTA shrink the L1 that serves the
-// re-read inputs, which costs more than the exposed checkpoint loads.
+// the resident kernels where both run (tests force tiny chunks on K = 16 to prove it).
 #pragma once
 
 #include "mtg_twisted_tmem_v4_kernel.cuh"
@@ -32,9 +26,7 @@
 namespace mtg {
 
 struct ChunkedLaunch {
-  int chunk;          // C: vertex blocks resident per lane
-  int n_tmem_blocks;  // of which in tensor memory (the rest in shared memory)
-  int tmem_cols;
+  int chunk;          // C: vertex blocks resident per lane (in shared memory)
   double* ckpt;       // [(nc-1)][m*m + m*D][gridDim.x * 128] loop-carried state at chunk starts
 };
 
@@ -42,11 +34,11 @@ template <int N, int D>
 __host__ __device__ constexpr int chunked_ckpt_slots() {
   return (N / 2 - 1) * (N / 2 - 1) + (N / 2 - 1) * D;
 }
-// dynamic shared memory: [holder][staging][ring RD x (1+D)][times C+1][stash D+1][restart 1+2D][smem blocks]
+// dynamic shared memory: [staging][ring RD x (1+D)][times C+1][stash D+1][restart 1+2D][state blocks]
 template <int N, int D, int RD>
-__host__ __device__ constexpr size_t chunked_smem_bytes(int C, int ntm) {
-  return size_t(kTmemHeaderBytes) + size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() +
-         size_t(RD * (1 + D) + (C + 1) + (D + 1) + (1 + 2 * D) + (C - ntm) * v4_state_slots<N, D>()) * kTmemThreads * 8;
+__host__ __device__ constexpr size_t chunked_smem_bytes(int C) {
+  return size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() +
+         size_t(RD * (1 + D) + (C + 1) + (D + 1) + (1 + 2 * D) + C * v4_state_slots<N, D>()) * kTmemThreads * 8;
 }
 
 template <int N, int R, int D, int RD>
@@ -56,7 +48,6 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   constexpr int m = h - 1;
   constexpr int kL = m * (m + 1) / 2;
   constexpr int kSlots = kL + m * D + D;
-  constexpr int kWords = 2 * kSlots;
   constexpr int kCk = chunked_ckpt_slots<N, D>();
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
@@ -74,56 +65,27 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   const int nh = half ? K - M - 1 : M - 1;
   const int n = M - 1;
   const int C = cl.chunk;
-  const int ntm = cl.n_tmem_blocks;
   const int nc = n > 0 ? (n + C - 1) / C : 1;
 
-  uint32_t* holder = reinterpret_cast<uint32_t*>(smem_raw);
-  double2* stage = reinterpret_cast<double2*>(smem_raw + kTmemHeaderBytes) + size_t(warp) * 32 * (D * h);
-  double* base = reinterpret_cast<double*>(smem_raw + kTmemHeaderBytes + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) +
+  double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);
+  double* base = reinterpret_cast<double*>(smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) +
                  threadIdx.x;
   auto PF = [&](int buf, int slot) -> double* { return base + (size_t(buf) * (1 + D) + slot) * kTmemThreads; };
   double* thist = base + size_t(RD) * (1 + D) * kTmemThreads;
   auto HT = [&](int b) -> double& { return thist[size_t(b) * kTmemThreads]; };  // time of the step that made block b
   double* stash = thist + size_t(C + 1) * kTmemThreads;    // x0[D], T0
   double* restart = stash + size_t(D + 1) * kTmemThreads;  // T of own segment lo, x_lo[D], x_{lo+1}[D]
-  double* spill = restart + size_t(1 + 2 * D) * kTmemThreads;
-  auto SP = [&](int blk, int slot) -> double& { return spill[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
+  double* state = restart + size_t(1 + 2 * D) * kTmemThreads;
+  auto SP = [&](int blk, int slot) -> double& { return state[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
   auto RS = [&](int slot) -> double* { return restart + size_t(slot) * kTmemThreads; };
 
-  uint32_t tbase = 0;
-  if (cl.tmem_cols > 0) {
-    if (warp == 0) tmem::alloc(tmem::smem_u32(holder), (uint32_t)cl.tmem_cols);
-    tmem::fence_before_sync();
-    __syncthreads();
-    tmem::fence_after_sync();
-    tbase = *holder + (uint32_t(warp * 32) << 16);
-  }
   auto put_state = [&](int blk, const double (&sv)[kSlots]) {
-    if (blk < ntm) {
 #pragma unroll
-      for (int i = 0; i < kSlots; ++i) {
-        const uint32_t w[2] = {(uint32_t)__double2loint(sv[i]), (uint32_t)__double2hiint(sv[i])};
-        tmem::st<2>(tbase + uint32_t(blk * kWords + 2 * i), w);
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) SP(blk - ntm, i) = sv[i];
-    }
+    for (int i = 0; i < kSlots; ++i) SP(blk, i) = sv[i];
   };
-  // The tensor-memory read is asynchronous until tcgen05.wait::ld: state_issue() starts it, the caller does the
-  // work that does not depend on the state (segment time, its powers, E_v u_{v+1}), state_finish() waits.
-  auto state_issue = [&](int blk, uint32_t (&w)[kWords]) {
-    if (blk < ntm) tmem::ld_words<kWords>(tbase + uint32_t(blk * kWords), w);
-  };
-  auto state_finish = [&](int blk, const uint32_t (&w)[kWords], double (&sv)[kSlots]) {
-    if (blk < ntm) {
-      tmem::wait_ld();
+  auto get_state = [&](int blk, double (&sv)[kSlots]) {
 #pragma unroll
-      for (int i = 0; i < kSlots; ++i) sv[i] = __hiloint2double((int)w[2 * i + 1], (int)w[2 * i]);
-    } else {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk - ntm, i);
-    }
+    for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk, i);
   };
 
   auto seg = [&](int j) -> int { return half ? K - 1 - j : j; };
@@ -431,7 +393,6 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
         }
       }
       __syncwarp();
-      if (ntm > 0) tmem::wait_st();
 
       // ---- middle vertex (round 0 only): both halves meet
       if (j == 0) {
@@ -521,9 +482,7 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
         segment_powers<N, R>(T, iT, pw);
         double sv[kSlots];
         {
-          uint32_t w[kWords];
-          state_issue(v - lo - 1, w);
-          state_finish(v - lo - 1, w, sv);
+          get_state(v - lo - 1, sv);
         }
         double tE[m][D];  // E_v u_{v+1} (after the wait: this kernel runs at the register limit)
 #pragma unroll
@@ -606,11 +565,6 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   }
 
   if (lane == 0) bulk_wait_all();
-  if (cl.tmem_cols > 0) {
-    tmem::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem::dealloc(*holder, (uint32_t)cl.tmem_cols);
-  }
 }
 
 }  // namespace mtg

@@ -10,8 +10,7 @@
 // partner with warp shuffles, both factor the middle block (redundantly, ~3 % extra flops) and
 // then back-substitute their own half outward, emitting the coefficients of their own segments.
 // Versus one thread per trajectory this halves the serial dependency chain and the per-thread
-// sweep state at an identical flop count, which is what the latency-bound C3 shape needs
-// (profiles/: v1 ran 2 warps/SM on K = 16).
+// sweep state at an identical flop count, which is what the latency-bound C3 shape needs.
 //
 // Per-lane sweep state (L_v, inverse pivots, y_v of its M-1 vertices) is in shared memory,
 // [vertex][slot][lane] (bank-conflict free).

@@ -1,13 +1,10 @@
 // mtg_twisted_tmem_kernel.cuh -- K1 (v3): twisted two-lanes-per-trajectory sweep with the
-// per-thread sweep state held in TENSOR MEMORY and coalesced output.
+// per-thread sweep state held in shared memory and coalesced output.
 //
-// Why TMEM: the sweep state (L_v, inverse pivots, y_v per eliminated vertex; 22 doubles per
-// vertex for N=10, D=3) is what bounds the number of trajectories in flight per SM.  Shared
-// memory alone gives 5 warps/SM at K = 16.  Blackwell's 256 KB tensor memory is otherwise idle
-// on this (tensor-core-free) path, and tcgen05.st / tcgen05.ld with the 32x32b shape give every
-// thread of a warp a private, dynamically indexed row of 512 32-bit columns -- exactly a
-// per-thread LIFO.  A 128-thread CTA covers the 128 TMEM lanes; two CTAs per SM take 256 columns
-// each (128 doubles per thread); what does not fit spills to shared memory [vertex][slot][thread].
+// The sweep state (L_v, inverse pivots, y_v and the vertex position per eliminated vertex; 25 doubles
+// per vertex for N=10, D=3) is what bounds the number of trajectories in flight per SM.  It lives in
+// shared memory as [vertex][slot][thread] (consecutive threads hit consecutive banks); the host only
+// routes a K to this kernel when two CTAs fit on an SM, longer trajectories take the chunked kernel.
 //
 // Output: each lane writes the D*N coefficients of the segment it has just solved into its row of a
 // 128-byte aligned per-warp staging tile ([half][16 trajectories][D*N doubles]); one elected lane then hands
@@ -27,127 +24,9 @@
 #include "mtg_twisted_kernel.cuh"
 
 namespace mtg {
-namespace tmem {
-
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-__device__ __forceinline__ void alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 bit, repeated along columns: thread i of the warp owns lane (quarter base + i) and
-// moves NV consecutive 32-bit columns starting at taddr.
-template <int NV>
-__device__ __forceinline__ void st(uint32_t taddr, const uint32_t* v);
-template <int NV>
-__device__ __forceinline__ void ld(uint32_t taddr, uint32_t* v);
-
-template <>
-__device__ __forceinline__ void st<2>(uint32_t a, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(a), "r"(v[0]), "r"(v[1]) : "memory");
-}
-template <>
-__device__ __forceinline__ void st<4>(uint32_t a, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v[0]), "r"(v[1]),
-               "r"(v[2]), "r"(v[3])
-               : "memory");
-}
-template <>
-__device__ __forceinline__ void st<8>(uint32_t a, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(a), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-template <>
-__device__ __forceinline__ void st<16>(uint32_t a, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15, %16};" ::"r"(a),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-template <>
-__device__ __forceinline__ void ld<2>(uint32_t a, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(v[0]), "=r"(v[1]) : "r"(a) : "memory");
-}
-template <>
-__device__ __forceinline__ void ld<4>(uint32_t a, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
-               : "r"(a)
-               : "memory");
-}
-template <>
-__device__ __forceinline__ void ld<8>(uint32_t a, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(a)
-               : "memory");
-}
-template <>
-__device__ __forceinline__ void ld<16>(uint32_t a, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(a)
-      : "memory");
-}
-
-// NW 32-bit words starting at column `col` of this thread's lane, greedy chunks of 16/8/4/2.
-template <int NW, int OFF = 0>
-__device__ __forceinline__ void st_words(uint32_t taddr, const uint32_t* w) {
-  if constexpr (NW - OFF >= 16) {
-    st<16>(taddr + OFF, w + OFF);
-    st_words<NW, OFF + 16>(taddr, w);
-  } else if constexpr (NW - OFF >= 8) {
-    st<8>(taddr + OFF, w + OFF);
-    st_words<NW, OFF + 8>(taddr, w);
-  } else if constexpr (NW - OFF >= 4) {
-    st<4>(taddr + OFF, w + OFF);
-    st_words<NW, OFF + 4>(taddr, w);
-  } else if constexpr (NW - OFF >= 2) {
-    st<2>(taddr + OFF, w + OFF);
-    st_words<NW, OFF + 2>(taddr, w);
-  }
-}
-template <int NW, int OFF = 0>
-__device__ __forceinline__ void ld_words(uint32_t taddr, uint32_t* w) {
-  if constexpr (NW - OFF >= 16) {
-    ld<16>(taddr + OFF, w + OFF);
-    ld_words<NW, OFF + 16>(taddr, w);
-  } else if constexpr (NW - OFF >= 8) {
-    ld<8>(taddr + OFF, w + OFF);
-    ld_words<NW, OFF + 8>(taddr, w);
-  } else if constexpr (NW - OFF >= 4) {
-    ld<4>(taddr + OFF, w + OFF);
-    ld_words<NW, OFF + 4>(taddr, w);
-  } else if constexpr (NW - OFF >= 2) {
-    ld<2>(taddr + OFF, w + OFF);
-    ld_words<NW, OFF + 2>(taddr, w);
-  }
-}
-
-}  // namespace tmem
-
-struct TmemLaunch {
-  int n_tmem_blocks;   // eliminated vertices whose state lives in TMEM (the rest spill to shared memory)
-  int tmem_cols;       // power of two >= 32, 0 = no TMEM used
-};
-
 constexpr int kTmemThreads = 128;
-constexpr int kTmemHeaderBytes = 128;  // TMEM base-address holder, padded so that the staging tiles stay 128-B aligned
 
 template <int N, int D>
 __host__ __device__ constexpr int tmem_stage_bytes_per_warp() {
@@ -160,7 +39,7 @@ __host__ __device__ constexpr int tmem_prefetch_bytes() {
 }
 
 __device__ __forceinline__ void cp_async8(const double* smem_dst, const double* gsrc) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(tmem::smem_u32(smem_dst)), "l"(gsrc) : "memory");
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 // TMA tensor store of a [16 rows][D*N doubles] shared-memory box to coeffs viewed as a 2-D tensor
@@ -169,7 +48,7 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 __device__ __forceinline__ void tma_store_box(const CUtensorMap* tmap, const void* ssrc, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(tmap)),
-               "r"(tmem::smem_u32(ssrc)), "r"(c0), "r"(c1)
+               "r"(smem_u32(ssrc)), "r"(c0), "r"(c1)
                : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -179,14 +58,13 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 
 template <int N, int R, int D, bool FUSED = false, bool COST = false>
 __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
-    twisted_tmem_kernel(const WaypointParams prm, const TmemLaunch tl, const __grid_constant__ CUtensorMap tmap) {
+    twisted_tmem_kernel(const WaypointParams prm, const __grid_constant__ CUtensorMap tmap) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
   constexpr int kL = m * (m + 1) / 2;
   // per eliminated vertex: L (strictly lower) + inverse pivots + y + the vertex position (so that the
   // outward sweep does not re-read it from global memory)
   constexpr int kSlots = kL + m * D + D;
-  constexpr int kWords = 2 * kSlots;
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
   using G = H1Imm<N, R>;     // immediates: this kernel is register-bound (see mtg_device.cuh)
@@ -202,51 +80,28 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
   const int nh = half ? K - M - 1 : M - 1;
   const int nmax = M - 1;
 
-  // ---- shared memory carve-up: [holder 16 B][staging: kWarps tiles][spilled state]
-  uint32_t* holder = reinterpret_cast<uint32_t*>(smem_raw);
-  double2* stage = reinterpret_cast<double2*>(smem_raw + kTmemHeaderBytes) + size_t(warp) * 32 * (D * h);  // [half][16][D*h]
+  // ---- shared memory carve-up: [staging: kWarps tiles][prefetch ring][time history][sweep state]
+  double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);  // [half][16][D*h]
   // per-thread prefetch ring for the next step's inputs (segment time + D positions), filled by
   // cp.async: a register prefetch would share its scoreboard slot with the load being consumed and the
   // consumer would wait for the NEW loads as well (measured: 25 % of all stall samples).
-  double* pf = reinterpret_cast<double*>(smem_raw + kTmemHeaderBytes + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) + threadIdx.x;
+  double* pf = reinterpret_cast<double*>(smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) + threadIdx.x;
   auto PF = [&](int buf, int slot) -> double* { return pf + (size_t(buf) * (1 + D) + slot) * kTmemThreads; };
   // per-thread history of the own-frame segment times seen by the inward sweep (nmax+1 doubles): the
   // outward sweep reads them back from shared memory (in FUSED mode this also saves the sqrt/exp)
-  double* thist = reinterpret_cast<double*>(smem_raw + kTmemHeaderBytes + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>() +
+  double* thist = reinterpret_cast<double*>(smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>() +
                                             tmem_prefetch_bytes<D>()) +
                   threadIdx.x;
   auto HT = [&](int j) -> double& { return thist[size_t(j) * kTmemThreads]; };
-  double* spill = thist + size_t(nmax + 1) * kTmemThreads;
-  auto SP = [&](int blk, int slot) -> double& { return spill[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
-
-  // ---- tensor memory for the sweep state
-  uint32_t tbase = 0;  // assigned after the first global loads have been issued (see below)
-  const int ntm = tl.n_tmem_blocks;
+  double* state = thist + size_t(nmax + 1) * kTmemThreads;
+  auto SP = [&](int blk, int slot) -> double& { return state[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
   auto put_state = [&](int blk, const double (&sv)[kSlots]) {
-    if (blk < ntm) {  // warp-uniform
-      // one tcgen05.st.x2 per double: a double already is an aligned register pair, so no packing
-      // moves are needed (a wide .x16 store wants 16 consecutive registers)
 #pragma unroll
-      for (int i = 0; i < kSlots; ++i) {
-        const uint32_t w[2] = {(uint32_t)__double2loint(sv[i]), (uint32_t)__double2hiint(sv[i])};
-        tmem::st<2>(tbase + uint32_t(blk * kWords + 2 * i), w);
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) SP(blk - ntm, i) = sv[i];
-    }
+    for (int i = 0; i < kSlots; ++i) SP(blk, i) = sv[i];
   };
   auto get_state = [&](int blk, double (&sv)[kSlots]) {
-    if (blk < ntm) {
-      uint32_t w[kWords];
-      tmem::ld_words<kWords>(tbase + uint32_t(blk * kWords), w);
-      tmem::wait_ld();
 #pragma unroll
-      for (int i = 0; i < kSlots; ++i) sv[i] = __hiloint2double((int)w[2 * i + 1], (int)w[2 * i]);
-    } else {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk - ntm, i);
-    }
+    for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk, i);
   };
 
   const long long traj0 = ((long long)blockIdx.x * kWarps + warp) * 16;  // first trajectory of this warp
@@ -294,8 +149,7 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
   };
   double* __restrict__ tout = (FUSED && prm.times_out != nullptr) ? prm.times_out + traj * K : nullptr;
 
-  // ---- issue the first global loads NOW: their latency overlaps the TMEM allocation, the CTA barrier
-  // and the index set-up below (measured: the prologue loads were ~9 % of all stall samples)
+  // ---- issue the first global loads NOW: their latency overlaps the index set-up below
   double T0e = 0.0, x0e[D], x1e[D], u0e[m][D];
   {
     const int e0 = half ? h + K : 1;
@@ -308,15 +162,6 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
     }
     if constexpr (!FUSED) T0e = __ldg(tt + seg(0));
     pf_issue(1, 1, 2);  // inputs of sweep step v = 1 -> ring buffer (v & 1)
-  }
-
-  // ---- tensor memory for the sweep state
-  if (tl.tmem_cols > 0) {
-    if (warp == 0) tmem::alloc(tmem::smem_u32(holder), (uint32_t)tl.tmem_cols);
-    tmem::fence_before_sync();
-    __syncthreads();
-    tmem::fence_after_sync();
-    tbase = *holder + (uint32_t(warp * 32) << 16);  // this warp's lane quarter
   }
 
   // ---- output: each lane writes the D*N doubles of the segment it emits into row (half*16 + trajectory) of
@@ -580,10 +425,9 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
       }
     }
     __syncwarp();
-    put_state(v - 1, sv);  // all lanes (tcgen05.st is warp-collective)
+    put_state(v - 1, sv);
   }
   __syncwarp();
-  if (ntm > 0) tmem::wait_st();
 
   // ---------------------------------------------------------------- middle vertex
   double um[m][D];
@@ -690,7 +534,7 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
 
   for (int v = nmax; v >= 1; --v) {
     double sv[kSlots];
-    get_state(v - 1, sv);  // all lanes
+    get_state(v - 1, sv);
     const bool act = v <= nh;
     double T = 1.0, iT = 1.0;
     double sd[h][D];  // inactive lanes (odd K only) emit garbage rows that are never stored
@@ -794,11 +638,6 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
     if (valid && half == 0 && prm.cost != nullptr) prm.cost[traj] = (cost_acc + other) * (1.0 / G::scale);
   }
   if (lane == 0) bulk_wait_all();  // every TMA store issued by this warp has completed
-  if (tl.tmem_cols > 0) {
-    tmem::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem::dealloc(*holder, (uint32_t)tl.tmem_cols);
-  }
 }
 
 }  // namespace mtg

@@ -1,17 +1,13 @@
-// mtg_twisted_tmem_v4_kernel.cuh -- K1 (v4): the twisted TMEM kernel made PERSISTENT, with every global
-// read issued several sweep steps (or half a tile) before it is consumed.
+// mtg_twisted_tmem_v4_kernel.cuh -- K1 (v4): the twisted shared-memory-state kernel made PERSISTENT, with every
+// global read issued several sweep steps (or half a tile) before it is consumed.
 //
-// What the ncu source page of v3 showed (profiles/r01_tmem_c3.ncu-rep): 22 % of all warp-stall samples are
-// long-scoreboard waits on INPUT data -- the first loads of a tile (4.4 %), the cp.async ring that ran one
-// step ahead (4.3 % + 2.9 %) -- and 4 % are CTA barriers around the per-CTA TMEM allocation.  The kernel's
-// HBM traffic is 83 % writes, and reads queued behind write bursts take 2-3 us, longer than one sweep step.
-// v4 therefore
-//   * runs one CTA per TMEM/shared-memory slot for the whole launch (2 per SM); every WARP loops over its own
-//     16-trajectory tiles (tile = blockIdx.x * 4 + warp, stride gridDim.x * 4): TMEM is allocated once, no CTA
-//     barrier inside the loop;
+// Input reads queue behind the kernel's write bursts (its HBM traffic is mostly coefficient stores), so a read
+// issued one sweep step ahead is often not back in time.  v4 therefore
+//   * runs a grid of resident CTAs for the whole launch; every WARP loops over its own 16-trajectory tiles
+//     (tile = blockIdx.x * 4 + warp, stride gridDim.x * 4), no CTA barrier inside the loop;
 //   * prefetches the NEXT tile's prologue inputs (end vertex, its derivatives, first waypoint, first time)
-//     with cp.async half a tile ahead, into the part of shared memory that holds the spilled sweep state
-//     (dead by then);
+//     with cp.async at the end of the outward sweep, into the part of shared memory that holds the sweep
+//     state (dead by then);
 //   * deepens the per-thread input ring to RD buffers (prefetch distance RD-1 sweep steps, cp.async groups);
 //   * keeps the end vertex position in a 3-double per-thread stash and prefetches the end derivatives for the
 //     final emission at the start of the outward sweep -- no exposed global read at the end of a tile;
@@ -26,9 +22,7 @@
 namespace mtg {
 
 struct TmemLaunchV4 {
-  int n_tmem_blocks;  // eliminated vertices whose state lives in TMEM (the rest spill to shared memory)
-  int tmem_cols;      // power of two >= 32, 0 = no TMEM used
-  int region_slots;   // doubles per thread of the spill / next-tile-prologue region
+  int region_slots;   // doubles per thread of the sweep-state / next-tile-prologue region
   unsigned long long* tile_counter;  // non-null: warps draw their 16-trajectory tiles from this counter (zeroed by
                                      // the host before the launch); null: static round-robin assignment
 };
@@ -44,11 +38,11 @@ __host__ __device__ constexpr int v4_state_slots() {
 }
 // dynamic shared memory of a CTA
 template <int N, int D, int RD>
-__host__ __device__ constexpr size_t v4_smem_bytes(int K, int ntm) {
+__host__ __device__ constexpr size_t v4_smem_bytes(int K) {
   const int nmax = (K + 1) / 2 - 1;
-  const int spill = (nmax - ntm) > 0 ? (nmax - ntm) * v4_state_slots<N, D>() : 0;
-  const int region = spill > v4_pro_slots<N, D>() ? spill : v4_pro_slots<N, D>();
-  return size_t(kTmemHeaderBytes) + size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() +
+  const int state = nmax * v4_state_slots<N, D>();
+  const int region = state > v4_pro_slots<N, D>() ? state : v4_pro_slots<N, D>();
+  return size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() +
          size_t(RD * (1 + D) + (nmax + 1) + D + region) * kTmemThreads * 8;
 }
 
@@ -58,25 +52,18 @@ __device__ __forceinline__ void cp_async_wait_group() {
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 
-template <int N, int R, int D, bool FUSED, int RD, int MINB, int HOIST = 0>
+template <int N, int R, int D, bool FUSED, int RD, int MINB>
 __global__ void __launch_bounds__(kTmemThreads, MINB)
     twisted_tmem_v4_kernel(const WaypointParams prm, const TmemLaunchV4 tl, const __grid_constant__ CUtensorMap tmap) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
   constexpr int kL = m * (m + 1) / 2;
   constexpr int kSlots = kL + m * D + D;
-  constexpr int kWords = 2 * kSlots;
   constexpr int kPro = v4_pro_slots<N, D>();
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
   constexpr double kTiny = 0x1p-600, kHuge = 0x1p+600;
   static_assert(RD >= 2, "ring depth");
-  // work overlapped with the asynchronous tensor-memory read of the outward sweep: 0 = none, 1 = segment time and
-  // its powers, 2 = also E_v u_{v+1} (the fetched words stay live meanwhile: ~50 registers).  Measured on C3
-  // (profiles/r02_k1_variants.json): 0.563 / 0.511 / 0.511 of the HBM roofline for 0 / 1 / 2 -- the extra live
-  // registers cost more than the exposed tcgen05.wait::ld, so 0 is the default.
-  constexpr int kHoist = HOIST;
-  constexpr bool kHoistE = HOIST >= 2;
   using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
 
@@ -89,56 +76,26 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   const int M = (K + 1) >> 1;
   const int nh = half ? K - M - 1 : M - 1;
   const int nmax = M - 1;
-  const int ntm = tl.n_tmem_blocks;
 
-  // ---- shared memory: [holder][staging x kWarps][ring RD x (1+D)][time history nmax+1][x0 stash D][region]
-  uint32_t* holder = reinterpret_cast<uint32_t*>(smem_raw);
-  double2* stage = reinterpret_cast<double2*>(smem_raw + kTmemHeaderBytes) + size_t(warp) * 32 * (D * h);
-  double* base = reinterpret_cast<double*>(smem_raw + kTmemHeaderBytes + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) +
+  // ---- shared memory: [staging x kWarps][ring RD x (1+D)][time history nmax+1][x0 stash D][region]
+  double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);
+  double* base = reinterpret_cast<double*>(smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) +
                  threadIdx.x;
   auto PF = [&](int buf, int slot) -> double* { return base + (size_t(buf) * (1 + D) + slot) * kTmemThreads; };
   double* thist = base + size_t(RD) * (1 + D) * kTmemThreads;
   auto HT = [&](int j) -> double& { return thist[size_t(j) * kTmemThreads]; };
   double* x0s = thist + size_t(nmax + 1) * kTmemThreads;
-  double* region = x0s + size_t(D) * kTmemThreads;  // spilled state blocks; next tile's prologue inputs
+  double* region = x0s + size_t(D) * kTmemThreads;  // sweep state blocks; next tile's prologue inputs
   auto SP = [&](int blk, int slot) -> double& { return region[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
   auto PRO = [&](int slot) -> double* { return region + size_t(slot) * kTmemThreads; };
 
-  // ---- tensor memory, once per CTA
-  uint32_t tbase = 0;
-  if (tl.tmem_cols > 0) {
-    if (warp == 0) tmem::alloc(tmem::smem_u32(holder), (uint32_t)tl.tmem_cols);
-    tmem::fence_before_sync();
-    __syncthreads();
-    tmem::fence_after_sync();
-    tbase = *holder + (uint32_t(warp * 32) << 16);
-  }
   auto put_state = [&](int blk, const double (&sv)[kSlots]) {
-    if (blk < ntm) {
 #pragma unroll
-      for (int i = 0; i < kSlots; ++i) {
-        const uint32_t w[2] = {(uint32_t)__double2loint(sv[i]), (uint32_t)__double2hiint(sv[i])};
-        tmem::st<2>(tbase + uint32_t(blk * kWords + 2 * i), w);
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) SP(blk - ntm, i) = sv[i];
-    }
+    for (int i = 0; i < kSlots; ++i) SP(blk, i) = sv[i];
   };
-  // The tensor-memory read is asynchronous until tcgen05.wait::ld: state_issue() starts it, the caller does the
-  // work that does not depend on the state (segment time, its powers, E_v u_{v+1}), state_finish() waits.
-  auto state_issue = [&](int blk, uint32_t (&w)[kWords]) {
-    if (blk < ntm) tmem::ld_words<kWords>(tbase + uint32_t(blk * kWords), w);
-  };
-  auto state_finish = [&](int blk, const uint32_t (&w)[kWords], double (&sv)[kSlots]) {
-    if (blk < ntm) {
-      tmem::wait_ld();
+  auto get_state = [&](int blk, double (&sv)[kSlots]) {
 #pragma unroll
-      for (int i = 0; i < kSlots; ++i) sv[i] = __hiloint2double((int)w[2 * i + 1], (int)w[2 * i]);
-    } else {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk - ntm, i);
-    }
+    for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk, i);
   };
 
   auto seg = [&](int j) -> int { return half ? K - 1 - j : j; };
@@ -211,9 +168,6 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
 
   double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
   const int nhF = M - 1, nhB = K - M - 1;
-  // outward step at which the next tile's prologue prefetch is issued: the spill blocks (index >= ntm) have all
-  // been read back once step v <= ntm starts
-  const int v_pro = ntm < nmax ? ntm : nmax;
 
   while (wt < n_wtiles) {
     long long wt_next = dyn ? draw_tile() : wt + wt_stride;  // known one tile ahead: its prologue is prefetched
@@ -449,7 +403,6 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       put_state(v - 1, sv);
     }
     __syncwarp();
-    if (ntm > 0) tmem::wait_st();
 
     // ---------------------------------------------------------------- middle vertex
     double um[m][D];
@@ -556,46 +509,38 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         for (int b = 0; b < m; ++b) cp_async8(base + size_t(b * D + d) * kTmemThreads, P.fx + d * nf + e0 + b);
       cp_async_commit();
     }
-    auto maybe_pro = [&](int v) {
-      if (v == v_pro && !next_known) {
+    // the next tile's prologue inputs go to the state region: issued once every state block has been read back
+    auto issue_next_pro = [&]() {
+      if (!next_known) {
         wt_next = __shfl_sync(kFull, wt_next, 0);
         next_known = true;
       }
-      if (v == v_pro && wt_next < n_wtiles) {  // warp-uniform
+      if (wt_next < n_wtiles) {  // warp-uniform
         const Ptrs pn = tile_ptrs(wt_next);
         pro_issue(pn);
         cp_async_commit();
       }
     };
-    if (nmax == 0) maybe_pro(0);  // v_pro == 0
+    if (nmax == 0) issue_next_pro();
 
     for (int v = nmax; v >= 1; --v) {
-      uint32_t w[kWords];
-      if constexpr (kHoist > 0) state_issue(v - 1, w);
       const bool act = v <= nh;
-      // independent of the state being fetched: segment time, its powers, t = E_v u_{v+1}
       const double T = act ? HT(v) : 1.0;
       const double iT = fast_rcp(T);
       double pw[N - 1];
       segment_powers<N, R>(T, iT, pw);
-      double tE[m][D];
-      auto compute_tE = [&]() {
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int a = 0; a < m; ++a) {
-            double s = 0.0;
-#pragma unroll
-            for (int b = 0; b < m; ++b) s = fma(pw[a + b + 2] * G::at(1 + a, h + 1 + b), ed[1 + b][d], s);
-            tE[a][d] = s;
-          }
-      };
-      if constexpr (kHoistE) compute_tE();
-      maybe_pro(v);
       double sv[kSlots];
-      if constexpr (kHoist == 0) state_issue(v - 1, w);
-      state_finish(v - 1, w, sv);
-      if constexpr (!kHoistE) compute_tE();
+      get_state(v - 1, sv);
+      double tE[m][D];
+#pragma unroll
+      for (int d = 0; d < D; ++d)
+#pragma unroll
+        for (int a = 0; a < m; ++a) {
+          double s = 0.0;
+#pragma unroll
+          for (int b = 0; b < m; ++b) s = fma(pw[a + b + 2] * G::at(1 + a, h + 1 + b), ed[1 + b][d], s);
+          tE[a][d] = s;
+        }
       double sd[h][D];
       if (act) {
         double xv[D];
@@ -652,7 +597,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
           for (int k = 0; k < h; ++k) ed[k][d] = sd[k][d];
       }
     }
-    if (nmax > 0 && v_pro == 0) maybe_pro(0);  // no TMEM blocks: the spill region is dead only now
+    if (nmax > 0) issue_next_pro();  // the state region is dead only now
     {
       double sd[h][D];
       if constexpr (kEndInRing) {
@@ -685,11 +630,6 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   }
 
   if (lane == 0) bulk_wait_all();
-  if (tl.tmem_cols > 0) {
-    tmem::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem::dealloc(*holder, (uint32_t)tl.tmem_cols);
-  }
 }
 
 }  // namespace mtg

@@ -1,18 +1,16 @@
-// mtg_twisted_tmem_v5_kernel.cuh -- K1 (v5): the persistent twisted TMEM kernel with its INPUTS MOVED BY THE TMA.
+// mtg_twisted_tmem_v5_kernel.cuh -- K1 (v5): the persistent twisted kernel with its INPUTS MOVED BY THE TMA.
 //
 // The whole input record of a 16-trajectory warp tile -- seg_times[16][K] and d_fixed[16][D][n_fixed], two
 // contiguous spans of global memory -- is brought into shared memory by one elected lane with two cp.async.bulk
 // copies completing on an mbarrier, and every lane then reads its segment times, waypoints and end derivatives
-// from shared memory.  For short trajectories (K <= 8) two tiles fit next to the coefficient staging tile and the
-// NEXT tile is fetched a whole tile ahead; for longer ones (K = 16: 11.6 KB per tile) one tile fits beside the part
-// of the sweep state that overflows tensor memory, and the refill is issued while the last segment of the current
-// tile is emitted.  The waypoints are no longer copied into the sweep state (the tile stays resident), which
-// shrinks the state to 22 doubles per vertex, and the state is split between TMEM and shared memory slot by slot
-// instead of block by block (K = 16: 128 of 154 doubles per lane in TMEM, 26 in shared memory).  Compared with v4 this removes every per-lane global
-// load (LDG / LDGSTS: 16 distinct 128-byte lines per warp instruction), the cp.async ring, the time history, the
-// prologue prefetch region and their address arithmetic; what is left on the LSU are shared-memory accesses and
-// the TMA descriptors.  Requirements (checked by the host, which otherwise launches v4): B a multiple of 16 and
-// 16-byte aligned seg_times / d_fixed, so that every tile is a whole, aligned bulk copy.
+// from shared memory.  For short trajectories two tiles fit next to the coefficient staging tile and the sweep
+// state, and the NEXT tile is fetched a whole tile ahead; for longer ones one tile fits, and the refill is issued
+// while the last segment of the current tile is emitted.  The waypoints are not copied into the sweep state (the
+// tile stays resident), which shrinks the state to 22 doubles per vertex at N = 10, D = 3.  Compared with v4 this
+// removes every per-lane global load, the cp.async ring, the time history, the prologue prefetch region and their
+// address arithmetic; what is left on the LSU are shared-memory accesses and the TMA descriptors.  Requirements
+// (checked by the host, which otherwise launches v4): B a multiple of 16 and 16-byte aligned seg_times / d_fixed,
+// so that every tile is a whole, aligned bulk copy.
 // Arithmetic per trajectory is the v3/v4 sequence: results are bitwise identical.
 #pragma once
 
@@ -21,10 +19,6 @@
 namespace mtg {
 
 struct TmemLaunchV5 {
-  int tmem_slots;   // sweep-state doubles per lane held in tensor memory (= tmem_cols / 2); the state is split at SLOT
-                    // granularity: state double number s (block * 22 + slot at N = 10, D = 3) lives in TMEM when
-                    // s < tmem_slots, in shared memory otherwise
-  int tmem_cols;
   int n_buffers;    // input tiles per warp: 2 = next tile fetched a whole tile ahead (K <= 12 at N = 10, D = 3), 1 = the
                     // state of longer trajectories leaves room for one tile only: refilled during the outward sweep
                     // (EARLY template parameter) or while the last segment is emitted
@@ -37,14 +31,13 @@ __host__ __device__ constexpr int v5_state_slots() {
   constexpr int m = N / 2 - 1;
   return m * (m + 1) / 2 + m * D;
 }
-// dynamic shared memory: [holder 128][staging x 4 warps][mbarriers 128][input tiles: 4 warps x nbuf x 16*(K + D*nf)][spill]
+// dynamic shared memory: [staging x 4 warps][mbarriers 128][input tiles: 4 warps x nbuf x 16*(K + D*nf)][state]
 template <int N, int D>
-__host__ __device__ constexpr size_t v5_smem_bytes(int K, int nf, int tmem_slots, int nbuf) {
+__host__ __device__ constexpr size_t v5_smem_bytes(int K, int nf, int nbuf) {
   const int nmax = (K + 1) / 2 - 1;
   const int total = nmax * v5_state_slots<N, D>();
-  const int spill = total > tmem_slots ? total - tmem_slots : 0;
-  return size_t(kTmemHeaderBytes) + size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() + 128 +
-         size_t(kTmemThreads / 32) * nbuf * 16 * size_t(K + D * nf) * 8 + size_t(spill) * kTmemThreads * 8;
+  return size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() + 128 +
+         size_t(kTmemThreads / 32) * nbuf * 16 * size_t(K + D * nf) * 8 + size_t(total) * kTmemThreads * 8;
 }
 
 namespace bulk {
@@ -76,10 +69,10 @@ __device__ __forceinline__ void copy_g2s(uint32_t dst, const void* src, uint32_t
 }  // namespace bulk
 
 // EARLY = E > 0 (single tile buffer only): when the outward sweep reaches own vertex E, what its last E steps and the
-// closing step still read from the tile ((D+1)*E + D + m*D + 1 doubles per lane) is parked in tensor-memory slots of
-// state blocks that are already popped (blocks >= E), and the tile buffer is refilled with the next tile there and
+// closing step still read from the tile ((D+1)*E + D + m*D + 1 doubles per lane) is parked in the shared-memory slots
+// of state blocks that are already popped (blocks >= E), and the tile buffer is refilled with the next tile there and
 // then: E back-substitution + emission steps of lead for the fetch instead of one.  The host launches this
-// instantiation only when n_buffers == 1, both lanes own >= E vertices, and the parking area lies inside tensor memory.
+// instantiation only when n_buffers == 1, both lanes own >= E vertices, and the parking area lies inside the state.
 template <int N, int D>
 __host__ __device__ constexpr int v5_early_stash_slots(int E) {
   return (D + 1) * E + D + (N / 2 - 1) * D + 1;
@@ -92,7 +85,6 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   constexpr int m = h - 1;
   constexpr int kL = m * (m + 1) / 2;
   constexpr int kSlots = kL + m * D;  // no positions in the state: the input tile stays resident for the whole tile
-  constexpr int kWords = 2 * kSlots;
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
   constexpr double kTiny = 0x1p-600, kHuge = 0x1p+600;
@@ -108,80 +100,28 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   const int M = (K + 1) >> 1;
   const int nh = half ? K - M - 1 : M - 1;
   const int nmax = M - 1;
-  const int tslots = tl.tmem_slots;
   const int nbuf = tl.n_buffers;
 
-  uint32_t* holder = reinterpret_cast<uint32_t*>(smem_raw);
-  double2* stage = reinterpret_cast<double2*>(smem_raw + kTmemHeaderBytes) + size_t(warp) * 32 * (D * h);
-  unsigned char* after_stage = smem_raw + kTmemHeaderBytes + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>();
-  const uint32_t bar0 = tmem::smem_u32(after_stage) + uint32_t(warp) * 16;  // two 8-byte mbarriers per warp
+  double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);
+  unsigned char* after_stage = smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>();
+  const uint32_t bar0 = smem_u32(after_stage) + uint32_t(warp) * 16;  // two 8-byte mbarriers per warp
   // FUSED (SURVEY.md 8f-1): the tile is the waypoint record positions[16][K+1][D]; segment times are computed from it
   // (estimateSegmentTimesNfabian) and kept in a small per-thread history for the outward sweep
   const int tile_t = FUSED ? 0 : 16 * K, tile_f = FUSED ? 16 * (K + 1) * D : 16 * D * nf, tile_doubles = tile_t + tile_f;
   double* tiles = reinterpret_cast<double*>(after_stage + 128) + size_t(warp) * nbuf * tile_doubles;
-  double* spill = reinterpret_cast<double*>(after_stage + 128) + size_t(kWarps) * nbuf * tile_doubles + threadIdx.x;
-  double* thist = nullptr;  // FUSED only: behind the spilled state
-  if constexpr (FUSED) {
-    const int total_state = nmax * kSlots;
-    thist = spill + size_t(total_state > tslots ? total_state - tslots : 0) * kTmemThreads;
-  }
+  // sweep state: state double s (block * kSlots + slot) of this thread at state[s * kTmemThreads]
+  double* state = reinterpret_cast<double*>(after_stage + 128) + size_t(kWarps) * nbuf * tile_doubles + threadIdx.x;
+  double* thist = nullptr;  // FUSED only: behind the sweep state
+  if constexpr (FUSED) thist = state + size_t(nmax) * kSlots * kTmemThreads;
   auto TH = [&](int j) -> double& { return thist[size_t(j) * kTmemThreads]; };
-  auto SPG = [&](int s_global) -> double& { return spill[size_t(s_global - tslots) * kTmemThreads]; };
-
-  uint32_t tbase = 0;
-  if (tl.tmem_cols > 0) {
-    if (warp == 0) tmem::alloc(tmem::smem_u32(holder), (uint32_t)tl.tmem_cols);
-    tmem::fence_before_sync();
-    __syncthreads();
-    tmem::fence_after_sync();
-    tbase = *holder + (uint32_t(warp * 32) << 16);
-  }
-  // State block `blk` occupies state doubles [blk*kSlots, (blk+1)*kSlots): entirely in TMEM, entirely in shared
-  // memory, or -- for the one block that straddles tmem_slots -- split slot by slot (all tests are warp-uniform).
+  auto ST = [&](int s_global) -> double& { return state[size_t(s_global) * kTmemThreads]; };
   auto put_state = [&](int blk, const double (&sv)[kSlots]) {
-    const int s0 = blk * kSlots;
-    if (s0 + kSlots <= tslots) {
 #pragma unroll
-      for (int i = 0; i < kSlots; ++i) {
-        const uint32_t w[2] = {(uint32_t)__double2loint(sv[i]), (uint32_t)__double2hiint(sv[i])};
-        tmem::st<2>(tbase + uint32_t(2 * (s0 + i)), w);
-      }
-    } else if (s0 >= tslots) {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) SPG(s0 + i) = sv[i];
-    } else {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) {
-        if (s0 + i < tslots) {
-          const uint32_t w[2] = {(uint32_t)__double2loint(sv[i]), (uint32_t)__double2hiint(sv[i])};
-          tmem::st<2>(tbase + uint32_t(2 * (s0 + i)), w);
-        } else {
-          SPG(s0 + i) = sv[i];
-        }
-      }
-    }
+    for (int i = 0; i < kSlots; ++i) ST(blk * kSlots + i) = sv[i];
   };
   auto get_state = [&](int blk, double (&sv)[kSlots]) {
-    const int s0 = blk * kSlots;
-    if (s0 + kSlots <= tslots) {
-      uint32_t w[kWords];
-      tmem::ld_words<kWords>(tbase + uint32_t(2 * s0), w);
-      tmem::wait_ld();
 #pragma unroll
-      for (int i = 0; i < kSlots; ++i) sv[i] = __hiloint2double((int)w[2 * i + 1], (int)w[2 * i]);
-    } else if (s0 >= tslots) {
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i) sv[i] = SPG(s0 + i);
-    } else {
-      uint32_t w[kWords];
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i)
-        if (s0 + i < tslots) tmem::ld<2>(tbase + uint32_t(2 * (s0 + i)), &w[2 * i]);
-      tmem::wait_ld();
-#pragma unroll
-      for (int i = 0; i < kSlots; ++i)
-        sv[i] = (s0 + i < tslots) ? __hiloint2double((int)w[2 * i + 1], (int)w[2 * i]) : SPG(s0 + i);
-    }
+    for (int i = 0; i < kSlots; ++i) sv[i] = ST(blk * kSlots + i);
   };
 
   auto seg = [&](int j) -> int { return half ? K - 1 - j : j; };
@@ -221,10 +161,10 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       double* dst = tiles + size_t(buf) * tile_doubles;
       bulk::mbar_expect_tx(bar, uint32_t(tile_doubles) * 8u);
       if constexpr (FUSED) {
-        bulk::copy_g2s(tmem::smem_u32(dst), prm.positions + w * 16 * (long long)(K + 1) * D, uint32_t(tile_f) * 8u, bar);
+        bulk::copy_g2s(smem_u32(dst), prm.positions + w * 16 * (long long)(K + 1) * D, uint32_t(tile_f) * 8u, bar);
       } else {
-        bulk::copy_g2s(tmem::smem_u32(dst), prm.times + w * 16 * K, uint32_t(tile_t) * 8u, bar);
-        bulk::copy_g2s(tmem::smem_u32(dst + tile_t), prm.dfix + w * 16 * (long long)D * nf, uint32_t(tile_f) * 8u, bar);
+        bulk::copy_g2s(smem_u32(dst), prm.times + w * 16 * K, uint32_t(tile_t) * 8u, bar);
+        bulk::copy_g2s(smem_u32(dst + tile_t), prm.dfix + w * 16 * (long long)D * nf, uint32_t(tile_f) * 8u, bar);
       }
     }
   };
@@ -475,7 +415,6 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       put_state(v - 1, sv);
     }
     __syncwarp();
-    if (tslots > 0) tmem::wait_st();
 
     // ---------------------------------------------------------------- middle vertex
     double um[m][D];
@@ -573,10 +512,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     if (half == 0) store_free(nh + 1, ed);
 
     constexpr int kStash0 = EARLY * kSlots;  // state slots of the blocks >= EARLY: popped when the sweep reaches vertex EARLY
-    auto park = [&](int slot, double val) {
-      const uint32_t w[2] = {(uint32_t)__double2loint(val), (uint32_t)__double2hiint(val)};
-      tmem::st<2>(tbase + uint32_t(2 * (kStash0 + slot)), w);
-    };
+    auto park = [&](int slot, double val) { ST(kStash0 + slot) = val; };
     for (int v = nmax; v >= 1; --v) {
       if constexpr (EARLY > 0) {
         if (v == EARLY) {
@@ -594,7 +530,6 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
 #pragma unroll
             for (int b = 0; b < m; ++b) park(EARLY * (D + 1) + D + d * m + b, in_u0(b, d));
           park(EARLY * (D + 1) + D + m * D, in_T(0));
-          tmem::wait_st();
           fence_proxy_async();
           __syncwarp();
           if (wt_next < n_wtiles) fetch_tile(wt_next, 0);
@@ -608,12 +543,10 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       if (act) {
         double xv[D];
         if (EARLY > 0 && v <= EARLY) {
-          uint32_t w[2 * (D + 1)];
-          tmem::ld_words<2 * (D + 1)>(tbase + uint32_t(2 * (kStash0 + (EARLY - v) * (D + 1))), w);
-          tmem::wait_ld();
+          const int s0 = kStash0 + (EARLY - v) * (D + 1);
 #pragma unroll
-          for (int d = 0; d < D; ++d) xv[d] = __hiloint2double((int)w[2 * d + 1], (int)w[2 * d]);
-          T = __hiloint2double((int)w[2 * D + 1], (int)w[2 * D]);
+          for (int d = 0; d < D; ++d) xv[d] = ST(s0 + d);
+          T = ST(s0 + D);
         } else {
 #pragma unroll
           for (int d = 0; d < D; ++d) xv[d] = in_x(v, d);
@@ -687,18 +620,14 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       double sd[h][D];
       double T;
       if constexpr (EARLY > 0) {
-        constexpr int kClose = D + m * D + 1;
-        uint32_t w[2 * kClose];
-        tmem::ld_words<2 * kClose>(tbase + uint32_t(2 * (kStash0 + EARLY * (D + 1))), w);
-        tmem::wait_ld();
+        const int s0 = kStash0 + EARLY * (D + 1);
 #pragma unroll
         for (int d = 0; d < D; ++d) {
-          sd[0][d] = __hiloint2double((int)w[2 * d + 1], (int)w[2 * d]);
+          sd[0][d] = ST(s0 + d);
 #pragma unroll
-          for (int b = 0; b < m; ++b)
-            sd[1 + b][d] = __hiloint2double((int)w[2 * (D + d * m + b) + 1], (int)w[2 * (D + d * m + b)]);
+          for (int b = 0; b < m; ++b) sd[1 + b][d] = ST(s0 + D + d * m + b);
         }
-        T = __hiloint2double((int)w[2 * (kClose - 1) + 1], (int)w[2 * (kClose - 1)]);
+        T = ST(s0 + D + m * D);
       } else {
 #pragma unroll
         for (int d = 0; d < D; ++d) {
@@ -726,11 +655,6 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   }
 
   if (lane == 0) bulk_wait_all();
-  if (tl.tmem_cols > 0) {
-    tmem::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem::dealloc(*holder, (uint32_t)tl.tmem_cols);
-  }
 }
 
 }  // namespace mtg

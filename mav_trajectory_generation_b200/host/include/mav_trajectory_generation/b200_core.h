@@ -1,6 +1,6 @@
 // b200_core.h -- non-template implementation behind PolynomialOptimization<N> and
 // BatchPolynomialOptimization<N>: packs Vertex constraints into the flat buffers of the C-ABI
-// (include/mtg_b200.h), calls the sm_100a kernels, unpacks Segment::Vector.
+// (include/mtg_b200.h), calls the sm_90a kernels, unpacks Segment::Vector.
 // There is no host solve in here -- only index bookkeeping and the small debug matrices the
 // reference exposes (getA/getAInverse/getM/getR), which are built from the same exact tables
 // the kernels use.
@@ -21,7 +21,7 @@ namespace mav_trajectory_generation {
 namespace b200 {
 
 // Process-wide handle (device from env MTG_B200_DEVICE, default 0), created on first use.
-// Aborts with a clear message when no sm_100 device / library is available: the GPU path is
+// Aborts with a clear message when no sm_90 device / library is available: the GPU path is
 // the only path.
 mtg_handle* defaultHandle();
 // Serialises callers of the shared handle (a handle is single-caller, include/mtg_b200.h).

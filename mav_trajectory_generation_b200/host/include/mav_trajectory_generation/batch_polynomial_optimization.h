@@ -1,5 +1,5 @@
 // batch_polynomial_optimization.h -- B independent problems of ONE constraint topology solved in a
-// single pass of the B200 kernels.  This is the throughput entry point: the reference solves one
+// single pass of the H100 kernels.  This is the throughput entry point: the reference solves one
 // trajectory per PolynomialOptimization<N> object (its benchmark loops over objects,
 // src/polynomial_timing_evaluation.cpp:93-112); here the loop is the GPU grid.
 // Buffers are pinned host memory; solveLinear() pipelines H2D / kernels / D2H.

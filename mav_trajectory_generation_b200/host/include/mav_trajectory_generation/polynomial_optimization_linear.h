@@ -1,6 +1,6 @@
 // polynomial_optimization_linear.h -- PolynomialOptimization<N> with the reference's public
 // surface (include/mav_trajectory_generation/polynomial_optimization_linear.h:45-284), backed by
-// the B200 kernels.  Behaviour kept from the reference:
+// the H100 kernels.  Behaviour kept from the reference:
 //   * value semantics: inputs are copied in, results copied out to caller-owned objects;
 //   * argument errors CHECK-abort (impl/...linear_impl.h:60,76,289,297,502-504);
 //   * setupFromVertices()/solveLinear() return true (:108,:348,:378);
@@ -182,7 +182,7 @@ class PolynomialOptimization {
     stream << "Mapping matrix:\n" << M << std::endl;
   }
 
-  // B200 extension: status bits of the last solveLinear() (0 = solved; see MTG_STATUS_*).
+  // Extension: status bits of the last solveLinear() (0 = solved; see MTG_STATUS_*).
   int getLastStatus() const { return core_.last_status_; }
 
  private:

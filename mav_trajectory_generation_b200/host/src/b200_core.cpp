@@ -51,7 +51,7 @@ mtg_handle* defaultHandle() {
     const int rc = mtg_create(device, &g_handle);
     if (rc != MTG_OK)
       LOG(FATAL) << "mtg_create(device " << device << ") failed (rc=" << rc << "): " << mtg_last_error(nullptr)
-                 << " -- the B200 CUDA path is the only solver path; there is no CPU fallback.";
+                 << " -- the H100 CUDA path is the only solver path; there is no CPU fallback.";
   }
   return g_handle;
 }

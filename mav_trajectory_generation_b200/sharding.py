@@ -111,7 +111,7 @@ def solve_scattered(solve_fn, times_root, dfix_root, total, K, D, N, n_fixed, de
 
 # ---- fused solve + gather over NVLink peer memory (no collective, no intermediate buffers) --------------------------
 #
-# The B200-first form of "gather the solved coefficients": every rank maps the ROOT's output tensor into its own
+# The peer-memory form of "gather the solved coefficients": every rank maps the ROOT's output tensor into its own
 # address space (CUDA IPC) and hands the solver a slice of it as the coefficient buffer -- the kernels' TMA tensor
 # stores then travel over NVLink / NVSwitch straight into their final place in the root's HBM while the sweep of
 # the following tiles continues.  The transfer overlaps the math tile by tile inside ONE kernel; there is no gather

@@ -4,7 +4,7 @@
 // and bench.py's cpu_baseline / --impl reference legs may load this library.  The
 // product path (mav_trajectory_generation_b200/, include/) never links or calls it.
 //
-// What it restates (all paths under /root/reference/mav_trajectory_generation/):
+// What it restates (paths under mav_trajectory_generation/ of the reference repository):
 //   include/mav_trajectory_generation/impl/polynomial_optimization_linear_impl.h
 //     :56-109   setupFromVertices      -> Problem::setup
 //     :111-121  setupMappingMatrix     -> setup_mapping_matrix
@@ -21,8 +21,8 @@
 //   src/vertex.cpp:27-82    createRandomVertices  (std::mt19937 + uniform_real_distribution)
 //   src/vertex.cpp:255-272  estimateSegmentTimesNfabian
 //
-// The reference's arithmetic lives partly in Eigen (eigen_catkin, version unpinned, NOT
-// present in /root/reference nor in this image): fixed-size .inverse() (PartialPivLU for
+// The reference's arithmetic lives partly in Eigen (eigen_catkin, version unpinned, not
+// vendored by the reference): fixed-size .inverse() (PartialPivLU for
 // 5x5), dense products, and Eigen::SparseQR<COLAMDOrdering>.  Those calls are restated with
 // their published algorithms: partial-pivot LU inverse; row-times-column products evaluated
 // left to right ((Ai^T Q) Ai); a Householder QR solve of the full (non-symmetrised) R_pp

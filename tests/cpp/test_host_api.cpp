@@ -1,6 +1,6 @@
 // test_host_api.cpp -- the reference's own gtest cases for the linear path
 // (mav_trajectory_generation/test/test_polynomial_optimization.cpp), re-stated against the
-// B200-backed PolynomialOptimization<N>.  `--cpu-only` runs the cases that need no device
+// H100-backed PolynomialOptimization<N>.  `--cpu-only` runs the cases that need no device
 // (value types, fixtures, static helpers, layout); without it every solve goes through the GPU.
 #include <cmath>
 #include <cstdio>

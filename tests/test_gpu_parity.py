@@ -32,8 +32,7 @@ def check_parity(out, ref, exact, label, baseline=False):
           the excursion is the reference-order rounding, shown by (1) holding at the same time).
 
     For the BASELINE shapes additionally the distribution is pinned: median <= 1e-13, 99th percentile <= 2e-12
-    against exact (profiles/r02_parity.json: C3 1.8e-14 / 3.4e-13, max 1.5e-11 on a trajectory with a 0.82 s
-    segment between 10 s segments, where the oracle is at 6.2e-11).
+    against exact.
     Returns the three per-trajectory error arrays."""
     e_ge = global_rel_err(out, exact)
     e_go = global_rel_err(out, ref)
@@ -88,7 +87,7 @@ def test_baseline_configs_8192_fixtures_vs_exact_and_oracle(solver, oracle, name
           f"oracle-exact max {e_oe.max():.2e}")
 
 
-@pytest.mark.parametrize("variant", [1, 2, 3, 4, 6])  # 1: thread/trajectory, 2: twisted, 3: + TMEM state, 4: persistent, 6: + TMA inputs
+@pytest.mark.parametrize("variant", [1, 2, 3, 4, 6])  # 1: thread/trajectory, 2: twisted, 3: + shared-memory state and TMA stores, 4: persistent, 6: + TMA inputs
 @pytest.mark.parametrize("N,r,K,D,B", [
     (10, 4, 16, 3, 4096),   # C3 headline shape, >= 4096 bit-exact fixture trajectories (SURVEY.md 8d)
     (10, 4, 8, 3, 2048),    # C2
@@ -183,7 +182,7 @@ def test_tma_input_kernel_bitwise_vs_resident(solver, oracle, N, r, K, D, B):
     equal to the persistent kernel v4 on the same inputs (identical arithmetic, only the input path differs) --
     many tiles per warp (buffer reuse, mbarrier phase flips), a single tile, odd K, dynamic and static tile
     assignment, NON-ZERO end derivatives; K <= 8 double-buffered tiles, K >= 10 a single tile buffer refilled
-    during the last emission with the sweep state split between TMEM and shared memory inside a block; d_free and
+    during the last emission; d_free and
     status outputs included.  Against the per-tile kernel v3 the
     results agree to rounding only: v4/v5 add the end-derivative carry of the first sweep step last instead of
     first (the 2^+-600 folding)."""
