@@ -81,7 +81,6 @@ struct mtg_handle {
     int K = 0;
     int ctas = 0;
     size_t smem = 0;
-    bool attr_plain = false, attr_fused = false;
   };
   std::vector<TmemPlan> plans;
   // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of the FUNCTION (shared by every K routed to it):
@@ -174,30 +173,30 @@ void compute_layout(int N, int K, const std::vector<uint8_t>& mask, Layout* L) {
 }
 
 // ---- waypoint kernel registry ---------------------------------------------------------
+// depth of the cp.async input ring of the v4 and chunked instantiations (their layouts depend on it)
+constexpr int kRingDepth = 3;
 typedef void (*WaypointKernel)(const mtg::WaypointParams);
 struct WaypointEntry {
   int N, R, D, slots;
   WaypointKernel fn;          // one thread per trajectory
   WaypointKernel fn_twisted;  // two lanes per trajectory (twisted factorisation)
   void (*fn_tmem)(const mtg::WaypointParams, const CUtensorMap);  // + shared-memory state, TMA stores
-  int stage_bytes_per_warp;
   void (*fn_tmem_fused)(const mtg::WaypointParams, const CUtensorMap);  // + fused Nfabian
+  size_t (*tmem_smem)(int K);  // dynamic shared memory of fn_tmem / fn_tmem_fused (mtg::V3Layout)
   void (*fn_chunked)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap);  // any K (K3)
+  size_t (*chunked_smem)(int C);  // dynamic shared memory of fn_chunked with C resident blocks (mtg::ChunkedLayout)
+  int chunked_ckpt_slots;         // doubles per thread of one global checkpoint of fn_chunked
 };
-#define MTG_WP(N_, R_, D_)                                                                   \
-  {                                                                                          \
-    N_, R_, D_, mtg::waypoint_state_slots<N_, D_>(), mtg::waypoint_solve_kernel<N_, R_, D_>, \
-        mtg::twisted_solve_kernel<N_, R_, D_>, mtg::twisted_tmem_kernel<N_, R_, D_>,         \
-        mtg::tmem_stage_bytes_per_warp<N_, D_>(), mtg::twisted_tmem_kernel<N_, R_, D_, true>, \
-        mtg::twisted_chunked_kernel<N_, R_, D_, 3>                                           \
+#define MTG_WP_(N_, R_, D_, V1_)                                                                                  \
+  {                                                                                                               \
+    N_, R_, D_, mtg::sweep_state_slots<N_, D_>(), V1_, mtg::twisted_solve_kernel<N_, R_, D_>,                     \
+        mtg::twisted_tmem_kernel<N_, R_, D_>, mtg::twisted_tmem_kernel<N_, R_, D_, true>,                         \
+        mtg::V3Layout<N_, D_>::bytes, mtg::twisted_chunked_kernel<N_, R_, D_, kRingDepth>,                        \
+        mtg::ChunkedLayout<N_, D_, kRingDepth>::bytes, mtg::ChunkedLayout<N_, D_, kRingDepth>::kCkpt              \
   }
+#define MTG_WP(N_, R_, D_) MTG_WP_(N_, R_, D_, (mtg::waypoint_solve_kernel<N_, R_, D_>))
 // v1 (thread per trajectory) is kept for the headline shapes only (cross-check / profiles)
-#define MTG_WP2(N_, R_, D_)                                                                           \
-  {                                                                                                   \
-    N_, R_, D_, mtg::waypoint_state_slots<N_, D_>(), nullptr, mtg::twisted_solve_kernel<N_, R_, D_>,  \
-        mtg::twisted_tmem_kernel<N_, R_, D_>, mtg::tmem_stage_bytes_per_warp<N_, D_>(),               \
-        mtg::twisted_tmem_kernel<N_, R_, D_, true>, mtg::twisted_chunked_kernel<N_, R_, D_, 3>        \
-  }
+#define MTG_WP2(N_, R_, D_) MTG_WP_(N_, R_, D_, nullptr)
 const WaypointEntry kWaypointKernels[] = {
     MTG_WP(10, 4, 3),  MTG_WP(10, 4, 1),  MTG_WP2(10, 4, 2), MTG_WP2(10, 4, 4),   // min snap, N = 10
     MTG_WP(10, 3, 3),  MTG_WP2(10, 3, 1), MTG_WP(10, 2, 3),  MTG_WP2(10, 2, 1),   // jerk / acceleration on N = 10
@@ -211,8 +210,9 @@ typedef void (*TmemKernel)(const mtg::WaypointParams, const CUtensorMap);
 struct CostEntry {
   int N, R, D;
   TmemKernel fn;
+  size_t (*smem)(int K);
 };
-#define MTG_COST(N_, R_, D_) {N_, R_, D_, mtg::twisted_tmem_kernel<N_, R_, D_, false, true>}
+#define MTG_COST(N_, R_, D_) {N_, R_, D_, mtg::twisted_tmem_kernel<N_, R_, D_, false, true>, mtg::V3Layout<N_, D_>::bytes}
 const CostEntry kCostKernels[] = {MTG_COST(10, 4, 3), MTG_COST(10, 4, 1), MTG_COST(10, 4, 4), MTG_COST(10, 3, 3),
                                   MTG_COST(10, 2, 3), MTG_COST(8, 3, 3),  MTG_COST(12, 5, 3)};
 const CostEntry* find_cost(const mtg_problem* p) {
@@ -227,11 +227,13 @@ typedef void (*V4Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV4, con
 struct V4Entry {
   int N, R, D;
   V4Kernel fn, fn_fused;
+  size_t (*smem)(int K);
 };
 #define MTG_V4(N_, R_, D_, MB_)                                                                    \
   {                                                                                                \
-    N_, R_, D_, mtg::twisted_tmem_v4_kernel<N_, R_, D_, false, 3, MB_>,                           \
-        mtg::twisted_tmem_v4_kernel<N_, R_, D_, true, 3, MB_>                                      \
+    N_, R_, D_, mtg::twisted_tmem_v4_kernel<N_, R_, D_, false, kRingDepth, MB_>,                  \
+        mtg::twisted_tmem_v4_kernel<N_, R_, D_, true, kRingDepth, MB_>,                            \
+        mtg::V4Layout<N_, D_, kRingDepth>::bytes                                                   \
   }
 const V4Entry kV4Kernels[] = {MTG_V4(10, 4, 3, 2), MTG_V4(8, 3, 3, 3), MTG_V4(10, 4, 1, 2), MTG_V4(10, 3, 3, 2),
                               MTG_V4(10, 2, 3, 2), MTG_V4(12, 5, 3, 2)};
@@ -245,10 +247,14 @@ struct V5Entry {
   int N, R, D;
   V5Kernel fn, fn_fused;
   V5Kernel fn_early, fn_fused_early;  // the EARLY = kV5Early instantiations
+  size_t (*smem)(int K, int nf, int nbuf), (*smem_fused)(int K, int nf, int nbuf);
+  bool (*early_fits)(int K);  // the EARLY instantiations may run for this K
 };
 #define MTG_V5(N_, R_, D_, MB_)                                                                                       \
   {N_, R_, D_, mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, false>, mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, true>, \
-   mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, false, kV5Early>, mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, true, kV5Early>}
+   mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, false, kV5Early>, mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, true, kV5Early>, \
+   mtg::V5Layout<N_, D_, false>::bytes, mtg::V5Layout<N_, D_, true>::bytes,                                          \
+   mtg::V5Layout<N_, D_, false>::early_fits<kV5Early>}
 const V5Entry kV5Kernels[] = {MTG_V5(10, 4, 3, 2), MTG_V5(8, 3, 3, 3),  MTG_V5(10, 4, 1, 2),
                               MTG_V5(10, 3, 3, 2), MTG_V5(10, 2, 3, 2), MTG_V5(12, 5, 3, 2)};
 const V5Entry* find_v5(const mtg_problem* p) {
@@ -423,38 +429,30 @@ struct FusedInput {
 // shared memory of an SM that resident CTAs share (H100: 228 KB; every CTA also reserves 1 KB of it)
 constexpr int kSmemPerSm = 228 * 1024;
 
-// dynamic shared memory of the v3 kernel (and its cost-only instantiation): staging tiles, prefetch ring, time
-// history and the sweep state of nmax eliminated vertices (the state block also keeps the vertex position)
-size_t v3_smem_bytes(const WaypointEntry* e, int D, int nmax) {
-  return size_t(4) * e->stage_bytes_per_warp + size_t(2) * (1 + D) * mtg::kTmemThreads * 8 +
-         size_t(nmax + 1) * mtg::kTmemThreads * 8 + size_t(nmax) * (e->slots + D) * mtg::kTmemThreads * sizeof(double);
+// Resident CTAs per SM of a kTmemThreads-thread kernel with `smem` bytes of dynamic shared memory: limited by its
+// registers, by shared memory and by `cap`; 0 when `smem` exceeds the per-block opt-in limit.
+int resident_ctas(mtg_handle* h, const void* fn, size_t smem, int cap, int* ctas) {
+  int n_regs = 0;
+  const int rc = kernel_regs(h, fn, &n_regs);
+  if (rc != MTG_OK) return rc;
+  const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
+  *ctas = smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024))), cap);
+  return MTG_OK;
 }
 
 // K3: the chunked (checkpoint + recompute) twisted kernel -- any K, fixed on-chip footprint.
 int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, const mtg::WaypointParams& prm,
                    double* coeffs, int64_t B, cudaStream_t stream, int slot) {
-  const int hh = p->N / 2, mm = hh - 1, D = p->D, rd = 3;
-  const int kslots = mm * (mm + 1) / 2 + mm * D + D, kck = mm * mm + mm * D;
   const int nmax = (p->K + 1) / 2 - 1;
-  int n_regs = 0;
-  {
-    const int rc_regs = kernel_regs(h, (const void*)e->fn_chunked, &n_regs);
-    if (rc_regs != MTG_OK) return rc_regs;
-  }
-  const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
-  auto smem_of = [&](int C) {
-    return size_t(4) * e->stage_bytes_per_warp +
-           size_t(rd * (1 + D) + (C + 1) + (D + 1) + (1 + 2 * D) + C * kslots) * mtg::kTmemThreads * 8;
-  };
   int best_ctas = 0, best_C = 0;
   size_t best_smem = 0;
   const int cmax = std::max(1, std::min(nmax, 24));
   for (int C = cmax; C >= 1; --C) {
     if (h->chunk_blocks > 0 && C != std::min(h->chunk_blocks, cmax)) continue;
-    const size_t smem = smem_of(C);
-    if (smem > h->smem_optin) continue;
-    int ctas = std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024)));
-    ctas = std::min(ctas, 8);
+    const size_t smem = e->chunked_smem(C);
+    int ctas = 0;
+    const int rc_ctas = resident_ctas(h, (const void*)e->fn_chunked, smem, 8, &ctas);
+    if (rc_ctas != MTG_OK) return rc_ctas;
     // More resident CTAs first; then a single round (C >= nmax) wins over recomputation; then the larger chunk.
     const bool single = C >= nmax, best_single = best_C >= nmax && best_C > 0;
     bool better = ctas > best_ctas;
@@ -477,7 +475,7 @@ int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, 
   cl.ckpt = nullptr;
   mtg_handle::Arena& ar = h->scratch[slot];
   if (nc > 1) {
-    const size_t bytes = size_t(nc - 1) * kck * size_t(blocks) * mtg::kTmemThreads * sizeof(double);
+    const size_t bytes = size_t(nc - 1) * e->chunked_ckpt_slots * size_t(blocks) * mtg::kTmemThreads * sizeof(double);
     const int rc = arena_acquire(h, ar, bytes, stream);
     if (rc != MTG_OK) return rc;
     cl.ckpt = ar.p;
@@ -568,15 +566,12 @@ int launch_cost_fused(mtg_handle* h, const mtg_problem* p, CachedTopology* topo,
   const CostEntry* ce = find_cost(p);
   const WaypointEntry* e = L.waypoint ? find_waypoint(h, p, L) : nullptr;
   if (!ce || !e || L.n_free == 0) return MTG_ERR_ALLOC;
-  const int nmax = (p->K + 1) / 2 - 1;
-  int n_regs = 0;
+  const size_t smem = ce->smem(p->K);
+  int ctas = 0;
   {
-    const int rc_regs = kernel_regs(h, (const void*)ce->fn, &n_regs);
-    if (rc_regs != MTG_OK) return rc_regs;
+    const int rc_ctas = resident_ctas(h, (const void*)ce->fn, smem, 16, &ctas);
+    if (rc_ctas != MTG_OK) return rc_ctas;
   }
-  const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
-  const size_t smem = v3_smem_bytes(e, p->D, nmax);
-  const int ctas = smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024))), 16);
   if (ctas < 2) return MTG_ERR_ALLOC;  // large K: unfused path (chunked kernel + cost kernel)
   mtg::WaypointParams prm;
   prm.K = p->K;
@@ -654,24 +649,13 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
       const V5Entry* e5 = find_v5(p);
       if (e5) {
         const V5Kernel fn5 = fused ? e5->fn_fused : e5->fn;
-        const int hh = p->N / 2, mm = hh - 1;
-        const int kslots = mm * (mm + 1) / 2 + mm * p->D;  // no positions in the v5 state
-        const int nmax = (p->K + 1) / 2 - 1;
-        const int total_state = nmax * kslots;
-        int n_regs = 0;
-        {
-          const int rc_regs = kernel_regs(h, (const void*)fn5, &n_regs);
-          if (rc_regs != MTG_OK) return rc_regs;
-        }
-        const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
         int best_ctas = 0, best_nbuf = 0;
         size_t best_smem = 0;
         for (int nbuf = 2; nbuf >= 1; --nbuf) {
-          const size_t tile_doubles = fused ? size_t(16) * (p->K + 1) * p->D : size_t(16) * (p->K + p->D * L.n_fixed);
-          const size_t smem = size_t(4) * e->stage_bytes_per_warp + 128 + size_t(4) * nbuf * tile_doubles * 8 +
-                              size_t(total_state + (fused ? nmax + 1 : 0)) * mtg::kTmemThreads * 8;
-          if (smem > h->smem_optin) continue;
-          const int ctas = std::min(std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024))), 8);
+          const size_t smem = (fused ? e5->smem_fused : e5->smem)(p->K, L.n_fixed, nbuf);
+          int ctas = 0;
+          const int rc_ctas = resident_ctas(h, (const void*)fn5, smem, 8, &ctas);
+          if (rc_ctas != MTG_OK) return rc_ctas;
           // more resident CTAs first; then double buffering
           if (ctas > best_ctas) {
             best_ctas = ctas;
@@ -691,11 +675,8 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
           if (best_nbuf == 1 && h->early_steps >= 0) {
             // early refill of the single tile buffer (EARLY instantiation): both lanes must own >= E vertices and the
             // parking area must lie inside the sweep state, behind the state blocks still needed
-            const int E = kV5Early;
-            const int own_min = p->K - (p->K + 1) / 2 - 1;
-            const int stash = (p->D + 1) * E + p->D + mm * p->D + 1;
             const V5Kernel fe = fused ? e5->fn_fused_early : e5->fn_early;
-            if (fe != nullptr && E <= own_min && E <= nmax && E * kslots + stash <= total_state) {
+            if (fe != nullptr && e5->early_fits(p->K)) {
               int regs_e = 0;
               const int rc_regs = kernel_regs(h, (const void*)fe, &regs_e);
               if (rc_regs != MTG_OK) return rc_regs;
@@ -731,26 +712,16 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
       const V4Entry* e4 = find_v4(p);
       if (e4) {
         V4Kernel fn = fused ? e4->fn_fused : e4->fn;
-        const int rd = 3;
-        const int hh = p->N / 2, mm = hh - 1;
-        const int kslots = mm * (mm + 1) / 2 + mm * p->D + p->D, kpro = 2 * p->D + mm * p->D + 1;
-        const int nmax = (p->K + 1) / 2 - 1;
-        int n_regs = 0;
+        const size_t best_smem = e4->smem(p->K);
+        int best_ctas = 0;
         {
-          const int rc_regs = kernel_regs(h, (const void*)fn, &n_regs);
-          if (rc_regs != MTG_OK) return rc_regs;
+          const int rc_ctas = resident_ctas(h, (const void*)fn, best_smem, 8, &best_ctas);
+          if (rc_ctas != MTG_OK) return rc_ctas;
         }
-        const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
-        const size_t best_smem = size_t(4) * e->stage_bytes_per_warp +
-                                 size_t(rd * (1 + p->D) + (nmax + 1) + p->D + std::max(nmax * kslots, kpro)) *
-                                     mtg::kTmemThreads * 8;
-        int best_ctas =
-            best_smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (best_smem + 1024))), 8);
         if (best_ctas >= (h->waypoint_variant == 4 ? 1 : 2)) {  // as for v5: a forced v4 runs whenever one CTA fits
           const bool per_tile = h->ctas_per_sm == 9;
           if (h->ctas_per_sm > 0 && !per_tile) best_ctas = std::min(best_ctas, h->ctas_per_sm);
           mtg::TmemLaunchV4 tl;
-          tl.region_slots = 0;
           tl.tile_counter = nullptr;
           // dynamic tile counter when every warp has many tiles to draw (balances the tail); static round-robin for
           // small batches, where the first draw's round trip to L2 is not amortised (measured: C2 static, C4 dynamic)
@@ -784,24 +755,18 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
                               (h->waypoint_variant == 2 && !twisted_fits) || (h->waypoint_variant == 1 && !use_v1 && !twisted_fits);
     if (want_default && (coeffs_aligned || fused)) {
       if (!coeffs_aligned) return MTG_ERR_ALLOC;  // fused entry: caller falls back to pack + solve
-      const int nmax = (p->K + 1) / 2 - 1;
       // ---- launch plan (resident CTAs per SM): computed and the function attributes set ONCE per (kernel, K);
       // a B = 1 solveLinear() call pays none of it again.
       mtg_handle::TmemPlan* plan = nullptr;
       for (auto& pl : h->plans)
         if (pl.entry == (const void*)e && pl.K == p->K) plan = &pl;
       if (!plan) {
-        int n_regs = 0;
-        {
-          const int rc_regs = kernel_regs(h, (const void*)e->fn_tmem, &n_regs);
-          if (rc_regs != MTG_OK) return rc_regs;
-        }
-        const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
         mtg_handle::TmemPlan np;
         np.entry = (const void*)e;
         np.K = p->K;
-        np.smem = v3_smem_bytes(e, p->D, nmax);
-        np.ctas = np.smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (np.smem + 1024))), 16);
+        np.smem = e->tmem_smem(p->K);
+        const int rc_ctas = resident_ctas(h, (const void*)e->fn_tmem, np.smem, 16, &np.ctas);
+        if (rc_ctas != MTG_OK) return rc_ctas;
         h->plans.push_back(np);
         plan = &h->plans.back();
       }

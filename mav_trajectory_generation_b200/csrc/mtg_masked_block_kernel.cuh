@@ -319,40 +319,13 @@ __global__ void __launch_bounds__(128, 2)
         // ---- emit segment v: start z_v, end z_{v+1}   (A(1)^-1 in Hermite form, as the waypoint kernels)
         const double iT = 1.0 / T;
         double tp[h], itp[h];
-        tp[0] = 1.0;
-#pragma unroll
-        for (int k = 1; k < h; ++k) tp[k] = tp[k - 1] * T;
-        itp[0] = pow_int<h>(iT);
-#pragma unroll
-        for (int k = 1; k < h; ++k) itp[k] = itp[k - 1] * iT;
+        sweep::Hermite<N, AI>::powers(T, iT, false, tp, itp);
         if (lane == 0) bulk_wait_read();
         __syncwarp();
 #pragma unroll
         for (int d = 0; d < DG; ++d) {
-          double c[N], ss[h], se[h], ee[h];
-#pragma unroll
-          for (int k = 0; k < h; ++k) {
-            c[k] = z[k][d] * AI::at(k, k);
-            ss[k] = tp[k] * z[k][d];
-            se[k] = tp[k] * zn[k][d];
-          }
-#pragma unroll
-          for (int k = 0; k < h; ++k) {
-            double acc = se[k] - ss[k];
-#pragma unroll
-            for (int j2 = k + 1; j2 < h; ++j2) {
-              constexpr double kInvFact[6] = {1.0, 1.0, 0.5, 1.0 / 6.0, 1.0 / 24.0, 1.0 / 120.0};
-              acc = (j2 - k == 1) ? acc - ss[j2] : fma(-kInvFact[j2 - k], ss[j2], acc);
-            }
-            ee[k] = acc;
-          }
-#pragma unroll
-          for (int q = 0; q < h; ++q) {
-            double acc = AI::at(h + q, h) * ee[0];
-#pragma unroll
-            for (int k = 1; k < h; ++k) acc = fma(AI::at(h + q, h + k), ee[k], acc);
-            c[h + q] = acc * itp[q];
-          }
+          double c[N];
+          sweep::Hermite<N, AI>::template coeffs<DG>(false, tp, itp, z, zn, d, c);
 #pragma unroll
           for (int q = 0; q < h; ++q) my_row[d * h + q] = make_double2(c[2 * q], c[2 * q + 1]);
         }

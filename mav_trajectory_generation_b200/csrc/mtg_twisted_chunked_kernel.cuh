@@ -30,30 +30,36 @@ struct ChunkedLaunch {
   double* ckpt;       // [(nc-1)][m*m + m*D][gridDim.x * 128] loop-carried state at chunk starts
 };
 
-template <int N, int D>
-__host__ __device__ constexpr int chunked_ckpt_slots() {
-  return (N / 2 - 1) * (N / 2 - 1) + (N / 2 - 1) * D;
-}
-// dynamic shared memory: [staging][ring RD x (1+D)][times C+1][stash D+1][restart 1+2D][state blocks]
+// Dynamic shared memory of K3 behind the staging tiles, in per-thread slots:
+// [input ring RD x (1+D)][times C+1][stash D+1][restart 1+2D][state: C blocks with the vertex position]
 template <int N, int D, int RD>
-__host__ __device__ constexpr size_t chunked_smem_bytes(int C) {
-  return size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() +
-         size_t(RD * (1 + D) + (C + 1) + (D + 1) + (1 + 2 * D) + C * v4_state_slots<N, D>()) * kTmemThreads * 8;
-}
+struct ChunkedLayout {
+  static constexpr int kSlots = sweep_state_slots<N, D, true>();
+  static constexpr int kCkpt = (N / 2 - 1) * (N / 2 - 1) + (N / 2 - 1) * D;  // global checkpoint: W, y
+  static constexpr int kHist = RD * (1 + D);      // ring, then the times of the chunk
+  static constexpr int kStash = D + 1;             // x0[D], T0
+  static constexpr int kRestart = 1 + 2 * D;       // T of own segment lo, x_lo[D], x_{lo+1}[D]
+  __host__ __device__ static constexpr int hist_slots(int C) { return C + 1; }
+  __host__ __device__ static constexpr size_t stash(int C) { return size_t(kHist) + hist_slots(C); }
+  __host__ __device__ static constexpr size_t restart(int C) { return stash(C) + kStash; }
+  __host__ __device__ static constexpr size_t state(int C) { return restart(C) + kRestart; }
+  __host__ __device__ static constexpr size_t bytes(int C) {
+    return tmem_stage_bytes<N, D>() + tmem_slot_bytes(state(C) + size_t(C) * kSlots);
+  }
+};
 
 template <int N, int R, int D, int RD>
 __global__ void __launch_bounds__(kTmemThreads, 2)
     twisted_chunked_kernel(const WaypointParams prm, const ChunkedLaunch cl, const __grid_constant__ CUtensorMap tmap) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
-  constexpr int kL = m * (m + 1) / 2;
-  constexpr int kSlots = kL + m * D + D;
-  constexpr int kCk = chunked_ckpt_slots<N, D>();
-  constexpr unsigned kFull = 0xffffffffu;
+  using Lay = ChunkedLayout<N, D, RD>;
+  constexpr int kSlots = Lay::kSlots;
+  constexpr int kCk = Lay::kCkpt;
   constexpr int kWarps = kTmemThreads / 32;
-  constexpr double kTiny = 0x1p-600, kHuge = 0x1p+600;
   using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
+  using S = sweep::Sweep<N, D, G>;
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -68,33 +74,18 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   const int nc = n > 0 ? (n + C - 1) / C : 1;
 
   double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);
-  double* base = reinterpret_cast<double*>(smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) +
-                 threadIdx.x;
+  double* base = reinterpret_cast<double*>(smem_raw + tmem_stage_bytes<N, D>()) + threadIdx.x;
   auto PF = [&](int buf, int slot) -> double* { return base + (size_t(buf) * (1 + D) + slot) * kTmemThreads; };
-  double* thist = base + size_t(RD) * (1 + D) * kTmemThreads;
+  double* thist = base + size_t(Lay::kHist) * kTmemThreads;
   auto HT = [&](int b) -> double& { return thist[size_t(b) * kTmemThreads]; };  // time of the step that made block b
-  double* stash = thist + size_t(C + 1) * kTmemThreads;    // x0[D], T0
-  double* restart = stash + size_t(D + 1) * kTmemThreads;  // T of own segment lo, x_lo[D], x_{lo+1}[D]
-  double* state = restart + size_t(1 + 2 * D) * kTmemThreads;
+  double* stash = thist + size_t(Lay::hist_slots(C)) * kTmemThreads;  // x0[D], T0
+  double* restart = stash + size_t(Lay::kStash) * kTmemThreads;       // T of own segment lo, x_lo[D], x_{lo+1}[D]
+  double* state = restart + size_t(Lay::kRestart) * kTmemThreads;
   auto SP = [&](int blk, int slot) -> double& { return state[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
   auto RS = [&](int slot) -> double* { return restart + size_t(slot) * kTmemThreads; };
 
-  auto put_state = [&](int blk, const double (&sv)[kSlots]) {
-#pragma unroll
-    for (int i = 0; i < kSlots; ++i) SP(blk, i) = sv[i];
-  };
-  auto get_state = [&](int blk, double (&sv)[kSlots]) {
-#pragma unroll
-    for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk, i);
-  };
-
-  auto seg = [&](int j) -> int { return half ? K - 1 - j : j; };
-  auto pidx = [&](int v) -> int {
-    const int o = half ? K - v : v;
-    return o == 0 ? 0 : (o < K ? h + o - 1 : h + K - 1);
-  };
-  auto sgn = [&](int idx) -> double { return (half && !(idx & 1)) ? -1.0 : 1.0; };
-  const int e0 = half ? h + K : 1;
+  const sweep::Frame<N> fr{K, half};
+  const int e0 = fr.e0();
 
   const long long n_wtiles = (prm.B + 15) >> 4;
   const long long wt_stride = (long long)gridDim.x * kWarps;
@@ -104,6 +95,7 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
 
   double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
   const int nhF = M - 1, nhB = K - M - 1;
+  const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB};
 
   for (long long wt = (long long)blockIdx.x * kWarps + warp; wt < n_wtiles; wt += wt_stride) {
     long long traj = wt * 16 + (lane >> 1);
@@ -112,80 +104,24 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
     if (!valid) traj = prm.B - 1;
     const double* __restrict__ tt = prm.times + traj * K;
     const double* __restrict__ fx = prm.dfix + traj * (long long)D * nf;
-    auto xaddr = [&](int v, int d) -> const double* { return fx + d * nf + pidx(v); };
+    auto xaddr = [&](int v, int d) -> const double* { return fx + d * nf + fr.pidx(v); };
     auto ring_issue = [&](int v) {
       const int j = v < K ? v : K - 1;
       const int vn = v + 1 <= K ? v + 1 : K;
       const int buf = v % RD;
-      cp_async8(PF(buf, 0), tt + seg(j));
+      cp_async8(PF(buf, 0), tt + fr.seg(j));
 #pragma unroll
       for (int d = 0; d < D; ++d) cp_async8(PF(buf, 1 + d), xaddr(vn, d));
     };
     // restart inputs of a chunk that starts after own step lo
     auto restart_issue = [&](int lo) {
-      cp_async8(RS(0), tt + seg(lo));
+      cp_async8(RS(0), tt + fr.seg(lo));
 #pragma unroll
       for (int d = 0; d < D; ++d) {
         cp_async8(RS(1 + d), xaddr(lo, d));
         cp_async8(RS(1 + D + d), xaddr(lo + 1, d));
       }
     };
-
-    // emit own-frame segment j for every lane of the warp at once (convergent)
-    auto emit_all = [&](int j, int v_step, double T, double iT, const double (&sd)[h][D], const double (&ed)[h][D]) {
-      double tp[h], itp[h];
-      const double Ts = half ? -T : T;
-      tp[0] = 1.0;
-#pragma unroll
-      for (int k = 1; k < h; ++k) tp[k] = tp[k - 1] * Ts;
-      itp[0] = pow_int<h>(iT);
-#pragma unroll
-      for (int k = 1; k < h; ++k) itp[k] = itp[k - 1] * iT;
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double c[N], ss[h], se[h];
-#pragma unroll
-        for (int k = 0; k < h; ++k) {
-          const double s0 = half ? ed[k][d] : sd[k][d];
-          const double e0v = half ? sd[k][d] : ed[k][d];
-          c[k] = s0 * ((half && (k & 1)) ? -AI::at(k, k) : AI::at(k, k));
-          ss[k] = tp[k] * s0;
-          se[k] = tp[k] * e0v;
-        }
-        double ee[h];
-#pragma unroll
-        for (int k = 0; k < h; ++k) {
-          double acc = se[k] - ss[k];
-#pragma unroll
-          for (int j2 = k + 1; j2 < h; ++j2) {
-            constexpr double kInvFact[6] = {1.0, 1.0, 0.5, 1.0 / 6.0, 1.0 / 24.0, 1.0 / 120.0};
-            acc = (j2 - k == 1) ? acc - ss[j2] : fma(-kInvFact[j2 - k], ss[j2], acc);
-          }
-          ee[k] = acc;
-        }
-#pragma unroll
-        for (int q = 0; q < h; ++q) {
-          double acc = AI::at(h + q, h) * ee[0];
-#pragma unroll
-          for (int k = 1; k < h; ++k) acc = fma(AI::at(h + q, h + k), ee[k], acc);
-          c[h + q] = acc * itp[q];
-        }
-        if (d == 0) {  // the TMA must have finished reading the previous segment's tile
-          if (lane == 0) bulk_wait_read();
-          __syncwarp();
-        }
-#pragma unroll
-        for (int q = 0; q < h; ++q) my_row[d * h + q] = make_double2(c[2 * q], c[2 * q + 1]);
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        if (v_step <= nhF) tma_store_box(&tmap, stage, j * (D * N), (int)traj0);
-        if (v_step <= nhB) tma_store_box(&tmap, stage + 16 * (D * h), (K - 1 - j) * (D * N), (int)traj0);
-        bulk_commit();
-      }
-    };
-
 
     int stat = 0;
     double Wp[m][m], yp[m][D], Cee[m][m], cps[m], cpe[m], xm[D], xc[D];
@@ -194,11 +130,11 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
     double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + traj * (long long)D * np : nullptr;
     auto store_free = [&](int v_own, const double (&u)[h][D]) {
       if (df != nullptr && valid) {
-        const int vo = half ? K - v_own : v_own;
+        const int vo = fr.vert(v_own);
 #pragma unroll
         for (int d = 0; d < D; ++d)
 #pragma unroll
-          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = sgn(j) * u[1 + j][d];
+          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
       }
     };
 
@@ -236,34 +172,12 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
         const double iTp = fast_rcp(Tp);
         double pw[N - 1];
         segment_powers<N, R>(Tp, iTp, pw);
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-#pragma unroll
-          for (int b = 0; b < m; ++b) Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-          cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-          cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
-        }
+        S::end_blocks(pw, Cee, cps, cpe);
         if (j == 0) {  // prologue of the tile: initial carry from the fixed end derivatives (exact 2^+-600 scaling)
 #pragma unroll
           for (int d = 0; d < D; ++d) stash[size_t(d) * kTmemThreads] = xm[d];
           stash[size_t(D) * kTmemThreads] = Tp;
-#pragma unroll
-          for (int a = 0; a < m; ++a)
-#pragma unroll
-            for (int b = 0; b < m; ++b) Wp[a][b] = (a == b) ? kTiny : 0.0;
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-            double u0[m];
-#pragma unroll
-            for (int b = 0; b < m; ++b) u0[b] = sgn(b) * __ldg(fx + d * nf + e0 + b);
-#pragma unroll
-            for (int a = 0; a < m; ++a) {
-              double acc = 0.0;
-#pragma unroll
-              for (int b = 0; b < m; ++b) acc = fma(pw[a + b + 2] * G::at(h + 1 + a, 1 + b), u0[b], acc);
-              yp[a][d] = acc * kHuge;
-            }
-          }
+          S::carry_fold(pw, [&](int b, int d) { return fr.sgn(b) * __ldg(fx + d * nf + e0 + b); }, Wp, yp);
         }
       }
 
@@ -299,88 +213,11 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
           double pw[N - 1];
           segment_powers<N, R>(T, iT, pw);
 
-          double Dp[m][m], E[m][m], bb[m][D];
-#pragma unroll
-          for (int a = 0; a < m; ++a) {
-#pragma unroll
-            for (int b = 0; b <= a; ++b) {
-              double s = fma(pw[a + b + 2], G::at(1 + a, 1 + b), Cee[a][b]);
-#pragma unroll
-              for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-              Dp[a][b] = s;
-            }
-#pragma unroll
-            for (int b = 0; b < m; ++b) E[a][b] = pw[a + b + 2] * G::at(1 + a, h + 1 + b);
-            const double gmid = fma(pw[a + 1], G::at(1 + a, 0), cpe[a]);
-            const double gnext = pw[a + 1] * G::at(1 + a, h);
-#pragma unroll
-            for (int d = 0; d < D; ++d) {
-              double s = -cps[a] * xm[d];
-              s = fma(-gmid, xc[d], s);
-              s = fma(-gnext, xn[d], s);
-#pragma unroll
-              for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-              bb[a][d] = s;
-            }
-          }
-          double L[m][m], inv[m];
-#pragma unroll
-          for (int jj = 0; jj < m; ++jj) {
-            double s = Dp[jj][jj];
-#pragma unroll
-            for (int k = 0; k < jj; ++k) s = fma(-L[jj][k], L[jj][k], s);
-            if (!(s > 0.0)) stat |= kStatusNotSpd;
-            inv[jj] = fast_rsqrt(s);
-#pragma unroll
-            for (int i = jj + 1; i < m; ++i) {
-              double t = Dp[i][jj];
-#pragma unroll
-              for (int k = 0; k < jj; ++k) t = fma(-L[i][k], L[jj][k], t);
-              L[i][jj] = t * inv[jj];
-            }
-          }
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-#pragma unroll
-            for (int jj = 0; jj < m; ++jj) {
-              double s = bb[jj][d];
-#pragma unroll
-              for (int k = 0; k < jj; ++k) s = fma(-L[jj][k], yp[k][d], s);
-              yp[jj][d] = s * inv[jj];
-            }
-          }
-#pragma unroll
-          for (int c = 0; c < m; ++c) {
-#pragma unroll
-            for (int jj = 0; jj < m; ++jj) {
-              double s = E[jj][c];
-#pragma unroll
-              for (int k = 0; k < jj; ++k) s = fma(-L[jj][k], Wp[k][c], s);
-              Wp[jj][c] = s * inv[jj];
-            }
-          }
-          {
-            int slot = 0;
-#pragma unroll
-            for (int i = 1; i < m; ++i)
-#pragma unroll
-              for (int jj = 0; jj < i; ++jj) sv[slot++] = L[i][jj];
-#pragma unroll
-            for (int jj = 0; jj < m; ++jj) sv[slot++] = inv[jj];
-#pragma unroll
-            for (int jj = 0; jj < m; ++jj)
-#pragma unroll
-              for (int d = 0; d < D; ++d) sv[slot++] = yp[jj][d];
-#pragma unroll
-            for (int d = 0; d < D; ++d) sv[slot++] = xc[d];
-          }
-#pragma unroll
-          for (int a = 0; a < m; ++a) {
-#pragma unroll
-            for (int b = 0; b <= a; ++b) Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-            cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-            cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
-          }
+          double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
+          S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
+          S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
+          S::pack(L, inv, yp, xc, sv);
+          S::end_blocks(pw, Cee, cps, cpe);
 #pragma unroll
           for (int d = 0; d < D; ++d) {
             xm[d] = xc[d];
@@ -389,7 +226,8 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
         }
         if (store) {  // warp-uniform
           __syncwarp();
-          put_state(v - lo - 1, sv);
+#pragma unroll
+          for (int i = 0; i < kSlots; ++i) SP(v - lo - 1, i) = sv[i];
         }
       }
       __syncwarp();
@@ -397,73 +235,7 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
       // ---- middle vertex (round 0 only): both halves meet
       if (j == 0) {
         double um[m][D];
-        double Dl[m][m], bl[m][D];
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-#pragma unroll
-          for (int b = 0; b <= a; ++b) {
-            double s = Cee[a][b];
-#pragma unroll
-            for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-            Dl[a][b] = s;
-          }
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-            double s = -cps[a] * xm[d];
-            s = fma(-cpe[a], xc[d], s);
-#pragma unroll
-            for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-            bl[a][d] = s;
-          }
-        }
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-#pragma unroll
-          for (int b = 0; b <= a; ++b) {
-            const double o = __shfl_xor_sync(kFull, Dl[a][b], 1);
-            Dl[a][b] += ((a + b) & 1) ? -o : o;
-          }
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-            const double o = __shfl_xor_sync(kFull, bl[a][d], 1);
-            bl[a][d] += (a & 1) ? o : -o;
-          }
-        }
-        stat |= __shfl_xor_sync(kFull, stat, 1);
-        double L[m][m], inv[m];
-#pragma unroll
-        for (int jj = 0; jj < m; ++jj) {
-          double s = Dl[jj][jj];
-#pragma unroll
-          for (int k = 0; k < jj; ++k) s = fma(-L[jj][k], L[jj][k], s);
-          if (!(s > 0.0)) stat |= kStatusNotSpd;
-          inv[jj] = fast_rsqrt(s);
-#pragma unroll
-          for (int i = jj + 1; i < m; ++i) {
-            double t = Dl[i][jj];
-#pragma unroll
-            for (int k = 0; k < jj; ++k) t = fma(-L[i][k], L[jj][k], t);
-            L[i][jj] = t * inv[jj];
-          }
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          double y[m];
-#pragma unroll
-          for (int jj = 0; jj < m; ++jj) {
-            double s = bl[jj][d];
-#pragma unroll
-            for (int k = 0; k < jj; ++k) s = fma(-L[jj][k], y[k], s);
-            y[jj] = s * inv[jj];
-          }
-#pragma unroll
-          for (int jj = m - 1; jj >= 0; --jj) {
-            double s = y[jj];
-#pragma unroll
-            for (int k = jj + 1; k < m; ++k) s = fma(-L[k][jj], um[k][d], s);
-            um[jj][d] = s * inv[jj];
-          }
-        }
+        S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
 #pragma unroll
         for (int d = 0; d < D; ++d) {
           ed[0][d] = xc[d];
@@ -481,65 +253,20 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
         double pw[N - 1];
         segment_powers<N, R>(T, iT, pw);
         double sv[kSlots];
-        {
-          get_state(v - lo - 1, sv);
-        }
+#pragma unroll
+        for (int i = 0; i < kSlots; ++i) sv[i] = SP(v - lo - 1, i);
         double tE[m][D];  // E_v u_{v+1} (after the wait: this kernel runs at the register limit)
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int a = 0; a < m; ++a) {
-            double s = 0.0;
-#pragma unroll
-            for (int b = 0; b < m; ++b) s = fma(pw[a + b + 2] * G::at(1 + a, h + 1 + b), ed[1 + b][d], s);
-            tE[a][d] = s;
-          }
+        S::couple(pw, ed, tE);
         double sd[h][D];
         if (act) {
           double xv[D];
 #pragma unroll
-          for (int d = 0; d < D; ++d) xv[d] = sv[kL + m * D + d];
-          double L[m][m], inv[m], rhs[m][D];
-          {
-            int slot = 0;
-#pragma unroll
-            for (int i = 1; i < m; ++i)
-#pragma unroll
-              for (int jj = 0; jj < i; ++jj) L[i][jj] = sv[slot++];
-#pragma unroll
-            for (int jj = 0; jj < m; ++jj) inv[jj] = sv[slot++];
-#pragma unroll
-            for (int jj = 0; jj < m; ++jj)
-#pragma unroll
-              for (int d = 0; d < D; ++d) rhs[jj][d] = sv[slot++];
-          }
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-            double t[m];
-#pragma unroll
-            for (int jj = 0; jj < m; ++jj) {
-              double s = tE[jj][d];
-#pragma unroll
-              for (int k = 0; k < jj; ++k) s = fma(-L[jj][k], t[k], s);
-              t[jj] = s * inv[jj];
-              rhs[jj][d] -= t[jj];
-            }
-          }
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-#pragma unroll
-            for (int jj = m - 1; jj >= 0; --jj) {
-              double s = rhs[jj][d];
-#pragma unroll
-              for (int k = jj + 1; k < m; ++k) s = fma(-L[k][jj], sd[1 + k][d], s);
-              sd[1 + jj][d] = s * inv[jj];
-            }
-            sd[0][d] = xv[d];
-          }
+          for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
+          S::back_substitute(sv, tE, xv, sd);
           store_free(v, sd);
         }
         __syncwarp();
-        emit_all(v, v, T, iT, sd, ed);
+        out.emit(v, v, T, iT, sd, ed, traj0);
         if (act) {
 #pragma unroll
           for (int d = 0; d < D; ++d)
@@ -555,12 +282,12 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
       for (int d = 0; d < D; ++d) {
         sd[0][d] = stash[size_t(d) * kTmemThreads];
 #pragma unroll
-        for (int b = 0; b < m; ++b) sd[1 + b][d] = sgn(b) * __ldg(fx + d * nf + e0 + b);
+        for (int b = 0; b < m; ++b) sd[1 + b][d] = fr.sgn(b) * __ldg(fx + d * nf + e0 + b);
       }
       const double T = stash[size_t(D) * kTmemThreads];
       const double iT = fast_rcp(T);
       __syncwarp();
-      emit_all(0, 0, T, iT, sd, ed);
+      out.emit(0, 0, T, iT, sd, ed, traj0);
     }
   }
 

@@ -28,15 +28,27 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast
 
 constexpr int kTmemThreads = 128;
 
+// coefficient staging tiles of the four warps of a CTA at the start of dynamic shared memory: one whole segment (D*N
+// contiguous output doubles) per lane, i.e. two 16-row TMA boxes per warp
 template <int N, int D>
-__host__ __device__ constexpr int tmem_stage_bytes_per_warp() {
-  return 32 * D * (N / 2) * 16;  // one whole segment (D*N contiguous output doubles) per lane: two 16-row TMA boxes
+__host__ __device__ constexpr size_t tmem_stage_bytes() {
+  return size_t(kTmemThreads / 32) * 32 * D * (N / 2) * 16;
 }
+// bytes of `slots` per-thread doubles (slot s of thread t at double s * kTmemThreads + t)
+__host__ __device__ constexpr size_t tmem_slot_bytes(size_t slots) { return slots * kTmemThreads * 8; }
 
-template <int D>
-__host__ __device__ constexpr int tmem_prefetch_bytes() {
-  return 2 * (1 + D) * kTmemThreads * 8;
-}
+// Dynamic shared memory of v3 (and its cost-only instantiation) behind the staging tiles, in per-thread slots:
+// [prefetch ring 2 x (1+D)][time history nmax+1][sweep state: nmax blocks with the vertex position]
+template <int N, int D>
+struct V3Layout {
+  static constexpr int kSlots = sweep_state_slots<N, D, true>();
+  static constexpr int kHist = 2 * (1 + D);                                 // ring, then the time history
+  __host__ __device__ static constexpr int hist_slots(int nmax) { return nmax + 1; }  // history, then the state
+  __host__ __device__ static constexpr size_t state(int nmax) { return size_t(kHist) + hist_slots(nmax); }
+  __host__ __device__ static constexpr size_t bytes(int K) {
+    return tmem_stage_bytes<N, D>() + tmem_slot_bytes(state((K + 1) / 2 - 1) + size_t((K + 1) / 2 - 1) * kSlots);
+  }
+};
 
 __device__ __forceinline__ void cp_async8(const double* smem_dst, const double* gsrc) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
@@ -56,19 +68,60 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
+// Output of the twisted TMA kernels: each lane writes the D*N doubles of the segment it emits into row (half*16 +
+// trajectory) of the warp's staging tile; one elected lane hands the two 16-row boxes (forward halves: segment j,
+// reversed halves: segment K-1-j) to the TMA.  No cooperative read-back and no global-store LSU wavefronts.
+template <int N, int D, class AI>
+struct TmaEmitter {
+  static constexpr int h = N / 2;
+  const CUtensorMap* tmap;
+  double2* stage;   // this warp's staging tile [half][16][D*h]
+  double2* my_row;  // this lane's row of it
+  int lane, K;
+  int nhF, nhB;  // a half is active in sweep step v iff v <= its nh
+  // emit own-frame segment j for every lane of the warp at once (convergent); v_step: the sweep step (0 = final).
+  // Rows of lanes that are not active in v_step are not stored.
+  __device__ __forceinline__ void emit(int j, int v_step, double T, double iT, const double (&sd)[h][D],
+                                       const double (&ed)[h][D], long long traj0) const {
+    using HF = sweep::Hermite<N, AI>;
+    const int half = lane & 1;
+    double tp[h], itp[h];
+    HF::powers(T, iT, half, tp, itp);
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+      double c[N];
+      HF::template coeffs<D>(half, tp, itp, sd, ed, d, c);
+      if (d == 0) {  // the TMA must have finished reading the previous segment's tile
+        if (lane == 0) bulk_wait_read();
+        __syncwarp();
+      }
+#pragma unroll
+      for (int q = 0; q < h; ++q) my_row[d * h + q] = make_double2(c[2 * q], c[2 * q + 1]);
+    }
+    fence_proxy_async();
+    __syncwarp();
+    if (lane == 0) {
+      if (v_step <= nhF) tma_store_box(tmap, stage, j * (D * N), (int)traj0);
+      if (v_step <= nhB) tma_store_box(tmap, stage + 16 * (D * h), (K - 1 - j) * (D * N), (int)traj0);
+      bulk_commit();
+    }
+  }
+};
+
 template <int N, int R, int D, bool FUSED = false, bool COST = false>
 __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
     twisted_tmem_kernel(const WaypointParams prm, const __grid_constant__ CUtensorMap tmap) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
-  constexpr int kL = m * (m + 1) / 2;
+  using Lay = V3Layout<N, D>;
   // per eliminated vertex: L (strictly lower) + inverse pivots + y + the vertex position (so that the
   // outward sweep does not re-read it from global memory)
-  constexpr int kSlots = kL + m * D + D;
+  constexpr int kSlots = Lay::kSlots;
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
   using G = H1Imm<N, R>;     // immediates: this kernel is register-bound (see mtg_device.cuh)
   using AI = A1InvImm<N>;
+  using S = sweep::Sweep<N, D, G>;
 
   extern __shared__ __align__(128) unsigned char smem_raw[];  // TMA tensor stores need 128-byte aligned tiles
   const int lane = threadIdx.x & 31;
@@ -79,30 +132,21 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
   const int M = (K + 1) >> 1;
   const int nh = half ? K - M - 1 : M - 1;
   const int nmax = M - 1;
+  const sweep::Frame<N> fr{K, half};
 
-  // ---- shared memory carve-up: [staging: kWarps tiles][prefetch ring][time history][sweep state]
+  // ---- shared memory carve-up (V3Layout): [staging: kWarps tiles][prefetch ring][time history][sweep state]
   double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);  // [half][16][D*h]
   // per-thread prefetch ring for the next step's inputs (segment time + D positions), filled by
   // cp.async: a register prefetch would share its scoreboard slot with the load being consumed and the
   // consumer would wait for the NEW loads as well (measured: 25 % of all stall samples).
-  double* pf = reinterpret_cast<double*>(smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) + threadIdx.x;
+  double* pf = reinterpret_cast<double*>(smem_raw + tmem_stage_bytes<N, D>()) + threadIdx.x;
   auto PF = [&](int buf, int slot) -> double* { return pf + (size_t(buf) * (1 + D) + slot) * kTmemThreads; };
   // per-thread history of the own-frame segment times seen by the inward sweep (nmax+1 doubles): the
   // outward sweep reads them back from shared memory (in FUSED mode this also saves the sqrt/exp)
-  double* thist = reinterpret_cast<double*>(smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>() +
-                                            tmem_prefetch_bytes<D>()) +
-                  threadIdx.x;
+  double* thist = pf + size_t(Lay::kHist) * kTmemThreads;
   auto HT = [&](int j) -> double& { return thist[size_t(j) * kTmemThreads]; };
-  double* state = thist + size_t(nmax + 1) * kTmemThreads;
+  double* state = thist + size_t(Lay::hist_slots(nmax)) * kTmemThreads;
   auto SP = [&](int blk, int slot) -> double& { return state[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
-  auto put_state = [&](int blk, const double (&sv)[kSlots]) {
-#pragma unroll
-    for (int i = 0; i < kSlots; ++i) SP(blk, i) = sv[i];
-  };
-  auto get_state = [&](int blk, double (&sv)[kSlots]) {
-#pragma unroll
-    for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk, i);
-  };
 
   const long long traj0 = ((long long)blockIdx.x * kWarps + warp) * 16;  // first trajectory of this warp
   long long traj = traj0 + (lane >> 1);
@@ -127,23 +171,17 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
   const double* __restrict__ tt = FUSED ? nullptr : prm.times + src * K;
   const double* __restrict__ fx =
       FUSED ? prm.positions + src * (long long)(K + 1) * D : prm.dfix + src * (long long)D * nf;
-  auto seg = [&](int j) -> int { return half ? K - 1 - j : j; };
-  auto pidx = [&](int v) -> int {
-    const int o = half ? K - v : v;
-    return o == 0 ? 0 : (o < K ? h + o - 1 : h + K - 1);
-  };
-  auto sgn = [&](int idx) -> double { return (half && !(idx & 1)) ? -1.0 : 1.0; };
   // address of coordinate d of own-frame vertex v
   auto xaddr = [&](int v, int d) -> const double* {
     if constexpr (FUSED) {
-      return fx + (half ? K - v : v) * D + d;
+      return fx + fr.vert(v) * D + d;
     } else {
-      return fx + d * nf + pidx(v);
+      return fx + d * nf + fr.pidx(v);
     }
   };
   // prefetch (time of own segment j, position of own vertex v) into ring buffer `buf`
   auto pf_issue = [&](int buf, int j, int v) {
-    if constexpr (!FUSED) cp_async8(PF(buf, 0), tt + seg(j));
+    if constexpr (!FUSED) cp_async8(PF(buf, 0), tt + fr.seg(j));
 #pragma unroll
     for (int d = 0; d < D; ++d) cp_async8(PF(buf, 1 + d), xaddr(v, d));
   };
@@ -152,26 +190,21 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
   // ---- issue the first global loads NOW: their latency overlaps the index set-up below
   double T0e = 0.0, x0e[D], x1e[D], u0e[m][D];
   {
-    const int e0 = half ? h + K : 1;
 #pragma unroll
     for (int d = 0; d < D; ++d) {
       x0e[d] = __ldg(xaddr(0, d));
       x1e[d] = __ldg(xaddr(1, d));
 #pragma unroll
-      for (int b = 0; b < m; ++b) u0e[b][d] = FUSED ? 0.0 : __ldg(fx + d * nf + e0 + b);
+      for (int b = 0; b < m; ++b) u0e[b][d] = FUSED ? 0.0 : __ldg(fx + d * nf + fr.e0() + b);
     }
-    if constexpr (!FUSED) T0e = __ldg(tt + seg(0));
+    if constexpr (!FUSED) T0e = __ldg(tt + fr.seg(0));
     pf_issue(1, 1, 2);  // inputs of sweep step v = 1 -> ring buffer (v & 1)
   }
 
-  // ---- output: each lane writes the D*N doubles of the segment it emits into row (half*16 + trajectory) of
-  // the warp's staging tile; one elected lane hands the two 16-row boxes (forward halves: segment j, reversed
-  // halves: segment K-1-j) to the TMA.  No cooperative read-back and no global-store LSU wavefronts.
   double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
   const int nhF = M - 1, nhB = K - M - 1;  // a half is active in sweep step v iff v <= its nh
+  const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB};
 
-  // emit own-frame segment j for every lane of the warp at once (convergent).  `act`: this lane's
-  // values are meaningful; rows of inactive lanes are not stored.  v_step: the sweep step (0 = final).
   double cost_acc = 0.0;
   auto emit_all = [&](int j, int v_step, double T, double iT, const double (&sd)[h][D], const double (&ed)[h][D]) {
     if constexpr (COST) {
@@ -206,61 +239,7 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
       }
       return;
     }
-    // original orientation: start = J*(own end) for the reversed half; J folded into the powers
-    double tp[h], itp[h];
-    const double Ts = half ? -T : T;
-    tp[0] = 1.0;
-#pragma unroll
-    for (int k = 1; k < h; ++k) tp[k] = tp[k - 1] * Ts;
-    itp[0] = pow_int<h>(iT);
-#pragma unroll
-    for (int k = 1; k < h; ++k) itp[k] = itp[k - 1] * iT;
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-      double c[N], ss[h], se[h];
-#pragma unroll
-      for (int k = 0; k < h; ++k) {
-        const double s0 = half ? ed[k][d] : sd[k][d];
-        const double e0 = half ? sd[k][d] : ed[k][d];
-        c[k] = s0 * ((half && (k & 1)) ? -AI::at(k, k) : AI::at(k, k));
-        ss[k] = tp[k] * s0;
-        se[k] = tp[k] * e0;
-      }
-      // Upper coefficients in Hermite form: A(1)^-1 = [[L^-1, 0], [-D^-1 C L^-1, D^-1]] and (C L^-1)[k][j] =
-      // 1/(j-k)! (derivative k of the Taylor part at tau = 1), so  q = D^-1 (se - C L^-1 ss):
-      // h(h+1)/2 + h^2 operations instead of 2 h^2, and the 1/(j-k)! factors are mostly dyadic immediates.
-      double ee[h];
-#pragma unroll
-      for (int k = 0; k < h; ++k) {
-        double acc = se[k] - ss[k];
-#pragma unroll
-        for (int j = k + 1; j < h; ++j) {
-          constexpr double kInvFact[6] = {1.0, 1.0, 0.5, 1.0 / 6.0, 1.0 / 24.0, 1.0 / 120.0};
-          acc = (j - k == 1) ? acc - ss[j] : fma(-kInvFact[j - k], ss[j], acc);
-        }
-        ee[k] = acc;
-      }
-#pragma unroll
-      for (int q = 0; q < h; ++q) {
-        double acc = AI::at(h + q, h) * ee[0];
-#pragma unroll
-        for (int k = 1; k < h; ++k) acc = fma(AI::at(h + q, h + k), ee[k], acc);
-        c[h + q] = acc * itp[q];
-      }
-      if (d == 0) {  // the TMA must have finished reading the previous segment's tile
-        if (lane == 0) bulk_wait_read();
-        __syncwarp();
-      }
-#pragma unroll
-      for (int q = 0; q < h; ++q) my_row[d * h + q] = make_double2(c[2 * q], c[2 * q + 1]);
-    }
-    fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) {
-      if (v_step <= nhF) tma_store_box(&tmap, stage, j * (D * N), (int)traj0);
-      if (v_step <= nhB) tma_store_box(&tmap, stage + 16 * (D * h), (K - 1 - j) * (D * N), (int)traj0);
-      bulk_commit();
-    }
+    out.emit(j, v_step, T, iT, sd, ed, traj0);
   };
 
   int stat = 0;
@@ -275,37 +254,15 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
     if constexpr (FUSED) {
       T0 = nfabian_time<D>(xm, xc, prm.v_max, prm.a_max, prm.magic);
     } else {
-      T0 = time_of(T0e, seg(0));
+      T0 = time_of(T0e, fr.seg(0));
     }
     if (!(T0 > 0.0)) stat |= kStatusBadTime;
     HT(0) = T0;
     const double iT0 = fast_rcp(T0);
     double pw[N - 1];
     segment_powers<N, R>(T0, iT0, pw);
-#pragma unroll
-    for (int a = 0; a < m; ++a) {
-#pragma unroll
-      for (int b = 0; b < m; ++b) {
-        Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-        Wp[a][b] = 0.0;
-      }
-      cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-      cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
-    }
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-      double u0[m];
-#pragma unroll
-      for (int b = 0; b < m; ++b) u0[b] = sgn(b) * u0e[b][d];
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-        double acc = 0.0;
-#pragma unroll
-        for (int b = 0; b < m; ++b) acc = fma(pw[a + b + 2] * G::at(h + 1 + a, 1 + b), u0[b], acc);
-        bcar[a][d] = -acc;
-        yp[a][d] = 0.0;
-      }
-    }
+    S::end_blocks(pw, Cee, cps, cpe);
+    S::carry_bcar(pw, [&](int b, int d) { return fr.sgn(b) * u0e[b][d]; }, Wp, yp, bcar);
   }
 
   // ---------------------------------------------------------------- sweep towards the middle
@@ -320,7 +277,7 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
       if constexpr (FUSED) {
         T = nfabian_time<D>(xc, xn, prm.v_max, prm.a_max, prm.magic);
       } else {
-        T = time_of(*PF(v & 1, 0), seg(v));
+        T = time_of(*PF(v & 1, 0), fr.seg(v));
       }
       HT(v) = T;
       {  // prefetch the next step's inputs (clamped indices: never out of bounds)
@@ -333,91 +290,15 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
       double pw[N - 1];
       segment_powers<N, R>(T, iT, pw);
 
-      double Dp[m][m], E[m][m], bb[m][D];
+      double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
+      S::assemble(pw, Cee, cps, cpe, bcar, Wp, yp, xm, xc, xn, Dp, E, bb);
+      S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
+      S::pack(L, inv, yp, xc, sv);  // with the position of the vertex just eliminated
+      S::end_blocks(pw, Cee, cps, cpe);
 #pragma unroll
-      for (int a = 0; a < m; ++a) {
-#pragma unroll
-        for (int b = 0; b <= a; ++b) {
-          double s = fma(pw[a + b + 2], G::at(1 + a, 1 + b), Cee[a][b]);
-#pragma unroll
-          for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-          Dp[a][b] = s;
-        }
-#pragma unroll
-        for (int b = 0; b < m; ++b) E[a][b] = pw[a + b + 2] * G::at(1 + a, h + 1 + b);
-        const double gmid = fma(pw[a + 1], G::at(1 + a, 0), cpe[a]);
-        const double gnext = pw[a + 1] * G::at(1 + a, h);
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          double s = bcar[a][d];
-          s = fma(-cps[a], xm[d], s);
-          s = fma(-gmid, xc[d], s);
-          s = fma(-gnext, xn[d], s);
-#pragma unroll
-          for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-          bb[a][d] = s;
-        }
-      }
-      double L[m][m], inv[m];
-#pragma unroll
-      for (int j = 0; j < m; ++j) {
-        double s = Dp[j][j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) s = fma(-L[j][k], L[j][k], s);
-        if (!(s > 0.0)) stat |= kStatusNotSpd;
-        inv[j] = fast_rsqrt(s);
-#pragma unroll
-        for (int i = j + 1; i < m; ++i) {
-          double t = Dp[i][j];
-#pragma unroll
-          for (int k = 0; k < j; ++k) t = fma(-L[i][k], L[j][k], t);
-          L[i][j] = t * inv[j];
-        }
-      }
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-#pragma unroll
-        for (int j = 0; j < m; ++j) {
-          double s = bb[j][d];
-#pragma unroll
-          for (int k = 0; k < j; ++k) s = fma(-L[j][k], yp[k][d], s);
-          yp[j][d] = s * inv[j];
-        }
-      }
-#pragma unroll
-      for (int c = 0; c < m; ++c) {
-#pragma unroll
-        for (int j = 0; j < m; ++j) {
-          double s = E[j][c];
-#pragma unroll
-          for (int k = 0; k < j; ++k) s = fma(-L[j][k], Wp[k][c], s);
-          Wp[j][c] = s * inv[j];
-        }
-      }
-      {
-        int slot = 0;
-#pragma unroll
-        for (int i = 1; i < m; ++i)
-#pragma unroll
-          for (int j = 0; j < i; ++j) sv[slot++] = L[i][j];
-#pragma unroll
-        for (int j = 0; j < m; ++j) sv[slot++] = inv[j];
-#pragma unroll
-        for (int j = 0; j < m; ++j)
-#pragma unroll
-          for (int d = 0; d < D; ++d) sv[slot++] = yp[j][d];
-#pragma unroll
-        for (int d = 0; d < D; ++d) sv[slot++] = xc[d];  // position of the vertex just eliminated
-      }
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-#pragma unroll
-        for (int b = 0; b <= a; ++b) Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-        cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-        cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
+      for (int a = 0; a < m; ++a)
 #pragma unroll
         for (int d = 0; d < D; ++d) bcar[a][d] = 0.0;
-      }
 #pragma unroll
       for (int d = 0; d < D; ++d) {
         xm[d] = xc[d];
@@ -425,82 +306,14 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
       }
     }
     __syncwarp();
-    put_state(v - 1, sv);
+#pragma unroll
+    for (int i = 0; i < kSlots; ++i) SP(v - 1, i) = sv[i];
   }
   __syncwarp();
 
   // ---------------------------------------------------------------- middle vertex
   double um[m][D];
-  {
-    double Dl[m][m], bl[m][D];
-#pragma unroll
-    for (int a = 0; a < m; ++a) {
-#pragma unroll
-      for (int b = 0; b <= a; ++b) {
-        double s = Cee[a][b];
-#pragma unroll
-        for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-        Dl[a][b] = s;
-      }
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double s = bcar[a][d];
-        s = fma(-cps[a], xm[d], s);
-        s = fma(-cpe[a], xc[d], s);
-#pragma unroll
-        for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-        bl[a][d] = s;
-      }
-    }
-#pragma unroll
-    for (int a = 0; a < m; ++a) {
-#pragma unroll
-      for (int b = 0; b <= a; ++b) {
-        const double o = __shfl_xor_sync(kFull, Dl[a][b], 1);
-        Dl[a][b] += ((a + b) & 1) ? -o : o;
-      }
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        const double o = __shfl_xor_sync(kFull, bl[a][d], 1);
-        bl[a][d] += (a & 1) ? o : -o;
-      }
-    }
-    stat |= __shfl_xor_sync(kFull, stat, 1);
-    double L[m][m], inv[m];
-#pragma unroll
-    for (int j = 0; j < m; ++j) {
-      double s = Dl[j][j];
-#pragma unroll
-      for (int k = 0; k < j; ++k) s = fma(-L[j][k], L[j][k], s);
-      if (!(s > 0.0)) stat |= kStatusNotSpd;
-      inv[j] = fast_rsqrt(s);
-#pragma unroll
-      for (int i = j + 1; i < m; ++i) {
-        double t = Dl[i][j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) t = fma(-L[i][k], L[j][k], t);
-        L[i][j] = t * inv[j];
-      }
-    }
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-      double y[m];
-#pragma unroll
-      for (int j = 0; j < m; ++j) {
-        double s = bl[j][d];
-#pragma unroll
-        for (int k = 0; k < j; ++k) s = fma(-L[j][k], y[k], s);
-        y[j] = s * inv[j];
-      }
-#pragma unroll
-      for (int j = m - 1; j >= 0; --j) {
-        double s = y[j];
-#pragma unroll
-        for (int k = j + 1; k < m; ++k) s = fma(-L[k][j], um[k][d], s);
-        um[j][d] = s * inv[j];
-      }
-    }
-  }
+  S::middle(Cee, cps, cpe, bcar, Wp, yp, xm, xc, um, stat);
   if (valid && half == 0 && prm.status != nullptr) prm.status[traj] = stat;
 
   // ---------------------------------------------------------------- outward back-substitution
@@ -508,11 +321,11 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
   double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + traj * (long long)D * np : nullptr;
   auto store_free = [&](int v_own, const double (&u)[h][D]) {
     if (df != nullptr && valid) {
-      const int vo = half ? K - v_own : v_own;
+      const int vo = fr.vert(v_own);
 #pragma unroll
       for (int d = 0; d < D; ++d)
 #pragma unroll
-        for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = sgn(j) * u[1 + j][d];
+        for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
     }
   };
 
@@ -534,7 +347,8 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
 
   for (int v = nmax; v >= 1; --v) {
     double sv[kSlots];
-    get_state(v - 1, sv);
+#pragma unroll
+    for (int i = 0; i < kSlots; ++i) sv[i] = SP(v - 1, i);
     const bool act = v <= nh;
     double T = 1.0, iT = 1.0;
     double sd[h][D];  // inactive lanes (odd K only) emit garbage rows that are never stored
@@ -542,66 +356,24 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
       cp_async_wait_all();
       double xv[D];
 #pragma unroll
-      for (int d = 0; d < D; ++d) xv[d] = sv[kL + m * D + d];
+      for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
       T = HT(v);
       if constexpr (FUSED) {
-        if (tout != nullptr && valid) tout[seg(v)] = T;
+        if (tout != nullptr && valid) tout[fr.seg(v)] = T;
       }
       pf_issue_out(v - 1);
       if constexpr (!FUSED) {
         if (v == 1) {  // the final emission re-reads the fixed end derivatives: pull their lines into L1 now
-          const int e0 = half ? h + K : 1;
 #pragma unroll
-          for (int d = 0; d < D; ++d) asm volatile("prefetch.global.L1 [%0];" ::"l"(fx + d * nf + e0));
+          for (int d = 0; d < D; ++d) asm volatile("prefetch.global.L1 [%0];" ::"l"(fx + d * nf + fr.e0()));
         }
       }
       iT = fast_rcp(T);
-      double L[m][m], inv[m], rhs[m][D];
-      {
-        int slot = 0;
-#pragma unroll
-        for (int i = 1; i < m; ++i)
-#pragma unroll
-          for (int j = 0; j < i; ++j) L[i][j] = sv[slot++];
-#pragma unroll
-        for (int j = 0; j < m; ++j) inv[j] = sv[slot++];
-#pragma unroll
-        for (int j = 0; j < m; ++j)
-#pragma unroll
-          for (int d = 0; d < D; ++d) rhs[j][d] = sv[slot++];
-      }
-      double pw[N - 1];
+      double L[m][m], inv[m], rhs[m][D], pw[N - 1];
+      S::unpack(sv, L, inv, rhs);
       segment_powers<N, R>(T, iT, pw);
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double t[m];
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-          double s = 0.0;
-#pragma unroll
-          for (int b = 0; b < m; ++b) s = fma(pw[a + b + 2] * G::at(1 + a, h + 1 + b), ed[1 + b][d], s);
-          t[a] = s;
-        }
-#pragma unroll
-        for (int j = 0; j < m; ++j) {
-          double s = t[j];
-#pragma unroll
-          for (int k = 0; k < j; ++k) s = fma(-L[j][k], t[k], s);
-          t[j] = s * inv[j];
-          rhs[j][d] -= t[j];
-        }
-      }
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-#pragma unroll
-        for (int j = m - 1; j >= 0; --j) {
-          double s = rhs[j][d];
-#pragma unroll
-          for (int k = j + 1; k < m; ++k) s = fma(-L[k][j], sd[1 + k][d], s);
-          sd[1 + j][d] = s * inv[j];
-        }
-        sd[0][d] = xv[d];
-      }
+      S::uncouple_from(pw, ed, L, inv, rhs);
+      S::solve_back(L, inv, rhs, xv, sd);
       store_free(v, sd);
     }
     __syncwarp();
@@ -615,17 +387,16 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
   }
   {
     cp_async_wait_all();
-    const int e0 = half ? h + K : 1;
     double sd[h][D];
 #pragma unroll
     for (int d = 0; d < D; ++d) {
       sd[0][d] = *PF(0, 1 + d);
 #pragma unroll
-      for (int b = 0; b < m; ++b) sd[1 + b][d] = FUSED ? 0.0 : sgn(b) * __ldg(fx + d * nf + e0 + b);
+      for (int b = 0; b < m; ++b) sd[1 + b][d] = FUSED ? 0.0 : fr.sgn(b) * __ldg(fx + d * nf + fr.e0() + b);
     }
     const double T = HT(0);
     if constexpr (FUSED) {
-      if (tout != nullptr && valid) tout[seg(0)] = T;
+      if (tout != nullptr && valid) tout[fr.seg(0)] = T;
     }
     const double iT = fast_rcp(T);
     __syncwarp();

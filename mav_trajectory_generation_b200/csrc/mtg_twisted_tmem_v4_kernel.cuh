@@ -22,29 +22,26 @@
 namespace mtg {
 
 struct TmemLaunchV4 {
-  int region_slots;   // doubles per thread of the sweep-state / next-tile-prologue region
   unsigned long long* tile_counter;  // non-null: warps draw their 16-trajectory tiles from this counter (zeroed by
                                      // the host before the launch); null: static round-robin assignment
 };
 
-template <int N, int D>
-__host__ __device__ constexpr int v4_pro_slots() {
-  return 2 * D + (N / 2 - 1) * D + 1;  // x0, x1, u0[m], T0
-}
-template <int N, int D>
-__host__ __device__ constexpr int v4_state_slots() {
-  constexpr int m = N / 2 - 1;
-  return m * (m + 1) / 2 + m * D + D;
-}
-// dynamic shared memory of a CTA
+// Dynamic shared memory of v4 behind the staging tiles, in per-thread slots:
+// [input ring RD x (1+D)][time history nmax+1][x0 stash D][region: sweep state, or the next tile's prologue inputs]
 template <int N, int D, int RD>
-__host__ __device__ constexpr size_t v4_smem_bytes(int K) {
-  const int nmax = (K + 1) / 2 - 1;
-  const int state = nmax * v4_state_slots<N, D>();
-  const int region = state > v4_pro_slots<N, D>() ? state : v4_pro_slots<N, D>();
-  return size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() +
-         size_t(RD * (1 + D) + (nmax + 1) + D + region) * kTmemThreads * 8;
-}
+struct V4Layout {
+  static constexpr int kSlots = sweep_state_slots<N, D, true>();
+  static constexpr int kPro = 2 * D + (N / 2 - 1) * D + 1;  // x0, x1, u0[m], T0
+  static constexpr int kHist = RD * (1 + D);                                // ring, then the time history
+  __host__ __device__ static constexpr int hist_slots(int nmax) { return nmax + 1; }  // history, then the x0 stash
+  __host__ __device__ static constexpr size_t x0(int nmax) { return size_t(kHist) + hist_slots(nmax); }
+  __host__ __device__ static constexpr size_t region(int nmax) { return x0(nmax) + D; }
+  __host__ __device__ static constexpr size_t bytes(int K) {
+    return tmem_stage_bytes<N, D>() + tmem_slot_bytes(region((K + 1) / 2 - 1) + (size_t((K + 1) / 2 - 1) * kSlots > kPro
+                                                                                      ? size_t((K + 1) / 2 - 1) * kSlots
+                                                                                      : size_t(kPro)));
+  }
+};
 
 template <int NPEND>
 __device__ __forceinline__ void cp_async_wait_group() {
@@ -57,15 +54,15 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     twisted_tmem_v4_kernel(const WaypointParams prm, const TmemLaunchV4 tl, const __grid_constant__ CUtensorMap tmap) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
-  constexpr int kL = m * (m + 1) / 2;
-  constexpr int kSlots = kL + m * D + D;
-  constexpr int kPro = v4_pro_slots<N, D>();
+  using Lay = V4Layout<N, D, RD>;
+  constexpr int kSlots = Lay::kSlots;
+  constexpr int kPro = Lay::kPro;
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
-  constexpr double kTiny = 0x1p-600, kHuge = 0x1p+600;
   static_assert(RD >= 2, "ring depth");
   using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
+  using S = sweep::Sweep<N, D, G>;
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -77,34 +74,19 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   const int nh = half ? K - M - 1 : M - 1;
   const int nmax = M - 1;
 
-  // ---- shared memory: [staging x kWarps][ring RD x (1+D)][time history nmax+1][x0 stash D][region]
+  // ---- shared memory (V4Layout): [staging x kWarps][ring RD x (1+D)][time history nmax+1][x0 stash D][region]
   double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);
-  double* base = reinterpret_cast<double*>(smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>()) +
-                 threadIdx.x;
+  double* base = reinterpret_cast<double*>(smem_raw + tmem_stage_bytes<N, D>()) + threadIdx.x;
   auto PF = [&](int buf, int slot) -> double* { return base + (size_t(buf) * (1 + D) + slot) * kTmemThreads; };
-  double* thist = base + size_t(RD) * (1 + D) * kTmemThreads;
+  double* thist = base + size_t(Lay::kHist) * kTmemThreads;
   auto HT = [&](int j) -> double& { return thist[size_t(j) * kTmemThreads]; };
-  double* x0s = thist + size_t(nmax + 1) * kTmemThreads;
+  double* x0s = thist + size_t(Lay::hist_slots(nmax)) * kTmemThreads;
   double* region = x0s + size_t(D) * kTmemThreads;  // sweep state blocks; next tile's prologue inputs
   auto SP = [&](int blk, int slot) -> double& { return region[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
   auto PRO = [&](int slot) -> double* { return region + size_t(slot) * kTmemThreads; };
 
-  auto put_state = [&](int blk, const double (&sv)[kSlots]) {
-#pragma unroll
-    for (int i = 0; i < kSlots; ++i) SP(blk, i) = sv[i];
-  };
-  auto get_state = [&](int blk, double (&sv)[kSlots]) {
-#pragma unroll
-    for (int i = 0; i < kSlots; ++i) sv[i] = SP(blk, i);
-  };
-
-  auto seg = [&](int j) -> int { return half ? K - 1 - j : j; };
-  auto pidx = [&](int v) -> int {
-    const int o = half ? K - v : v;
-    return o == 0 ? 0 : (o < K ? h + o - 1 : h + K - 1);
-  };
-  auto sgn = [&](int idx) -> double { return (half && !(idx & 1)) ? -1.0 : 1.0; };
-  const int e0 = half ? h + K : 1;  // first fixed end-derivative slot of own-frame vertex 0
+  const sweep::Frame<N> fr{K, half};
+  const int e0 = fr.e0();
 
   const long long n_wtiles = (prm.B + 15) >> 4;
   const long long wt_stride = (long long)gridDim.x * kWarps;
@@ -132,9 +114,9 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   };
   auto xaddr = [&](const Ptrs& p, int v, int d) -> const double* {
     if constexpr (FUSED) {
-      return p.fx + (half ? K - v : v) * D + d;
+      return p.fx + fr.vert(v) * D + d;
     } else {
-      return p.fx + d * nf + pidx(v);
+      return p.fx + d * nf + fr.pidx(v);
     }
   };
   // next tile's prologue inputs -> PRO region (cp.async; the caller commits the group)
@@ -148,14 +130,14 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         for (int b = 0; b < m; ++b) cp_async8(PRO(2 * D + b * D + d), p.fx + d * nf + e0 + b);
       }
     }
-    if constexpr (!FUSED) cp_async8(PRO(kPro - 1), p.tt + seg(0));
+    if constexpr (!FUSED) cp_async8(PRO(kPro - 1), p.tt + fr.seg(0));
   };
   // inputs of inward step v (time of own segment v, position of own vertex v+1) -> ring buffer v % RD
   auto ring_issue = [&](const Ptrs& p, int v) {
     const int j = v < K ? v : K - 1;
     const int vn = v + 1 <= K ? v + 1 : K;
     const int buf = v % RD;
-    if constexpr (!FUSED) cp_async8(PF(buf, 0), p.tt + seg(j));
+    if constexpr (!FUSED) cp_async8(PF(buf, 0), p.tt + fr.seg(j));
 #pragma unroll
     for (int d = 0; d < D; ++d) cp_async8(PF(buf, 1 + d), xaddr(p, vn, d));
   };
@@ -168,6 +150,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
 
   double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
   const int nhF = M - 1, nhB = K - M - 1;
+  const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB};
 
   while (wt < n_wtiles) {
     long long wt_next = dyn ? draw_tile() : wt + wt_stride;  // known one tile ahead: its prologue is prefetched
@@ -176,61 +159,6 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     const long long traj0 = wt * 16;
     const bool valid = P.valid;
     double* __restrict__ tout = (FUSED && prm.times_out != nullptr) ? prm.times_out + P.traj * K : nullptr;
-
-    // emit own-frame segment j for every lane of the warp at once (convergent)
-    auto emit_all = [&](int j, int v_step, double T, double iT, const double (&sd)[h][D], const double (&ed)[h][D]) {
-      double tp[h], itp[h];
-      const double Ts = half ? -T : T;
-      tp[0] = 1.0;
-#pragma unroll
-      for (int k = 1; k < h; ++k) tp[k] = tp[k - 1] * Ts;
-      itp[0] = pow_int<h>(iT);
-#pragma unroll
-      for (int k = 1; k < h; ++k) itp[k] = itp[k - 1] * iT;
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double c[N], ss[h], se[h];
-#pragma unroll
-        for (int k = 0; k < h; ++k) {
-          const double s0 = half ? ed[k][d] : sd[k][d];
-          const double e0v = half ? sd[k][d] : ed[k][d];
-          c[k] = s0 * ((half && (k & 1)) ? -AI::at(k, k) : AI::at(k, k));
-          ss[k] = tp[k] * s0;
-          se[k] = tp[k] * e0v;
-        }
-        double ee[h];
-#pragma unroll
-        for (int k = 0; k < h; ++k) {
-          double acc = se[k] - ss[k];
-#pragma unroll
-          for (int j2 = k + 1; j2 < h; ++j2) {
-            constexpr double kInvFact[6] = {1.0, 1.0, 0.5, 1.0 / 6.0, 1.0 / 24.0, 1.0 / 120.0};
-            acc = (j2 - k == 1) ? acc - ss[j2] : fma(-kInvFact[j2 - k], ss[j2], acc);
-          }
-          ee[k] = acc;
-        }
-#pragma unroll
-        for (int q = 0; q < h; ++q) {
-          double acc = AI::at(h + q, h) * ee[0];
-#pragma unroll
-          for (int k = 1; k < h; ++k) acc = fma(AI::at(h + q, h + k), ee[k], acc);
-          c[h + q] = acc * itp[q];
-        }
-        if (d == 0) {  // the TMA must have finished reading the previous segment's tile
-          if (lane == 0) bulk_wait_read();
-          __syncwarp();
-        }
-#pragma unroll
-        for (int q = 0; q < h; ++q) my_row[d * h + q] = make_double2(c[2 * q], c[2 * q + 1]);
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        if (v_step <= nhF) tma_store_box(&tmap, stage, j * (D * N), (int)traj0);
-        if (v_step <= nhB) tma_store_box(&tmap, stage + 16 * (D * h), (K - 1 - j) * (D * N), (int)traj0);
-        bulk_commit();
-      }
-    };
 
     // ---- ring prefetch of the first RD-1 inward steps, then consume the prologue inputs (issued half a tile ago)
     // (a group is committed for every step even when it is empty -- steps beyond this lane's own range --
@@ -262,31 +190,8 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       const double iT0 = fast_rcp(T0);
       double pw[N - 1];
       segment_powers<N, R>(T0, iT0, pw);
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-#pragma unroll
-        for (int b = 0; b < m; ++b) {
-          Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-          Wp[a][b] = (a == b) ? kTiny : 0.0;
-        }
-        cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-        cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
-      }
-      // carry of the fixed end derivatives: b_1 -= H_0[end,start] u_0, stored as y = 2^600 * (H u_0) against
-      // W = 2^-600 I, so that  -W^T y  reproduces it exactly and  W^T W  underflows to zero
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double u0[m];
-#pragma unroll
-        for (int b = 0; b < m; ++b) u0[b] = FUSED ? 0.0 : sgn(b) * *PRO(2 * D + b * D + d);
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-          double acc = 0.0;
-#pragma unroll
-          for (int b = 0; b < m; ++b) acc = fma(pw[a + b + 2] * G::at(h + 1 + a, 1 + b), u0[b], acc);
-          yp[a][d] = acc * kHuge;
-        }
-      }
+      S::end_blocks(pw, Cee, cps, cpe);
+      S::carry_fold(pw, [&](int b, int d) { return FUSED ? 0.0 : fr.sgn(b) * *PRO(2 * D + b * D + d); }, Wp, yp);
     }
 
     // ---------------------------------------------------------------- sweep towards the middle
@@ -311,88 +216,11 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         double pw[N - 1];
         segment_powers<N, R>(T, iT, pw);
 
-        double Dp[m][m], E[m][m], bb[m][D];
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-#pragma unroll
-          for (int b = 0; b <= a; ++b) {
-            double s = fma(pw[a + b + 2], G::at(1 + a, 1 + b), Cee[a][b]);
-#pragma unroll
-            for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-            Dp[a][b] = s;
-          }
-#pragma unroll
-          for (int b = 0; b < m; ++b) E[a][b] = pw[a + b + 2] * G::at(1 + a, h + 1 + b);
-          const double gmid = fma(pw[a + 1], G::at(1 + a, 0), cpe[a]);
-          const double gnext = pw[a + 1] * G::at(1 + a, h);
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-            double s = -cps[a] * xm[d];
-            s = fma(-gmid, xc[d], s);
-            s = fma(-gnext, xn[d], s);
-#pragma unroll
-            for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-            bb[a][d] = s;
-          }
-        }
-        double L[m][m], inv[m];
-#pragma unroll
-        for (int j = 0; j < m; ++j) {
-          double s = Dp[j][j];
-#pragma unroll
-          for (int k = 0; k < j; ++k) s = fma(-L[j][k], L[j][k], s);
-          if (!(s > 0.0)) stat |= kStatusNotSpd;
-          inv[j] = fast_rsqrt(s);
-#pragma unroll
-          for (int i = j + 1; i < m; ++i) {
-            double t = Dp[i][j];
-#pragma unroll
-            for (int k = 0; k < j; ++k) t = fma(-L[i][k], L[j][k], t);
-            L[i][j] = t * inv[j];
-          }
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-#pragma unroll
-          for (int j = 0; j < m; ++j) {
-            double s = bb[j][d];
-#pragma unroll
-            for (int k = 0; k < j; ++k) s = fma(-L[j][k], yp[k][d], s);
-            yp[j][d] = s * inv[j];
-          }
-        }
-#pragma unroll
-        for (int c = 0; c < m; ++c) {
-#pragma unroll
-          for (int j = 0; j < m; ++j) {
-            double s = E[j][c];
-#pragma unroll
-            for (int k = 0; k < j; ++k) s = fma(-L[j][k], Wp[k][c], s);
-            Wp[j][c] = s * inv[j];
-          }
-        }
-        {
-          int slot = 0;
-#pragma unroll
-          for (int i = 1; i < m; ++i)
-#pragma unroll
-            for (int j = 0; j < i; ++j) sv[slot++] = L[i][j];
-#pragma unroll
-          for (int j = 0; j < m; ++j) sv[slot++] = inv[j];
-#pragma unroll
-          for (int j = 0; j < m; ++j)
-#pragma unroll
-            for (int d = 0; d < D; ++d) sv[slot++] = yp[j][d];
-#pragma unroll
-          for (int d = 0; d < D; ++d) sv[slot++] = xc[d];
-        }
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-#pragma unroll
-          for (int b = 0; b <= a; ++b) Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-          cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-          cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
-        }
+        double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
+        S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
+        S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
+        S::pack(L, inv, yp, xc, sv);
+        S::end_blocks(pw, Cee, cps, cpe);
 #pragma unroll
         for (int d = 0; d < D; ++d) {
           xm[d] = xc[d];
@@ -400,81 +228,14 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         }
       }
       __syncwarp();
-      put_state(v - 1, sv);
+#pragma unroll
+      for (int i = 0; i < kSlots; ++i) SP(v - 1, i) = sv[i];
     }
     __syncwarp();
 
     // ---------------------------------------------------------------- middle vertex
     double um[m][D];
-    {
-      double Dl[m][m], bl[m][D];
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-#pragma unroll
-        for (int b = 0; b <= a; ++b) {
-          double s = Cee[a][b];
-#pragma unroll
-          for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-          Dl[a][b] = s;
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          double s = -cps[a] * xm[d];
-          s = fma(-cpe[a], xc[d], s);
-#pragma unroll
-          for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-          bl[a][d] = s;
-        }
-      }
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-#pragma unroll
-        for (int b = 0; b <= a; ++b) {
-          const double o = __shfl_xor_sync(kFull, Dl[a][b], 1);
-          Dl[a][b] += ((a + b) & 1) ? -o : o;
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          const double o = __shfl_xor_sync(kFull, bl[a][d], 1);
-          bl[a][d] += (a & 1) ? o : -o;
-        }
-      }
-      stat |= __shfl_xor_sync(kFull, stat, 1);
-      double L[m][m], inv[m];
-#pragma unroll
-      for (int j = 0; j < m; ++j) {
-        double s = Dl[j][j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) s = fma(-L[j][k], L[j][k], s);
-        if (!(s > 0.0)) stat |= kStatusNotSpd;
-        inv[j] = fast_rsqrt(s);
-#pragma unroll
-        for (int i = j + 1; i < m; ++i) {
-          double t = Dl[i][j];
-#pragma unroll
-          for (int k = 0; k < j; ++k) t = fma(-L[i][k], L[j][k], t);
-          L[i][j] = t * inv[j];
-        }
-      }
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double y[m];
-#pragma unroll
-        for (int j = 0; j < m; ++j) {
-          double s = bl[j][d];
-#pragma unroll
-          for (int k = 0; k < j; ++k) s = fma(-L[j][k], y[k], s);
-          y[j] = s * inv[j];
-        }
-#pragma unroll
-        for (int j = m - 1; j >= 0; --j) {
-          double s = y[j];
-#pragma unroll
-          for (int k = j + 1; k < m; ++k) s = fma(-L[k][j], um[k][d], s);
-          um[j][d] = s * inv[j];
-        }
-      }
-    }
+    S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
     if (valid && half == 0 && prm.status != nullptr) prm.status[P.traj] = stat;
 
     // ---------------------------------------------------------------- outward back-substitution
@@ -482,11 +243,11 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + P.traj * (long long)D * np : nullptr;
     auto store_free = [&](int v_own, const double (&u)[h][D]) {
       if (df != nullptr && valid) {
-        const int vo = half ? K - v_own : v_own;
+        const int vo = fr.vert(v_own);
 #pragma unroll
         for (int d = 0; d < D; ++d)
 #pragma unroll
-          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = sgn(j) * u[1 + j][d];
+          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
       }
     };
 
@@ -530,66 +291,23 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       double pw[N - 1];
       segment_powers<N, R>(T, iT, pw);
       double sv[kSlots];
-      get_state(v - 1, sv);
+#pragma unroll
+      for (int i = 0; i < kSlots; ++i) sv[i] = SP(v - 1, i);
       double tE[m][D];
-#pragma unroll
-      for (int d = 0; d < D; ++d)
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-          double s = 0.0;
-#pragma unroll
-          for (int b = 0; b < m; ++b) s = fma(pw[a + b + 2] * G::at(1 + a, h + 1 + b), ed[1 + b][d], s);
-          tE[a][d] = s;
-        }
+      S::couple(pw, ed, tE);
       double sd[h][D];
       if (act) {
         double xv[D];
 #pragma unroll
-        for (int d = 0; d < D; ++d) xv[d] = sv[kL + m * D + d];
+        for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
         if constexpr (FUSED) {
-          if (tout != nullptr && valid) tout[seg(v)] = T;
+          if (tout != nullptr && valid) tout[fr.seg(v)] = T;
         }
-        double L[m][m], inv[m], rhs[m][D];
-        {
-          int slot = 0;
-#pragma unroll
-          for (int i = 1; i < m; ++i)
-#pragma unroll
-            for (int j = 0; j < i; ++j) L[i][j] = sv[slot++];
-#pragma unroll
-          for (int j = 0; j < m; ++j) inv[j] = sv[slot++];
-#pragma unroll
-          for (int j = 0; j < m; ++j)
-#pragma unroll
-            for (int d = 0; d < D; ++d) rhs[j][d] = sv[slot++];
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          double t[m];
-#pragma unroll
-          for (int j = 0; j < m; ++j) {
-            double s = tE[j][d];
-#pragma unroll
-            for (int k = 0; k < j; ++k) s = fma(-L[j][k], t[k], s);
-            t[j] = s * inv[j];
-            rhs[j][d] -= t[j];
-          }
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-#pragma unroll
-          for (int j = m - 1; j >= 0; --j) {
-            double s = rhs[j][d];
-#pragma unroll
-            for (int k = j + 1; k < m; ++k) s = fma(-L[k][j], sd[1 + k][d], s);
-            sd[1 + j][d] = s * inv[j];
-          }
-          sd[0][d] = xv[d];
-        }
+        S::back_substitute(sv, tE, xv, sd);
         store_free(v, sd);
       }
       __syncwarp();
-      emit_all(v, v, T, iT, sd, ed);
+      out.emit(v, v, T, iT, sd, ed, traj0);
       if (act) {
 #pragma unroll
         for (int d = 0; d < D; ++d)
@@ -612,19 +330,19 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
           if constexpr (FUSED) {
             sd[1 + b][d] = 0.0;
           } else if constexpr (kEndInRing) {
-            sd[1 + b][d] = sgn(b) * base[size_t(b * D + d) * kTmemThreads];
+            sd[1 + b][d] = fr.sgn(b) * base[size_t(b * D + d) * kTmemThreads];
           } else {
-            sd[1 + b][d] = sgn(b) * __ldg(P.fx + d * nf + e0 + b);
+            sd[1 + b][d] = fr.sgn(b) * __ldg(P.fx + d * nf + e0 + b);
           }
         }
       }
       const double T = HT(0);
       if constexpr (FUSED) {
-        if (tout != nullptr && valid) tout[seg(0)] = T;
+        if (tout != nullptr && valid) tout[fr.seg(0)] = T;
       }
       const double iT = fast_rcp(T);
       __syncwarp();
-      emit_all(0, 0, T, iT, sd, ed);
+      out.emit(0, 0, T, iT, sd, ed, traj0);
     }
     wt = wt_next;
   }

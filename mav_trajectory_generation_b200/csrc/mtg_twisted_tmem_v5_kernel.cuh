@@ -25,20 +25,37 @@ struct TmemLaunchV5 {
   unsigned long long* tile_counter;  // non-null: dynamic tile assignment
 };
 
-// sweep state per eliminated vertex: L (strictly lower) + inverse pivots + y  (positions come from the input tile)
-template <int N, int D>
-__host__ __device__ constexpr int v5_state_slots() {
-  constexpr int m = N / 2 - 1;
-  return m * (m + 1) / 2 + m * D;
-}
-// dynamic shared memory: [staging x 4 warps][mbarriers 128][input tiles: 4 warps x nbuf x 16*(K + D*nf)][state]
-template <int N, int D>
-__host__ __device__ constexpr size_t v5_smem_bytes(int K, int nf, int nbuf) {
-  const int nmax = (K + 1) / 2 - 1;
-  const int total = nmax * v5_state_slots<N, D>();
-  return size_t(kTmemThreads / 32) * tmem_stage_bytes_per_warp<N, D>() + 128 +
-         size_t(kTmemThreads / 32) * nbuf * 16 * size_t(K + D * nf) * 8 + size_t(total) * kTmemThreads * 8;
-}
+// Dynamic shared memory of v5: [staging x kWarps][mbarriers][input tiles: kWarps x nbuf][sweep state: nmax blocks]
+// [FUSED: time history nmax+1].  The state blocks hold no positions: the input tile stays resident for the whole tile.
+template <int N, int D, bool FUSED>
+struct V5Layout {
+  static constexpr int kSlots = sweep_state_slots<N, D>();
+  static constexpr int kBarBytes = 128;  // two 8-byte mbarriers per warp
+  // doubles of one input tile: seg_times[16][K] and d_fixed[16][D][nf], or (FUSED) positions[16][K+1][D]
+  __host__ __device__ static constexpr size_t tile_times(int K) { return FUSED ? 0 : size_t(16) * K; }
+  __host__ __device__ static constexpr size_t tile_fixed(int K, int nf) {
+    return FUSED ? size_t(16) * (K + 1) * D : size_t(16) * D * nf;
+  }
+  __host__ __device__ static constexpr size_t tile_doubles(int K, int nf) { return tile_times(K) + tile_fixed(K, nf); }
+  // per-thread slots behind the input tiles: nmax state blocks, then (FUSED) the time history
+  __host__ __device__ static constexpr size_t hist(int nmax) { return size_t(nmax) * kSlots; }
+  __host__ __device__ static constexpr size_t bytes(int K, int nf, int nbuf) {
+    return tmem_stage_bytes<N, D>() + kBarBytes + size_t(kTmemThreads / 32) * nbuf * tile_doubles(K, nf) * 8 +
+           tmem_slot_bytes(hist((K + 1) / 2 - 1) + (FUSED ? (K + 1) / 2 : 0));
+  }
+  // Early refill E (see below): parking area in the slots of the popped state blocks >= E, per lane:
+  // [own step u = E..1: x_u[D], T_u][x_0[D]][u_0[D][m]][T_0]
+  __host__ __device__ static constexpr int park_step(int E, int u) { return (E - u) * (D + 1); }
+  __host__ __device__ static constexpr int park_x0(int E) { return E * (D + 1); }
+  __host__ __device__ static constexpr int park_u0(int E) { return park_x0(E) + D; }
+  __host__ __device__ static constexpr int park_T0(int E) { return park_u0(E) + (N / 2 - 1) * D; }
+  __host__ __device__ static constexpr int early_stash_slots(int E) { return park_T0(E) + 1; }
+  template <int E>
+  __host__ __device__ static constexpr bool early_fits(int K) {
+    return E <= K - (K + 1) / 2 - 1 && E <= (K + 1) / 2 - 1 &&
+           size_t(E) * kSlots + early_stash_slots(E) <= size_t((K + 1) / 2 - 1) * kSlots;
+  }
+};
 
 namespace bulk {
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -72,24 +89,20 @@ __device__ __forceinline__ void copy_g2s(uint32_t dst, const void* src, uint32_t
 // closing step still read from the tile ((D+1)*E + D + m*D + 1 doubles per lane) is parked in the shared-memory slots
 // of state blocks that are already popped (blocks >= E), and the tile buffer is refilled with the next tile there and
 // then: E back-substitution + emission steps of lead for the fetch instead of one.  The host launches this
-// instantiation only when n_buffers == 1, both lanes own >= E vertices, and the parking area lies inside the state.
-template <int N, int D>
-__host__ __device__ constexpr int v5_early_stash_slots(int E) {
-  return (D + 1) * E + D + (N / 2 - 1) * D + 1;
-}
-
+// instantiation only when n_buffers == 1 and V5Layout::early_fits: both lanes own >= E vertices and the parking area
+// lies inside the state.
 template <int N, int R, int D, int MINB, bool FUSED = false, int EARLY = 0>
 __global__ void __launch_bounds__(kTmemThreads, MINB)
     twisted_tmem_v5_kernel(const WaypointParams prm, const TmemLaunchV5 tl, const __grid_constant__ CUtensorMap tmap) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
-  constexpr int kL = m * (m + 1) / 2;
-  constexpr int kSlots = kL + m * D;  // no positions in the state: the input tile stays resident for the whole tile
+  using Lay = V5Layout<N, D, FUSED>;
+  constexpr int kSlots = Lay::kSlots;
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
-  constexpr double kTiny = 0x1p-600, kHuge = 0x1p+600;
   using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
+  using S = sweep::Sweep<N, D, G>;
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -103,34 +116,21 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   const int nbuf = tl.n_buffers;
 
   double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);
-  unsigned char* after_stage = smem_raw + size_t(kWarps) * tmem_stage_bytes_per_warp<N, D>();
+  unsigned char* after_stage = smem_raw + tmem_stage_bytes<N, D>();
   const uint32_t bar0 = smem_u32(after_stage) + uint32_t(warp) * 16;  // two 8-byte mbarriers per warp
   // FUSED (SURVEY.md 8f-1): the tile is the waypoint record positions[16][K+1][D]; segment times are computed from it
   // (estimateSegmentTimesNfabian) and kept in a small per-thread history for the outward sweep
-  const int tile_t = FUSED ? 0 : 16 * K, tile_f = FUSED ? 16 * (K + 1) * D : 16 * D * nf, tile_doubles = tile_t + tile_f;
-  double* tiles = reinterpret_cast<double*>(after_stage + 128) + size_t(warp) * nbuf * tile_doubles;
+  const int tile_t = int(Lay::tile_times(K)), tile_f = int(Lay::tile_fixed(K, nf)), tile_doubles = tile_t + tile_f;
+  double* tiles = reinterpret_cast<double*>(after_stage + Lay::kBarBytes) + size_t(warp) * nbuf * tile_doubles;
   // sweep state: state double s (block * kSlots + slot) of this thread at state[s * kTmemThreads]
-  double* state = reinterpret_cast<double*>(after_stage + 128) + size_t(kWarps) * nbuf * tile_doubles + threadIdx.x;
+  double* state =
+      reinterpret_cast<double*>(after_stage + Lay::kBarBytes) + size_t(kWarps) * nbuf * tile_doubles + threadIdx.x;
   double* thist = nullptr;  // FUSED only: behind the sweep state
-  if constexpr (FUSED) thist = state + size_t(nmax) * kSlots * kTmemThreads;
+  if constexpr (FUSED) thist = state + Lay::hist(nmax) * kTmemThreads;
   auto TH = [&](int j) -> double& { return thist[size_t(j) * kTmemThreads]; };
   auto ST = [&](int s_global) -> double& { return state[size_t(s_global) * kTmemThreads]; };
-  auto put_state = [&](int blk, const double (&sv)[kSlots]) {
-#pragma unroll
-    for (int i = 0; i < kSlots; ++i) ST(blk * kSlots + i) = sv[i];
-  };
-  auto get_state = [&](int blk, double (&sv)[kSlots]) {
-#pragma unroll
-    for (int i = 0; i < kSlots; ++i) sv[i] = ST(blk * kSlots + i);
-  };
-
-  auto seg = [&](int j) -> int { return half ? K - 1 - j : j; };
-  auto pidx = [&](int v) -> int {
-    const int o = half ? K - v : v;
-    return o == 0 ? 0 : (o < K ? h + o - 1 : h + K - 1);
-  };
-  auto sgn = [&](int idx) -> double { return (half && !(idx & 1)) ? -1.0 : 1.0; };
-  const int e0 = half ? h + K : 1;
+  const sweep::Frame<N> fr{K, half};
+  const int e0 = fr.e0();
 
   const long long n_wtiles = prm.B >> 4;  // B is a multiple of 16 (host-checked)
   const long long wt_stride = (long long)gridDim.x * kWarps;
@@ -173,6 +173,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
   const int nhF = M - 1, nhB = K - M - 1;
   const int tl_row = lane >> 1;  // this lane's trajectory inside the tile
+  const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB};
 
   for (int it = 0; wt < n_wtiles; ++it) {
     const int buf = nbuf == 2 ? (it & 1) : 0;
@@ -193,74 +194,18 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     // time of own segment j: from the tile, or (FUSED) from the history filled by the inward sweep
     auto in_T = [&](int j) -> double {
       if constexpr (FUSED) return TH(j);
-      return tT[seg(j)];
+      return tT[fr.seg(j)];
     };
     auto in_x = [&](int v, int d) -> double {
-      if constexpr (FUSED) return tF[(half ? K - v : v) * D + d];
-      return tF[d * nf + pidx(v)];
+      if constexpr (FUSED) return tF[fr.vert(v) * D + d];
+      return tF[d * nf + fr.pidx(v)];
     };
     auto in_u0 = [&](int b, int d) -> double {  // fixed end derivative b+1 of own vertex 0, own-frame sign
       if constexpr (FUSED) return 0.0;
-      return sgn(b) * tF[d * nf + e0 + b];
+      return fr.sgn(b) * tF[d * nf + e0 + b];
     };
     const long long traj0 = wt * 16;
     const long long traj = traj0 + tl_row;
-
-    // emit own-frame segment j for every lane of the warp at once (convergent)
-    auto emit_all = [&](int j, int v_step, double T, double iT, const double (&sd)[h][D], const double (&ed)[h][D]) {
-      double tp[h], itp[h];
-      const double Ts = half ? -T : T;
-      tp[0] = 1.0;
-#pragma unroll
-      for (int k = 1; k < h; ++k) tp[k] = tp[k - 1] * Ts;
-      itp[0] = pow_int<h>(iT);
-#pragma unroll
-      for (int k = 1; k < h; ++k) itp[k] = itp[k - 1] * iT;
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double c[N], ss[h], se[h];
-#pragma unroll
-        for (int k = 0; k < h; ++k) {
-          const double s0 = half ? ed[k][d] : sd[k][d];
-          const double e0v = half ? sd[k][d] : ed[k][d];
-          c[k] = s0 * ((half && (k & 1)) ? -AI::at(k, k) : AI::at(k, k));
-          ss[k] = tp[k] * s0;
-          se[k] = tp[k] * e0v;
-        }
-        double ee[h];
-#pragma unroll
-        for (int k = 0; k < h; ++k) {
-          double acc = se[k] - ss[k];
-#pragma unroll
-          for (int j2 = k + 1; j2 < h; ++j2) {
-            constexpr double kInvFact[6] = {1.0, 1.0, 0.5, 1.0 / 6.0, 1.0 / 24.0, 1.0 / 120.0};
-            acc = (j2 - k == 1) ? acc - ss[j2] : fma(-kInvFact[j2 - k], ss[j2], acc);
-          }
-          ee[k] = acc;
-        }
-#pragma unroll
-        for (int q = 0; q < h; ++q) {
-          double acc = AI::at(h + q, h) * ee[0];
-#pragma unroll
-          for (int k = 1; k < h; ++k) acc = fma(AI::at(h + q, h + k), ee[k], acc);
-          c[h + q] = acc * itp[q];
-        }
-        if (d == 0) {  // the TMA must have finished reading the previous segment's tile
-          if (lane == 0) bulk_wait_read();
-          __syncwarp();
-        }
-#pragma unroll
-        for (int q = 0; q < h; ++q) my_row[d * h + q] = make_double2(c[2 * q], c[2 * q + 1]);
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        if (v_step <= nhF) tma_store_box(&tmap, stage, j * (D * N), (int)traj0);
-        if (v_step <= nhB) tma_store_box(&tmap, stage + 16 * (D * h), (K - 1 - j) * (D * N), (int)traj0);
-        bulk_commit();
-      }
-    };
-
 
     int stat = 0;
     double Wp[m][m], yp[m][D], Cee[m][m], cps[m], cpe[m], xm[D], xc[D];
@@ -281,29 +226,8 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       const double iT0 = fast_rcp(T0);
       double pw[N - 1];
       segment_powers<N, R>(T0, iT0, pw);
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-#pragma unroll
-        for (int b = 0; b < m; ++b) {
-          Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-          Wp[a][b] = (a == b) ? kTiny : 0.0;
-        }
-        cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-        cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
-      }
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double u0[m];
-#pragma unroll
-        for (int b = 0; b < m; ++b) u0[b] = in_u0(b, d);
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-          double acc = 0.0;
-#pragma unroll
-          for (int b = 0; b < m; ++b) acc = fma(pw[a + b + 2] * G::at(h + 1 + a, 1 + b), u0[b], acc);
-          yp[a][d] = acc * kHuge;
-        }
-      }
+      S::end_blocks(pw, Cee, cps, cpe);
+      S::carry_fold(pw, in_u0, Wp, yp);
     }
 
     // ---------------------------------------------------------------- sweep towards the middle
@@ -325,86 +249,11 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         double pw[N - 1];
         segment_powers<N, R>(T, iT, pw);
 
-        double Dp[m][m], E[m][m], bb[m][D];
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-#pragma unroll
-          for (int b = 0; b <= a; ++b) {
-            double s = fma(pw[a + b + 2], G::at(1 + a, 1 + b), Cee[a][b]);
-#pragma unroll
-            for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-            Dp[a][b] = s;
-          }
-#pragma unroll
-          for (int b = 0; b < m; ++b) E[a][b] = pw[a + b + 2] * G::at(1 + a, h + 1 + b);
-          const double gmid = fma(pw[a + 1], G::at(1 + a, 0), cpe[a]);
-          const double gnext = pw[a + 1] * G::at(1 + a, h);
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-            double s = -cps[a] * xm[d];
-            s = fma(-gmid, xc[d], s);
-            s = fma(-gnext, xn[d], s);
-#pragma unroll
-            for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-            bb[a][d] = s;
-          }
-        }
-        double L[m][m], inv[m];
-#pragma unroll
-        for (int j = 0; j < m; ++j) {
-          double s = Dp[j][j];
-#pragma unroll
-          for (int k = 0; k < j; ++k) s = fma(-L[j][k], L[j][k], s);
-          if (!(s > 0.0)) stat |= kStatusNotSpd;
-          inv[j] = fast_rsqrt(s);
-#pragma unroll
-          for (int i = j + 1; i < m; ++i) {
-            double t = Dp[i][j];
-#pragma unroll
-            for (int k = 0; k < j; ++k) t = fma(-L[i][k], L[j][k], t);
-            L[i][j] = t * inv[j];
-          }
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-#pragma unroll
-          for (int j = 0; j < m; ++j) {
-            double s = bb[j][d];
-#pragma unroll
-            for (int k = 0; k < j; ++k) s = fma(-L[j][k], yp[k][d], s);
-            yp[j][d] = s * inv[j];
-          }
-        }
-#pragma unroll
-        for (int c = 0; c < m; ++c) {
-#pragma unroll
-          for (int j = 0; j < m; ++j) {
-            double s = E[j][c];
-#pragma unroll
-            for (int k = 0; k < j; ++k) s = fma(-L[j][k], Wp[k][c], s);
-            Wp[j][c] = s * inv[j];
-          }
-        }
-        {
-          int slot = 0;
-#pragma unroll
-          for (int i = 1; i < m; ++i)
-#pragma unroll
-            for (int j = 0; j < i; ++j) sv[slot++] = L[i][j];
-#pragma unroll
-          for (int j = 0; j < m; ++j) sv[slot++] = inv[j];
-#pragma unroll
-          for (int j = 0; j < m; ++j)
-#pragma unroll
-            for (int d = 0; d < D; ++d) sv[slot++] = yp[j][d];
-        }
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-#pragma unroll
-          for (int b = 0; b <= a; ++b) Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-          cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-          cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
-        }
+        double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
+        S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
+        S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
+        S::pack(L, inv, yp, nullptr, sv);
+        S::end_blocks(pw, Cee, cps, cpe);
 #pragma unroll
         for (int d = 0; d < D; ++d) {
           xm[d] = xc[d];
@@ -412,81 +261,14 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         }
       }
       __syncwarp();
-      put_state(v - 1, sv);
+#pragma unroll
+      for (int i = 0; i < kSlots; ++i) ST((v - 1) * kSlots + i) = sv[i];
     }
     __syncwarp();
 
     // ---------------------------------------------------------------- middle vertex
     double um[m][D];
-    {
-      double Dl[m][m], bl[m][D];
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-#pragma unroll
-        for (int b = 0; b <= a; ++b) {
-          double s = Cee[a][b];
-#pragma unroll
-          for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-          Dl[a][b] = s;
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          double s = -cps[a] * xm[d];
-          s = fma(-cpe[a], xc[d], s);
-#pragma unroll
-          for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-          bl[a][d] = s;
-        }
-      }
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-#pragma unroll
-        for (int b = 0; b <= a; ++b) {
-          const double o = __shfl_xor_sync(kFull, Dl[a][b], 1);
-          Dl[a][b] += ((a + b) & 1) ? -o : o;
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          const double o = __shfl_xor_sync(kFull, bl[a][d], 1);
-          bl[a][d] += (a & 1) ? o : -o;
-        }
-      }
-      stat |= __shfl_xor_sync(kFull, stat, 1);
-      double L[m][m], inv[m];
-#pragma unroll
-      for (int j = 0; j < m; ++j) {
-        double s = Dl[j][j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) s = fma(-L[j][k], L[j][k], s);
-        if (!(s > 0.0)) stat |= kStatusNotSpd;
-        inv[j] = fast_rsqrt(s);
-#pragma unroll
-        for (int i = j + 1; i < m; ++i) {
-          double t = Dl[i][j];
-#pragma unroll
-          for (int k = 0; k < j; ++k) t = fma(-L[i][k], L[j][k], t);
-          L[i][j] = t * inv[j];
-        }
-      }
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double y[m];
-#pragma unroll
-        for (int j = 0; j < m; ++j) {
-          double s = bl[j][d];
-#pragma unroll
-          for (int k = 0; k < j; ++k) s = fma(-L[j][k], y[k], s);
-          y[j] = s * inv[j];
-        }
-#pragma unroll
-        for (int j = m - 1; j >= 0; --j) {
-          double s = y[j];
-#pragma unroll
-          for (int k = j + 1; k < m; ++k) s = fma(-L[k][j], um[k][d], s);
-          um[j][d] = s * inv[j];
-        }
-      }
-    }
+    S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
     if (half == 0 && prm.status != nullptr) prm.status[traj] = stat;
 
     // ---------------------------------------------------------------- outward back-substitution
@@ -494,11 +276,11 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + traj * (long long)D * np : nullptr;
     auto store_free = [&](int v_own, const double (&u)[h][D]) {
       if (df != nullptr) {
-        const int vo = half ? K - v_own : v_own;
+        const int vo = fr.vert(v_own);
 #pragma unroll
         for (int d = 0; d < D; ++d)
 #pragma unroll
-          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = sgn(j) * u[1 + j][d];
+          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
       }
     };
 
@@ -520,30 +302,31 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
 #pragma unroll
           for (int u = EARLY; u >= 1; --u) {
 #pragma unroll
-            for (int d = 0; d < D; ++d) park((EARLY - u) * (D + 1) + d, in_x(u, d));
-            park((EARLY - u) * (D + 1) + D, in_T(u));
+            for (int d = 0; d < D; ++d) park(Lay::park_step(EARLY, u) + d, in_x(u, d));
+            park(Lay::park_step(EARLY, u) + D, in_T(u));
           }
 #pragma unroll
-          for (int d = 0; d < D; ++d) park(EARLY * (D + 1) + d, in_x(0, d));
+          for (int d = 0; d < D; ++d) park(Lay::park_x0(EARLY) + d, in_x(0, d));
 #pragma unroll
           for (int d = 0; d < D; ++d)
 #pragma unroll
-            for (int b = 0; b < m; ++b) park(EARLY * (D + 1) + D + d * m + b, in_u0(b, d));
-          park(EARLY * (D + 1) + D + m * D, in_T(0));
+            for (int b = 0; b < m; ++b) park(Lay::park_u0(EARLY) + d * m + b, in_u0(b, d));
+          park(Lay::park_T0(EARLY), in_T(0));
           fence_proxy_async();
           __syncwarp();
           if (wt_next < n_wtiles) fetch_tile(wt_next, 0);
         }
       }
       double sv[kSlots];
-      get_state(v - 1, sv);
+#pragma unroll
+      for (int i = 0; i < kSlots; ++i) sv[i] = ST((v - 1) * kSlots + i);
       const bool act = v <= nh;
       double T = 1.0, iT = 1.0;
       double sd[h][D];
       if (act) {
         double xv[D];
         if (EARLY > 0 && v <= EARLY) {
-          const int s0 = kStash0 + (EARLY - v) * (D + 1);
+          const int s0 = kStash0 + Lay::park_step(EARLY, v);
 #pragma unroll
           for (int d = 0; d < D; ++d) xv[d] = ST(s0 + d);
           T = ST(s0 + D);
@@ -553,62 +336,18 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
           T = in_T(v);
         }
         if constexpr (FUSED) {
-          if (prm.times_out != nullptr) prm.times_out[traj * K + seg(v)] = T;
+          if (prm.times_out != nullptr) prm.times_out[traj * K + fr.seg(v)] = T;
         }
         iT = fast_rcp(T);
         double pw[N - 1];
         segment_powers<N, R>(T, iT, pw);
         double tE[m][D];
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int a = 0; a < m; ++a) {
-            double s = 0.0;
-#pragma unroll
-            for (int b = 0; b < m; ++b) s = fma(pw[a + b + 2] * G::at(1 + a, h + 1 + b), ed[1 + b][d], s);
-            tE[a][d] = s;
-          }
-        double L[m][m], inv[m], rhs[m][D];
-        {
-          int slot = 0;
-#pragma unroll
-          for (int i = 1; i < m; ++i)
-#pragma unroll
-            for (int j = 0; j < i; ++j) L[i][j] = sv[slot++];
-#pragma unroll
-          for (int j = 0; j < m; ++j) inv[j] = sv[slot++];
-#pragma unroll
-          for (int j = 0; j < m; ++j)
-#pragma unroll
-            for (int d = 0; d < D; ++d) rhs[j][d] = sv[slot++];
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          double t[m];
-#pragma unroll
-          for (int j = 0; j < m; ++j) {
-            double s = tE[j][d];
-#pragma unroll
-            for (int k = 0; k < j; ++k) s = fma(-L[j][k], t[k], s);
-            t[j] = s * inv[j];
-            rhs[j][d] -= t[j];
-          }
-        }
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-#pragma unroll
-          for (int j = m - 1; j >= 0; --j) {
-            double s = rhs[j][d];
-#pragma unroll
-            for (int k = j + 1; k < m; ++k) s = fma(-L[k][j], sd[1 + k][d], s);
-            sd[1 + j][d] = s * inv[j];
-          }
-          sd[0][d] = xv[d];
-        }
+        S::couple(pw, ed, tE);
+        S::back_substitute(sv, tE, xv, sd);
         store_free(v, sd);
       }
       __syncwarp();
-      emit_all(v, v, T, iT, sd, ed);
+      out.emit(v, v, T, iT, sd, ed, traj0);
       if (act) {
 #pragma unroll
         for (int d = 0; d < D; ++d)
@@ -620,14 +359,13 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       double sd[h][D];
       double T;
       if constexpr (EARLY > 0) {
-        const int s0 = kStash0 + EARLY * (D + 1);
 #pragma unroll
         for (int d = 0; d < D; ++d) {
-          sd[0][d] = ST(s0 + d);
+          sd[0][d] = ST(kStash0 + Lay::park_x0(EARLY) + d);
 #pragma unroll
-          for (int b = 0; b < m; ++b) sd[1 + b][d] = ST(s0 + D + d * m + b);
+          for (int b = 0; b < m; ++b) sd[1 + b][d] = ST(kStash0 + Lay::park_u0(EARLY) + d * m + b);
         }
-        T = ST(s0 + D + m * D);
+        T = ST(kStash0 + Lay::park_T0(EARLY));
       } else {
 #pragma unroll
         for (int d = 0; d < D; ++d) {
@@ -638,7 +376,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         T = in_T(0);
       }
       if constexpr (FUSED) {
-        if (prm.times_out != nullptr) prm.times_out[traj * K + seg(0)] = T;
+        if (prm.times_out != nullptr) prm.times_out[traj * K + fr.seg(0)] = T;
       }
       const double iT = fast_rcp(T);
       if (EARLY == 0 && nbuf == 1) {
@@ -649,7 +387,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         if (wt_next < n_wtiles) fetch_tile(wt_next, 0);
       }
       __syncwarp();
-      emit_all(0, 0, T, iT, sd, ed);
+      out.emit(0, 0, T, iT, sd, ed, traj0);
     }
     wt = wt_next;
   }

@@ -28,7 +28,7 @@
 // (consecutive lanes -> consecutive 8-byte words).
 #pragma once
 
-#include "mtg_device.cuh"
+#include "mtg_sweep.cuh"
 
 namespace mtg {
 
@@ -80,25 +80,6 @@ __device__ __forceinline__ double nfabian_time(const double (&a)[D], const doubl
   const double ex = exp(__dmul_rn(__ddiv_rn(-distance, v_max), 2.0));
   const double fac = __dadd_rn(1.0, __dmul_rn(__ddiv_rn(__dmul_rn(magic, v_max), a_max), ex));
   return __dmul_rn(lead, fac);
-}
-
-template <int N, int D>
-__host__ __device__ constexpr int waypoint_state_slots() {
-  return (N / 2 - 1) * (N / 2) / 2 + (N / 2 - 1) * D;
-}
-
-template <int E>
-__device__ __forceinline__ double pow_int(double x) {
-  if constexpr (E == 0) {
-    return 1.0;
-  } else if constexpr (E == 1) {
-    return x;
-  } else if constexpr (E % 2 == 0) {
-    const double y = pow_int<E / 2>(x);
-    return y * y;
-  } else {
-    return pow_int<E - 1>(x) * x;
-  }
 }
 
 // pw[e] = T^(1-2R+e), e = 0..2m.
@@ -166,14 +147,14 @@ template <int N, int R, int D>
 __global__ void __launch_bounds__(32) waypoint_solve_kernel(const WaypointParams prm) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
-  constexpr int kL = m * (m + 1) / 2;  // strictly-lower entries of L_v + inverse pivots
-  constexpr int kSlots = kL + m * D;
+  constexpr int kSlots = sweep_state_slots<N, D>();
   using G = H1<N, R>;
+  using S = sweep::Sweep<N, D, G>;
 
   extern __shared__ double smem[];
   const int lane = threadIdx.x & 31;
   double* st = smem + size_t(threadIdx.x >> 5) * size_t(prm.K - 1) * kSlots * 32 + lane;
-  auto S = [&](int blk, int slot) -> double& { return st[(size_t(blk) * kSlots + slot) * 32]; };
+  auto SP = [&](int blk, int slot) -> double& { return st[(size_t(blk) * kSlots + slot) * 32]; };
 
   const int K = prm.K;
   const int nf = prm.n_fixed;
@@ -201,29 +182,10 @@ __global__ void __launch_bounds__(32) waypoint_solve_kernel(const WaypointParams
     const double iT0 = fast_rcp(T0);
     double pw[N - 1];
     segment_powers<N, R>(T0, iT0, pw);
-#pragma unroll
-    for (int a = 0; a < m; ++a) {
-#pragma unroll
-      for (int b = 0; b < m; ++b) {
-        Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-        Wp[a][b] = 0.0;
-      }
-      cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-      cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
-    }
+    S::end_blocks(pw, Cee, cps, cpe);
+    S::carry_bcar(pw, [&](int b, int d) { return __ldg(fx + d * nf + 1 + b); }, Wp, yp, bcar);
 #pragma unroll
     for (int d = 0; d < D; ++d) {
-      double u0[m];
-#pragma unroll
-      for (int b = 0; b < m; ++b) u0[b] = __ldg(fx + d * nf + 1 + b);
-#pragma unroll
-      for (int a = 0; a < m; ++a) {
-        double acc = 0.0;
-#pragma unroll
-        for (int b = 0; b < m; ++b) acc = fma(pw[a + b + 2] * G::at(h + 1 + a, 1 + b), u0[b], acc);
-        bcar[a][d] = -acc;
-        yp[a][d] = 0.0;
-      }
       xm[d] = __ldg(fx + d * nf);
       xc[d] = __ldg(fx + d * nf + pidx(1));
     }
@@ -240,32 +202,8 @@ __global__ void __launch_bounds__(32) waypoint_solve_kernel(const WaypointParams
 #pragma unroll
     for (int d = 0; d < D; ++d) xn[d] = __ldg(fx + d * nf + pn);
 
-    // D'_v (lower triangle), E_v, b'_v
     double Dp[m][m], E[m][m], bb[m][D];
-#pragma unroll
-    for (int a = 0; a < m; ++a) {
-#pragma unroll
-      for (int b = 0; b <= a; ++b) {
-        double s = fma(pw[a + b + 2], G::at(1 + a, 1 + b), Cee[a][b]);
-#pragma unroll
-        for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], Wp[k][b], s);
-        Dp[a][b] = s;
-      }
-#pragma unroll
-      for (int b = 0; b < m; ++b) E[a][b] = pw[a + b + 2] * G::at(1 + a, h + 1 + b);
-      const double gmid = fma(pw[a + 1], G::at(1 + a, 0), cpe[a]);
-      const double gnext = pw[a + 1] * G::at(1 + a, h);
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double s = bcar[a][d];
-        s = fma(-cps[a], xm[d], s);
-        s = fma(-gmid, xc[d], s);
-        s = fma(-gnext, xn[d], s);
-#pragma unroll
-        for (int k = 0; k < m; ++k) s = fma(-Wp[k][a], yp[k][d], s);
-        bb[a][d] = s;
-      }
-    }
+    S::assemble(pw, Cee, cps, cpe, bcar, Wp, yp, xm, xc, xn, Dp, E, bb);
     if (v == K - 1) {  // last interior vertex: coupling to the fixed end derivatives u_K
 #pragma unroll
       for (int d = 0; d < D; ++d) {
@@ -282,68 +220,17 @@ __global__ void __launch_bounds__(32) waypoint_solve_kernel(const WaypointParams
       }
     }
 
-    // Cholesky of the m x m block: L strictly lower + inverse pivots.
-    double L[m][m], inv[m];
+    double L[m][m], inv[m], sv[kSlots];
+    S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
+    S::pack(L, inv, yp, nullptr, sv);
 #pragma unroll
-    for (int j = 0; j < m; ++j) {
-      double s = Dp[j][j];
-#pragma unroll
-      for (int k = 0; k < j; ++k) s = fma(-L[j][k], L[j][k], s);
-      if (!(s > 0.0)) stat |= kStatusNotSpd;
-      inv[j] = fast_rsqrt(s);
-#pragma unroll
-      for (int i = j + 1; i < m; ++i) {
-        double t = Dp[i][j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) t = fma(-L[i][k], L[j][k], t);
-        L[i][j] = t * inv[j];
-      }
-    }
-    // y_v = L^-1 b'_v ; W_v = L^-1 E_v
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-#pragma unroll
-      for (int j = 0; j < m; ++j) {
-        double s = bb[j][d];
-#pragma unroll
-        for (int k = 0; k < j; ++k) s = fma(-L[j][k], yp[k][d], s);
-        yp[j][d] = s * inv[j];
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < m; ++c) {
-#pragma unroll
-      for (int j = 0; j < m; ++j) {
-        double s = E[j][c];
-#pragma unroll
-        for (int k = 0; k < j; ++k) s = fma(-L[j][k], Wp[k][c], s);
-        Wp[j][c] = s * inv[j];
-      }
-    }
-    // store the sweep state of this vertex
-    {
-      int slot = 0;
-#pragma unroll
-      for (int i = 1; i < m; ++i)
-#pragma unroll
-        for (int j = 0; j < i; ++j) S(v - 1, slot++) = L[i][j];
-#pragma unroll
-      for (int j = 0; j < m; ++j) S(v - 1, slot++) = inv[j];
-#pragma unroll
-      for (int j = 0; j < m; ++j)
-#pragma unroll
-        for (int d = 0; d < D; ++d) S(v - 1, slot++) = yp[j][d];
-    }
+    for (int i = 0; i < kSlots; ++i) SP(v - 1, i) = sv[i];
     // carry the end-side blocks of segment v to the next vertex
+    S::end_blocks(pw, Cee, cps, cpe);
 #pragma unroll
-    for (int a = 0; a < m; ++a) {
-#pragma unroll
-      for (int b = 0; b <= a; ++b) Cee[a][b] = pw[a + b + 2] * G::at(h + 1 + a, h + 1 + b);
-      cps[a] = pw[a + 1] * G::at(h + 1 + a, 0);
-      cpe[a] = pw[a + 1] * G::at(h + 1 + a, h);
+    for (int a = 0; a < m; ++a)
 #pragma unroll
       for (int d = 0; d < D; ++d) bcar[a][d] = 0.0;
-    }
 #pragma unroll
     for (int d = 0; d < D; ++d) {
       xm[d] = xc[d];
@@ -367,55 +254,19 @@ __global__ void __launch_bounds__(32) waypoint_solve_kernel(const WaypointParams
   for (int v = K - 1; v >= 1; --v) {
     const double T = __ldg(tt + v);
     const double iT = fast_rcp(T);
-    double L[m][m], inv[m], rhs[m][D];
-    {
-      int slot = 0;
+    double sv[kSlots], L[m][m], inv[m], rhs[m][D];
 #pragma unroll
-      for (int i = 1; i < m; ++i)
-#pragma unroll
-        for (int j = 0; j < i; ++j) L[i][j] = S(v - 1, slot++);
-#pragma unroll
-      for (int j = 0; j < m; ++j) inv[j] = S(v - 1, slot++);
-#pragma unroll
-      for (int j = 0; j < m; ++j)
-#pragma unroll
-        for (int d = 0; d < D; ++d) rhs[j][d] = S(v - 1, slot++);
-    }
-    if (v < K - 1) {
+    for (int i = 0; i < kSlots; ++i) sv[i] = SP(v - 1, i);
+    S::unpack(sv, L, inv, rhs);
+    if (v < K - 1) {  // the last interior vertex's coupling to u_K is already in its right-hand side
       double pw[N - 1];
       segment_powers<N, R>(T, iT, pw);
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        double t[m];
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-          double s = 0.0;
-#pragma unroll
-          for (int b = 0; b < m; ++b) s = fma(pw[a + b + 2] * G::at(1 + a, h + 1 + b), ed[1 + b][d], s);
-          t[a] = s;
-        }
-#pragma unroll
-        for (int j = 0; j < m; ++j) {  // t = L^-1 t
-          double s = t[j];
-#pragma unroll
-          for (int k = 0; k < j; ++k) s = fma(-L[j][k], t[k], s);
-          t[j] = s * inv[j];
-          rhs[j][d] -= t[j];
-        }
-      }
+      S::uncouple_from(pw, ed, L, inv, rhs);
     }
-    double sd[h][D];
+    double xv[D], sd[h][D];
 #pragma unroll
-    for (int d = 0; d < D; ++d) {
-#pragma unroll
-      for (int j = m - 1; j >= 0; --j) {  // u = L^-T rhs
-        double s = rhs[j][d];
-#pragma unroll
-        for (int k = j + 1; k < m; ++k) s = fma(-L[k][j], sd[1 + k][d], s);
-        sd[1 + j][d] = s * inv[j];
-      }
-      sd[0][d] = __ldg(fx + d * nf + pidx(v));
-    }
+    for (int d = 0; d < D; ++d) xv[d] = __ldg(fx + d * nf + pidx(v));
+    S::solve_back(L, inv, rhs, xv, sd);
     if (prm.dfree != nullptr && valid) {
       double* __restrict__ df = prm.dfree + traj * (long long)D * np;
 #pragma unroll
