@@ -99,14 +99,16 @@ int mtg_device_is_sm90(const mtg_handle* h);
  *                             1 = one thread per trajectory, 2 = twisted (state in shared memory),
  *                             3 = twisted with the sweep state in shared memory + TMA tensor stores,
  *                             4 = persistent version of 3 with deep input prefetch,
- *                             5 = chunked (checkpoint + recompute) kernel, any K (default for K too large for 3),
+ *                             5 = chunked kernel (outer sweep blocks parked in global memory), any K (default for
+ *                                 K too large for 3),
  *                             6 = 4 with the inputs moved by TMA bulk copies (B % 16 == 0, 16-byte aligned inputs, K
  *                                 small enough for an input tile beside the state: K <= 16 at N = 10, D = 3). */
 #define MTG_OPT_WAYPOINT_VARIANT 1
 #define MTG_OPT_RING_DEPTH 2      /* reserved (the persistent kernel is built with a 3-deep input ring) */
 #define MTG_OPT_CTAS_PER_SM 3     /* variant 4 only: cap on resident CTAs per SM, 0 = as many as fit, 9 = one CTA per tile */
 #define MTG_OPT_STAGGER_US 4      /* reserved (accepted, no effect: the start-time stagger experiment was removed, DESIGN.md 4) */
-#define MTG_OPT_CHUNK_BLOCKS 6    /* chunked (large-K) kernel: resident vertex blocks per lane, 0 = auto */
+#define MTG_OPT_CHUNK_BLOCKS 6    /* chunked (large-K) kernel: vertex blocks per lane kept in shared memory (the
+                                     outer ones are parked in global memory), 0 = auto */
 #define MTG_OPT_GENERIC_VARIANT 7 /* arbitrary masks: 0 = masked block kernel (default), 1 = banded kernel in global scratch */
 #define MTG_OPT_MELLINGER_UNFUSED 8 /* 1 = batched Mellinger gradient through expand + solve + cost kernels */
 #define MTG_OPT_TMA_INPUTS 9      /* 0 = never, 1 = the TMA-input kernel (v5) where two input tiles fit (double buffered),

@@ -185,14 +185,14 @@ struct WaypointEntry {
   size_t (*tmem_smem)(int K);  // dynamic shared memory of fn_tmem / fn_tmem_fused (mtg::V3Layout)
   void (*fn_chunked)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap);  // any K (K3)
   size_t (*chunked_smem)(int C);  // dynamic shared memory of fn_chunked with C resident blocks (mtg::ChunkedLayout)
-  int chunked_ckpt_slots;         // doubles per thread of one global checkpoint of fn_chunked
+  int chunked_park_slots;         // doubles per thread of one vertex block that fn_chunked parks in global memory
 };
 #define MTG_WP_(N_, R_, D_, V1_)                                                                                  \
   {                                                                                                               \
     N_, R_, D_, mtg::sweep_state_slots<N_, D_>(), V1_, mtg::twisted_solve_kernel<N_, R_, D_>,                     \
         mtg::twisted_tmem_kernel<N_, R_, D_>, mtg::twisted_tmem_kernel<N_, R_, D_, true>,                         \
         mtg::V3Layout<N_, D_>::bytes, mtg::twisted_chunked_kernel<N_, R_, D_, kRingDepth>,                        \
-        mtg::ChunkedLayout<N_, D_, kRingDepth>::bytes, mtg::ChunkedLayout<N_, D_, kRingDepth>::kCkpt              \
+        mtg::ChunkedLayout<N_, D_, kRingDepth>::bytes, mtg::ChunkedLayout<N_, D_, kRingDepth>::kPark              \
   }
 #define MTG_WP(N_, R_, D_) MTG_WP_(N_, R_, D_, (mtg::waypoint_solve_kernel<N_, R_, D_>))
 // v1 (thread per trajectory) is kept for the headline shapes only (cross-check / profiles)
@@ -440,28 +440,28 @@ int resident_ctas(mtg_handle* h, const void* fn, size_t smem, int cap, int* ctas
   return MTG_OK;
 }
 
-// K3: the chunked (checkpoint + recompute) twisted kernel -- any K, fixed on-chip footprint.
+// K3: the chunked twisted kernel -- any K, fixed on-chip footprint; the vertex blocks beyond the C resident ones
+// are parked in global memory.
 int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, const mtg::WaypointParams& prm,
                    double* coeffs, int64_t B, cudaStream_t stream, int slot) {
   const int nmax = (p->K + 1) / 2 - 1;
   int best_ctas = 0, best_C = 0;
   size_t best_smem = 0;
-  const int cmax = std::max(1, std::min(nmax, 24));
-  for (int C = cmax; C >= 1; --C) {
+  // Auto: the largest chunk up to kAutoChunk that fits.  Measured on H100 at N = 10, D = 3 (K = 16, 50, 100): C = 3
+  // at one CTA per SM runs 20-35 % faster than C = 2 at two CTAs per SM -- the second CTA's warps hide less than
+  // its doubled parking area and halved L1 cost -- and C = 4 is level with C = 3, while C = 5 and 6 lose again as
+  // shared memory crowds out L1.
+  constexpr int kAutoChunk = 3;
+  const int cmax = std::max(1, std::min(nmax, h->chunk_blocks > 0 ? 24 : kAutoChunk));
+  for (int C = cmax; C >= 1 && best_ctas == 0; --C) {
     if (h->chunk_blocks > 0 && C != std::min(h->chunk_blocks, cmax)) continue;
     const size_t smem = e->chunked_smem(C);
     int ctas = 0;
     const int rc_ctas = resident_ctas(h, (const void*)e->fn_chunked, smem, 8, &ctas);
     if (rc_ctas != MTG_OK) return rc_ctas;
-    // More resident CTAs first; then a single round (C >= nmax) wins over recomputation; then the larger chunk.
-    const bool single = C >= nmax, best_single = best_C >= nmax && best_C > 0;
-    bool better = ctas > best_ctas;
-    if (ctas == best_ctas && ctas > 0) better = single != best_single ? single : C > best_C;
-    if (better) {
-      best_ctas = ctas;
-      best_C = C;
-      best_smem = smem;
-    }
+    best_ctas = ctas;
+    best_C = C;
+    best_smem = smem;
   }
   if (best_ctas == 0) {
     h->error = "chunked kernel: no launch configuration fits";
@@ -469,21 +469,21 @@ int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, 
   }
   const int64_t ctiles = (B + 63) / 64;
   const int64_t blocks = std::min<int64_t>(ctiles, int64_t(best_ctas) * h->sm_count);
-  const int nc = nmax > 0 ? (nmax + best_C - 1) / best_C : 1;
+  const int npark = nmax - best_C;  // parked vertex blocks per lane
   mtg::ChunkedLaunch cl;
   cl.chunk = best_C;
   cl.ckpt = nullptr;
   mtg_handle::Arena& ar = h->scratch[slot];
-  if (nc > 1) {
-    const size_t bytes = size_t(nc - 1) * e->chunked_ckpt_slots * size_t(blocks) * mtg::kTmemThreads * sizeof(double);
+  if (npark > 0) {
+    const size_t bytes = size_t(npark) * e->chunked_park_slots * size_t(blocks) * mtg::kTmemThreads * sizeof(double);
     const int rc = arena_acquire(h, ar, bytes, stream);
     if (rc != MTG_OK) return rc;
     cl.ckpt = ar.p;
   }
   {
-        const int rc_smem = ensure_dyn_smem(h, (const void*)e->fn_chunked, size_t(best_smem));
-        if (rc_smem != MTG_OK) return rc_smem;
-      }
+    const int rc_smem = ensure_dyn_smem(h, (const void*)e->fn_chunked, size_t(best_smem));
+    if (rc_smem != MTG_OK) return rc_smem;
+  }
   CUtensorMap tmap;
   {
     const int rc = encode_coeff_tmap(h, &tmap, coeffs, B, p);
@@ -492,7 +492,7 @@ int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, 
   e->fn_chunked<<<(unsigned)blocks, mtg::kTmemThreads, best_smem, stream>>>(prm, cl, tmap);
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
-  if (nc > 1) return arena_release(h, ar, stream);
+  if (npark > 0) return arena_release(h, ar, stream);
   return MTG_OK;
 }
 

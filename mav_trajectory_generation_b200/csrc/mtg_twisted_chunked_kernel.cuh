@@ -4,21 +4,24 @@
 //
 // The resident kernels keep the factor of every eliminated vertex in shared memory, which caps the number of
 // trajectories in flight per SM as K grows (25 doubles per lane and eliminated vertex at N = 10, D = 3).  Here
-// only a CHUNK of C vertex blocks per lane is ever resident -- the host picks C for the most resident CTAs per
-// SM -- and the rest is RECOMPUTED (checkpointing):
+// only the C innermost vertex blocks of a lane stay in shared memory -- the host picks C for the most resident CTAs
+// per SM -- and the outer ones are PARKED in global memory.  One pass per tile:
 //
-//   round 0   forward sweep over all own vertices 1..n (n = ceil(K/2)-1); only the innermost chunk (n-C, n] is
-//             stored; the loop-carried state (W, y: m*m + m*D doubles) is checkpointed to global memory at the
-//             start of every other chunk; middle vertex; back-substitution + emission over the innermost chunk;
-//   round j   (j = 1 .. nc-1, moving outwards) reload the checkpoint at the chunk's start, re-run the forward
-//             sweep over its <= C vertices storing their blocks on chip, back-substitute and emit them.
+//   forward   sweep over all own vertices 1..n (n = ceil(K/2)-1); the block of vertex v <= n-C (its pack() slots
+//             and the step's segment time) goes to the parking area, the innermost C blocks to shared slot
+//             (v-1) % C; then the middle vertex;
+//   outward   back-substitution + emission v = n..1 from the shared slots; once vertex v is back-substituted, its
+//             slot is refilled by cp.async with parked block v-C, which therefore has C-1 outward steps (and v's
+//             emission) to land.
 //
-// Cost: the forward sweep runs (2n - C)/n times (1.35x of all FP64 work at K = 50, 1.43x at K = 100); extra HBM
-// traffic 2 * (nc-1) * (m*m + m*D) * 8 bytes per lane for the checkpoints (+24 % at K = 100) and one re-read of
-// the inputs -- against 2.2x the algorithmic traffic if the whole factor were spilled to HBM.
-// CTAs are persistent (static tile assignment) so that the checkpoint area is bounded by the number of resident
-// threads, not by the batch.  Arithmetic per vertex is exactly the v3/v4 sequence: results are bitwise equal to
-// the resident kernels where both run (tests force tiny chunks on K = 16 to prove it).
+// Cost: no recomputation -- every vertex is factorised once, as in the resident kernels.  Extra global traffic
+// 2 * (n-C) * (kSlots+1) * 8 bytes per lane (written once, read once); CTAs are persistent (static tile
+// assignment), so the parking area is bounded by the number of resident threads, not by the batch (about 1 KB per
+// thread at K = 16, C = 3: it stays in L2; at K = 50 it spills to HBM).  Every thread owns one column of it,
+// laid out [block][slot][thread] so that a warp stores or loads one slot as 256 contiguous bytes.  As in v4, the
+// next tile's prologue inputs are prefetched into the dead state region at the end of the outward sweep, and the
+// fixed end derivatives of the final emission into the idle input ring.  Arithmetic per vertex is exactly the
+// v4 sequence: results are bitwise equal to v4 and independent of C (tests force tiny chunks on K = 16 to prove it).
 #pragma once
 
 #include "mtg_twisted_tmem_v4_kernel.cuh"
@@ -27,26 +30,37 @@ namespace mtg {
 
 struct ChunkedLaunch {
   int chunk;          // C: vertex blocks resident per lane (in shared memory)
-  double* ckpt;       // [(nc-1)][m*m + m*D][gridDim.x * 128] loop-carried state at chunk starts
+  double* ckpt;       // parking area [n-C][kPark][gridDim.x * 128]: the outer vertex blocks of the sweep
 };
 
 // Dynamic shared memory of K3 behind the staging tiles, in per-thread slots:
-// [input ring RD x (1+D)][times C+1][stash D+1][restart 1+2D][state: C blocks with the vertex position]
+// [input ring RD x (1+D)][times C][stash D+1][region: C blocks with the vertex position, or the next tile's prologue]
 template <int N, int D, int RD>
 struct ChunkedLayout {
   static constexpr int kSlots = sweep_state_slots<N, D, true>();
-  static constexpr int kCkpt = (N / 2 - 1) * (N / 2 - 1) + (N / 2 - 1) * D;  // global checkpoint: W, y
-  static constexpr int kHist = RD * (1 + D);      // ring, then the times of the chunk
-  static constexpr int kStash = D + 1;             // x0[D], T0
-  static constexpr int kRestart = 1 + 2 * D;       // T of own segment lo, x_lo[D], x_{lo+1}[D]
-  __host__ __device__ static constexpr int hist_slots(int C) { return C + 1; }
+  static constexpr int kPark = kSlots + 1;                   // a parked block: pack() slots, then the segment time
+  static constexpr int kPro = 2 * D + (N / 2 - 1) * D + 1;  // x0, x1, u0[m], T0
+  static constexpr int kHist = RD * (1 + D);                 // ring, then the times of the resident blocks
+  static constexpr int kStash = D + 1;                       // x0[D], T0
+  __host__ __device__ static constexpr int hist_slots(int C) { return C; }
   __host__ __device__ static constexpr size_t stash(int C) { return size_t(kHist) + hist_slots(C); }
-  __host__ __device__ static constexpr size_t restart(int C) { return stash(C) + kStash; }
-  __host__ __device__ static constexpr size_t state(int C) { return restart(C) + kRestart; }
+  __host__ __device__ static constexpr size_t region(int C) { return stash(C) + kStash; }
+  __host__ __device__ static constexpr size_t region_slots(int C) {
+    return size_t(C) * kSlots > size_t(kPro) ? size_t(C) * kSlots : size_t(kPro);
+  }
   __host__ __device__ static constexpr size_t bytes(int C) {
-    return tmem_stage_bytes<N, D>() + tmem_slot_bytes(state(C) + size_t(C) * kSlots);
+    return tmem_stage_bytes<N, D>() + tmem_slot_bytes(region(C) + region_slots(C));
   }
 };
+
+// cp.async.wait_group with a run-time bound: waits until at most min(pending, 3) groups are in flight, which is at
+// least what `pending` asks for
+__device__ __forceinline__ void cp_async_wait_at_most(int pending) {
+  if (pending <= 0) cp_async_wait_group<0>();
+  else if (pending == 1) cp_async_wait_group<1>();
+  else if (pending == 2) cp_async_wait_group<2>();
+  else cp_async_wait_group<3>();
+}
 
 template <int N, int R, int D, int RD>
 __global__ void __launch_bounds__(kTmemThreads, 2)
@@ -55,8 +69,10 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   constexpr int m = h - 1;
   using Lay = ChunkedLayout<N, D, RD>;
   constexpr int kSlots = Lay::kSlots;
-  constexpr int kCk = Lay::kCkpt;
+  constexpr int kPark = Lay::kPark;
+  constexpr int kPro = Lay::kPro;
   constexpr int kWarps = kTmemThreads / 32;
+  static_assert(RD >= 2, "ring depth");
   using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
   using S = sweep::Sweep<N, D, G>;
@@ -71,18 +87,17 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   const int nh = half ? K - M - 1 : M - 1;
   const int n = M - 1;
   const int C = cl.chunk;
-  const int nc = n > 0 ? (n + C - 1) / C : 1;
+  const int npark = n - C;  // vertices 1..npark are parked (none when C >= n)
 
   double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);
   double* base = reinterpret_cast<double*>(smem_raw + tmem_stage_bytes<N, D>()) + threadIdx.x;
   auto PF = [&](int buf, int slot) -> double* { return base + (size_t(buf) * (1 + D) + slot) * kTmemThreads; };
   double* thist = base + size_t(Lay::kHist) * kTmemThreads;
-  auto HT = [&](int b) -> double& { return thist[size_t(b) * kTmemThreads]; };  // time of the step that made block b
+  auto HT = [&](int b) -> double* { return thist + size_t(b) * kTmemThreads; };  // time of the step that made block b
   double* stash = thist + size_t(Lay::hist_slots(C)) * kTmemThreads;  // x0[D], T0
-  double* restart = stash + size_t(Lay::kStash) * kTmemThreads;       // T of own segment lo, x_lo[D], x_{lo+1}[D]
-  double* state = restart + size_t(Lay::kRestart) * kTmemThreads;
-  auto SP = [&](int blk, int slot) -> double& { return state[(size_t(blk) * kSlots + slot) * kTmemThreads]; };
-  auto RS = [&](int slot) -> double* { return restart + size_t(slot) * kTmemThreads; };
+  double* region = stash + size_t(Lay::kStash) * kTmemThreads;        // state blocks; next tile's prologue inputs
+  auto SP = [&](int blk, int slot) -> double* { return region + (size_t(blk) * kSlots + slot) * kTmemThreads; };
+  auto PRO = [&](int slot) -> double* { return region + size_t(slot) * kTmemThreads; };
 
   const sweep::Frame<N> fr{K, half};
   const int e0 = fr.e0();
@@ -90,44 +105,143 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   const long long n_wtiles = (prm.B + 15) >> 4;
   const long long wt_stride = (long long)gridDim.x * kWarps;
   const long long gthreads = (long long)gridDim.x * kTmemThreads;
-  double* __restrict__ ck = cl.ckpt ? cl.ckpt + ((long long)blockIdx.x * kTmemThreads + threadIdx.x) : nullptr;
-  auto CK = [&](int j, int slot) -> double& { return ck[((long long)(j - 1) * kCk + slot) * gthreads]; };
+  double* __restrict__ pk = cl.ckpt ? cl.ckpt + ((long long)blockIdx.x * kTmemThreads + threadIdx.x) : nullptr;
+  auto PK = [&](int b, int slot) -> double* { return pk + ((long long)b * kPark + slot) * gthreads; };
+
+  // pointers of a warp tile's trajectory for this lane
+  struct Ptrs {
+    const double* tt;
+    const double* fx;
+    long long traj;
+    bool valid;
+  };
+  auto tile_ptrs = [&](long long w) -> Ptrs {
+    Ptrs p;
+    p.traj = w * 16 + (lane >> 1);
+    p.valid = p.traj < prm.B;
+    if (!p.valid) p.traj = prm.B - 1;
+    p.tt = prm.times + p.traj * K;
+    p.fx = prm.dfix + p.traj * (long long)D * nf;
+    return p;
+  };
+  auto xaddr = [&](const Ptrs& p, int v, int d) -> const double* { return p.fx + d * nf + fr.pidx(v); };
+  // a tile's prologue inputs -> PRO region (cp.async; the caller commits the group)
+  auto pro_issue = [&](const Ptrs& p) {
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+      cp_async8(PRO(d), xaddr(p, 0, d));
+      cp_async8(PRO(D + d), xaddr(p, 1, d));
+#pragma unroll
+      for (int b = 0; b < m; ++b) cp_async8(PRO(2 * D + b * D + d), p.fx + d * nf + e0 + b);
+    }
+    cp_async8(PRO(kPro - 1), p.tt + fr.seg(0));
+  };
+  // inputs of inward step v (time of own segment v, position of own vertex v+1) -> ring buffer v % RD
+  auto ring_issue = [&](const Ptrs& p, int v) {
+    const int j = v < K ? v : K - 1;
+    const int vn = v + 1 <= K ? v + 1 : K;
+    const int buf = v % RD;
+    cp_async8(PF(buf, 0), p.tt + fr.seg(j));
+#pragma unroll
+    for (int d = 0; d < D; ++d) cp_async8(PF(buf, 1 + d), xaddr(p, vn, d));
+  };
+
+  long long wt = (long long)blockIdx.x * kWarps + warp;
+  if (wt < n_wtiles) {
+    pro_issue(tile_ptrs(wt));
+    cp_async_commit();
+  }
 
   double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
   const int nhF = M - 1, nhB = K - M - 1;
   const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB};
 
-  for (long long wt = (long long)blockIdx.x * kWarps + warp; wt < n_wtiles; wt += wt_stride) {
-    long long traj = wt * 16 + (lane >> 1);
+  for (; wt < n_wtiles; wt += wt_stride) {
+    const long long wt_next = wt + wt_stride;  // its prologue is prefetched at the end of this tile
+    const Ptrs P = tile_ptrs(wt);
     const long long traj0 = wt * 16;
-    const bool valid = traj < prm.B;
-    if (!valid) traj = prm.B - 1;
-    const double* __restrict__ tt = prm.times + traj * K;
-    const double* __restrict__ fx = prm.dfix + traj * (long long)D * nf;
-    auto xaddr = [&](int v, int d) -> const double* { return fx + d * nf + fr.pidx(v); };
-    auto ring_issue = [&](int v) {
-      const int j = v < K ? v : K - 1;
-      const int vn = v + 1 <= K ? v + 1 : K;
-      const int buf = v % RD;
-      cp_async8(PF(buf, 0), tt + fr.seg(j));
+    const bool valid = P.valid;
+
+    // ---- ring prefetch of the first RD-1 inward steps, then consume the prologue inputs (issued a tile ago)
+    // (a group is committed for every step even when it is empty, so that wait_group<RD-2> always means "the data
+    // of the current step has landed")
 #pragma unroll
-      for (int d = 0; d < D; ++d) cp_async8(PF(buf, 1 + d), xaddr(vn, d));
-    };
-    // restart inputs of a chunk that starts after own step lo
-    auto restart_issue = [&](int lo) {
-      cp_async8(RS(0), tt + fr.seg(lo));
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        cp_async8(RS(1 + d), xaddr(lo, d));
-        cp_async8(RS(1 + D + d), xaddr(lo + 1, d));
-      }
-    };
+    for (int q = 1; q < RD; ++q) {
+      if (q <= nh) ring_issue(P, q);
+      cp_async_commit();
+    }
+    cp_async_wait_group<RD - 1>();
 
     int stat = 0;
     double Wp[m][m], yp[m][D], Cee[m][m], cps[m], cpe[m], xm[D], xc[D];
-    double ed[h][D];
+    {
+#pragma unroll
+      for (int d = 0; d < D; ++d) {
+        xm[d] = *PRO(d);
+        xc[d] = *PRO(D + d);
+        stash[size_t(d) * kTmemThreads] = xm[d];
+      }
+      const double T0 = *PRO(kPro - 1);
+      stash[size_t(D) * kTmemThreads] = T0;
+      if (!(T0 > 0.0)) stat |= kStatusBadTime;
+      const double iT0 = fast_rcp(T0);
+      double pw[N - 1];
+      segment_powers<N, R>(T0, iT0, pw);
+      S::end_blocks(pw, Cee, cps, cpe);
+      // initial carry from the fixed end derivatives (exact 2^+-600 scaling)
+      S::carry_fold(pw, [&](int b, int d) { return fr.sgn(b) * *PRO(2 * D + b * D + d); }, Wp, yp);
+    }
+
+    // ---------------------------------------------------------------- sweep towards the middle
+    for (int v = 1; v <= n; ++v) {
+      double sv[kSlots];
+      double T;
+      if (v <= nh) {
+        cp_async_wait_group<RD - 2>();
+        double xn[D];
+#pragma unroll
+        for (int d = 0; d < D; ++d) xn[d] = *PF(v % RD, 1 + d);
+        T = *PF(v % RD, 0);
+        if (v + RD - 1 <= nh) ring_issue(P, v + RD - 1);  // nothing is left in flight after the last own step
+        cp_async_commit();
+        if (!(T > 0.0)) stat |= kStatusBadTime;
+        const double iT = fast_rcp(T);
+        double pw[N - 1];
+        segment_powers<N, R>(T, iT, pw);
+
+        double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
+        S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
+        S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
+        S::pack(L, inv, yp, xc, sv);
+        S::end_blocks(pw, Cee, cps, cpe);
+#pragma unroll
+        for (int d = 0; d < D; ++d) {
+          xm[d] = xc[d];
+          xc[d] = xn[d];
+        }
+      }
+      __syncwarp();
+      if (v <= npark) {  // warp-uniform; every lane is active here (v < n <= nh + 1)
+#pragma unroll
+        for (int i = 0; i < kSlots; ++i) *PK(v - 1, i) = sv[i];
+        *PK(v - 1, kSlots) = T;
+      } else {
+        const int b = (v - 1) % C;
+        if (v <= nh) *HT(b) = T;
+#pragma unroll
+        for (int i = 0; i < kSlots; ++i) *SP(b, i) = sv[i];
+      }
+    }
+    __syncwarp();
+
+    // ---------------------------------------------------------------- middle vertex: both halves meet
+    double um[m][D];
+    S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
+    if (valid && half == 0 && prm.status != nullptr) prm.status[P.traj] = stat;
+
+    // ---------------------------------------------------------------- outward back-substitution
     const int np = (K - 1) * m;
-    double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + traj * (long long)D * np : nullptr;
+    double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + P.traj * (long long)D * np : nullptr;
     auto store_free = [&](int v_own, const double (&u)[h][D]) {
       if (df != nullptr && valid) {
         const int vo = fr.vert(v_own);
@@ -138,151 +252,89 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
       }
     };
 
-    for (int j = 0; j < nc; ++j) {
-      const int hi = n - j * C;
-      const int lo = hi - C > 0 ? hi - C : 0;
-      const int from = j == 0 ? 0 : lo;  // round 0 sweeps everything, storing only (lo, hi]
-
-      // ---- (re)start state: inputs through the restart slots, carry from the prologue (round 0) or checkpoint
-      restart_issue(from);
-      cp_async_commit();
+    double ed[h][D];
 #pragma unroll
-      for (int q = 1; q < RD; ++q) {
-        if (from + q <= nh && from + q <= hi) ring_issue(from + q);
+    for (int d = 0; d < D; ++d) {
+      ed[0][d] = xc[d];
+#pragma unroll
+      for (int j = 0; j < m; ++j) ed[1 + j][d] = um[j][d];
+    }
+    if (half == 0) store_free(nh + 1, ed);
+
+    // The ring is idle during the outward sweep: the fixed end derivatives needed by the final emission are
+    // fetched into it now (slot q of the flattened ring), many steps ahead of their use.
+    constexpr bool kEndInRing = RD * (1 + D) >= m * D;
+    if constexpr (kEndInRing) {
+#pragma unroll
+      for (int d = 0; d < D; ++d)
+#pragma unroll
+        for (int b = 0; b < m; ++b) cp_async8(base + size_t(b * D + d) * kTmemThreads, P.fx + d * nf + e0 + b);
+      cp_async_commit();
+    }
+    // the next tile's prologue inputs go to the state region: issued once every state block has been read back
+    auto issue_next_pro = [&]() {
+      if (wt_next < n_wtiles) {  // warp-uniform
+        pro_issue(tile_ptrs(wt_next));
         cp_async_commit();
       }
-      if (j > 0) {
-#pragma unroll
-        for (int a = 0; a < m; ++a) {
-#pragma unroll
-          for (int b = 0; b < m; ++b) Wp[a][b] = CK(j, a * m + b);
-#pragma unroll
-          for (int d = 0; d < D; ++d) yp[a][d] = CK(j, m * m + a * D + d);
-        }
-      }
-      cp_async_wait_group<RD - 1>();
-      {
-        const double Tp = *RS(0);
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          xm[d] = *RS(1 + d);
-          xc[d] = *RS(1 + D + d);
-        }
-        if (!(Tp > 0.0)) stat |= kStatusBadTime;
-        const double iTp = fast_rcp(Tp);
-        double pw[N - 1];
-        segment_powers<N, R>(Tp, iTp, pw);
-        S::end_blocks(pw, Cee, cps, cpe);
-        if (j == 0) {  // prologue of the tile: initial carry from the fixed end derivatives (exact 2^+-600 scaling)
-#pragma unroll
-          for (int d = 0; d < D; ++d) stash[size_t(d) * kTmemThreads] = xm[d];
-          stash[size_t(D) * kTmemThreads] = Tp;
-          S::carry_fold(pw, [&](int b, int d) { return fr.sgn(b) * __ldg(fx + d * nf + e0 + b); }, Wp, yp);
-        }
-      }
+    };
+    if (n == 0) issue_next_pro();
 
-      // ---- forward sweep over (from, hi]
-      for (int v = from + 1; v <= hi; ++v) {
-        if (j == 0 && nc > 1) {  // checkpoint the carry at the start of every outer chunk (warp-uniform test)
-          const int dist = n - (v - 1);
-          const bool at0 = (v - 1) == 0;
-          if (at0 || (dist % C == 0 && dist >= 2 * C)) {
-            const int jc = at0 ? nc - 1 : dist / C - 1;
+    for (int v = n; v >= 1; --v) {
+      const int b = (v - 1) % C;
+      // parked block v was refilled C steps ago; the C-1 refill groups committed since may stay in flight
+      if (v <= npark) cp_async_wait_at_most(C - 1);
+      const bool act = v <= nh;
+      const double T = act ? *HT(b) : 1.0;
+      const double iT = fast_rcp(T);
+      double pw[N - 1];
+      segment_powers<N, R>(T, iT, pw);
+      double sv[kSlots];
 #pragma unroll
-            for (int a = 0; a < m; ++a) {
+      for (int i = 0; i < kSlots; ++i) sv[i] = *SP(b, i);
+      double tE[m][D];  // E_v u_{v+1} (before the activity test: this kernel runs at the register limit)
+      S::couple(pw, ed, tE);
+      double sd[h][D];
+      if (act) {
+        double xv[D];
 #pragma unroll
-              for (int b = 0; b < m; ++b) CK(jc, a * m + b) = Wp[a][b];
-#pragma unroll
-              for (int d = 0; d < D; ++d) CK(jc, m * m + a * D + d) = yp[a][d];
-            }
-          }
-        }
-        const bool store = v > lo;
-        double sv[kSlots];
-        if (v <= nh) {
-          cp_async_wait_group<RD - 2>();
-          double xn[D];
-#pragma unroll
-          for (int d = 0; d < D; ++d) xn[d] = *PF(v % RD, 1 + d);
-          const double T = *PF(v % RD, 0);
-          if (store) HT(v - lo - 1) = T;
-          if (v + RD - 1 <= nh && v + RD - 1 <= hi) ring_issue(v + RD - 1);
-          cp_async_commit();
-          if (!(T > 0.0)) stat |= kStatusBadTime;
-          const double iT = fast_rcp(T);
-          double pw[N - 1];
-          segment_powers<N, R>(T, iT, pw);
-
-          double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
-          S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
-          S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
-          S::pack(L, inv, yp, xc, sv);
-          S::end_blocks(pw, Cee, cps, cpe);
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-            xm[d] = xc[d];
-            xc[d] = xn[d];
-          }
-        }
-        if (store) {  // warp-uniform
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < kSlots; ++i) SP(v - lo - 1, i) = sv[i];
-        }
+        for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
+        S::back_substitute(sv, tE, xv, sd);
+        store_free(v, sd);
       }
+      if (v - C >= 1) {  // warp-uniform: the freed slot takes parked block v-C
+#pragma unroll
+        for (int i = 0; i < kSlots; ++i) cp_async8(SP(b, i), PK(v - C - 1, i));
+        cp_async8(HT(b), PK(v - C - 1, kSlots));
+      }
+      cp_async_commit();
       __syncwarp();
-
-      // ---- middle vertex (round 0 only): both halves meet
-      if (j == 0) {
-        double um[m][D];
-        S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
+      out.emit(v, v, T, iT, sd, ed, traj0);
+      if (act) {
 #pragma unroll
-        for (int d = 0; d < D; ++d) {
-          ed[0][d] = xc[d];
+        for (int d = 0; d < D; ++d)
 #pragma unroll
-          for (int jj = 0; jj < m; ++jj) ed[1 + jj][d] = um[jj][d];
-        }
-        if (half == 0) store_free(nh + 1, ed);
-      }
-
-      // ---- back-substitution + emission over (lo, hi], outwards
-      for (int v = hi; v > lo; --v) {
-        const bool act = v <= nh;
-        const double T = act ? HT(v - lo - 1) : 1.0;
-        const double iT = fast_rcp(T);
-        double pw[N - 1];
-        segment_powers<N, R>(T, iT, pw);
-        double sv[kSlots];
-#pragma unroll
-        for (int i = 0; i < kSlots; ++i) sv[i] = SP(v - lo - 1, i);
-        double tE[m][D];  // E_v u_{v+1} (after the wait: this kernel runs at the register limit)
-        S::couple(pw, ed, tE);
-        double sd[h][D];
-        if (act) {
-          double xv[D];
-#pragma unroll
-          for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
-          S::back_substitute(sv, tE, xv, sd);
-          store_free(v, sd);
-        }
-        __syncwarp();
-        out.emit(v, v, T, iT, sd, ed, traj0);
-        if (act) {
-#pragma unroll
-          for (int d = 0; d < D; ++d)
-#pragma unroll
-            for (int k = 0; k < h; ++k) ed[k][d] = sd[k][d];
-        }
+          for (int k = 0; k < h; ++k) ed[k][d] = sd[k][d];
       }
     }
-    if (valid && half == 0 && prm.status != nullptr) prm.status[traj] = stat;
+    if (n > 0) issue_next_pro();  // the state region is dead only now
     {  // own segment 0: the fixed end vertex
       double sd[h][D];
+      if constexpr (kEndInRing) {
+        // everything except (possibly) the next tile's prologue group has landed
+        if (wt_next < n_wtiles) cp_async_wait_group<1>(); else cp_async_wait_group<0>();
+      }
 #pragma unroll
       for (int d = 0; d < D; ++d) {
         sd[0][d] = stash[size_t(d) * kTmemThreads];
 #pragma unroll
-        for (int b = 0; b < m; ++b) sd[1 + b][d] = fr.sgn(b) * __ldg(fx + d * nf + e0 + b);
+        for (int b = 0; b < m; ++b) {
+          if constexpr (kEndInRing) {
+            sd[1 + b][d] = fr.sgn(b) * base[size_t(b * D + d) * kTmemThreads];
+          } else {
+            sd[1 + b][d] = fr.sgn(b) * __ldg(P.fx + d * nf + e0 + b);
+          }
+        }
       }
       const double T = stash[size_t(D) * kTmemThreads];
       const double iT = fast_rcp(T);
