@@ -105,7 +105,8 @@ int mtg_device_is_sm90(const mtg_handle* h);
  *                                 small enough for an input tile beside the state: K <= 16 at N = 10, D = 3). */
 #define MTG_OPT_WAYPOINT_VARIANT 1
 #define MTG_OPT_RING_DEPTH 2      /* reserved (the persistent kernel is built with a 3-deep input ring) */
-#define MTG_OPT_CTAS_PER_SM 3     /* variant 4 only: cap on resident CTAs per SM, 0 = as many as fit, 9 = one CTA per tile */
+#define MTG_OPT_CTAS_PER_SM 3     /* variant 4: cap on resident CTAs per SM, 0 = as many as fit, 9 = one CTA per tile;
+                                     chunked kernel: cap on resident warps per SM, 0 = as many as fit */
 #define MTG_OPT_STAGGER_US 4      /* reserved (accepted, no effect: the start-time stagger experiment was removed, DESIGN.md 4) */
 #define MTG_OPT_CHUNK_BLOCKS 6    /* chunked (large-K) kernel: vertex blocks per lane kept in shared memory (the
                                      outer ones are parked in global memory), 0 = auto */
@@ -115,6 +116,10 @@ int mtg_device_is_sm90(const mtg_handle* h);
                                     2 (default) = also where only one fits (single buffered) */
 #define MTG_OPT_EARLY_REFILL 10   /* TMA-input kernel with one tile buffer: 0 = the buffer is refilled with the next tile two
                                    * outward-sweep steps before the tile ends (default), -1 = while the last segment is emitted */
+#define MTG_OPT_CHUNK_WARPS 11    /* chunked kernel: warps per CTA, 1 or 4, 0 = auto (1: shared memory is allocated per warp,
+                                     so more warps fit per SM) */
+#define MTG_OPT_L2_HINTS 12       /* chunked kernel: 0 = no cache hints (default), 1 = inputs and coefficient stores marked
+                                     evict-first in L2 (meant to keep the parked blocks there; measured slower on H100) */
 #define MTG_OPT_DYNAMIC_TILES 5   /* persistent kernel: warps draw tiles from a global counter: 0 = auto, 1 = always, 2 = never */
 int mtg_set_option(mtg_handle* h, int key, int value);
 

@@ -51,12 +51,15 @@ struct mtg_handle {
   int waypoint_variant = 0;  // MTG_OPT_WAYPOINT_VARIANT
   int ring_depth = 3;        // MTG_OPT_RING_DEPTH (v4 kernel: cp.async input ring buffers, 2..4)
   int early_steps = 0;       // MTG_OPT_EARLY_REFILL (v5, single tile buffer): 0 = on (kV5Early steps of lead), -1 = off
-  int ctas_per_sm = 0;       // MTG_OPT_CTAS_PER_SM (v4 kernel: 0 = as many as fit, 9 = one CTA per tile, not persistent)
+  int ctas_per_sm = 0;       // MTG_OPT_CTAS_PER_SM (v4 kernel: 0 = as many as fit, 9 = one CTA per tile, not persistent;
+                             // chunked kernel: cap on resident warps per SM)
   int stagger_us = 0;        // MTG_OPT_STAGGER_US (v4 kernel: CTA start times spread over this many microseconds)
   int tma_inputs = 2;        // MTG_OPT_TMA_INPUTS (default routing prefers the TMA-input kernel v5 when eligible)
   int mellinger_unfused = 0; // MTG_OPT_MELLINGER_UNFUSED (1 = expand + solve + cost kernels, the round-1 path)
   int generic_variant = 0;   // MTG_OPT_GENERIC_VARIANT (0 = masked block kernel, 1 = banded kernel in global scratch)
   int chunk_blocks = 0;      // MTG_OPT_CHUNK_BLOCKS (chunked kernel: resident vertex blocks per lane, 0 = auto)
+  int chunk_warps = 0;       // MTG_OPT_CHUNK_WARPS (chunked kernel: warps per CTA, 1 or 4; 0 = auto)
+  int l2_hints = 0;          // MTG_OPT_L2_HINTS (chunked kernel: 0 = no cache hints, 1 = streamed data evict-first in L2)
   int dynamic_tiles = 0;     // MTG_OPT_DYNAMIC_TILES (v4 kernel: warps draw tiles from a global counter)
   std::vector<CachedTopology> topologies;
   // host-pointer pipeline
@@ -87,6 +90,16 @@ struct mtg_handle {
   // remember the largest value set so far and only ever raise it
   std::vector<std::pair<const void*, size_t>> smem_set;
   std::vector<std::pair<const void*, int>> regs_of;  // cudaFuncGetAttributes().numRegs, queried once per function
+  // cached residency of the chunked kernel per (function, dynamic shared memory, CTA cap)
+  struct ChunkedPlan {
+    const void* fn = nullptr;
+    size_t smem = 0;
+    int cap = 0;
+    int ctas = 0;
+    int carveout = 0;  // cudaFuncAttributePreferredSharedMemoryCarveout for these CTAs
+  };
+  std::vector<ChunkedPlan> chunked_plans;
+  std::vector<std::pair<const void*, int>> carveout_set;  // carveout last set per function
   // last encoded tensor map (B = 1 solveLinear() calls re-use the same output buffer)
   struct TmapKey {
     const void* base = nullptr;
@@ -176,6 +189,9 @@ void compute_layout(int N, int K, const std::vector<uint8_t>& mask, Layout* L) {
 // depth of the cp.async input ring of the v4 and chunked instantiations (their layouts depend on it)
 constexpr int kRingDepth = 3;
 typedef void (*WaypointKernel)(const mtg::WaypointParams);
+typedef void (*ChunkedKernel)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap);
+// warps per CTA of the chunked kernel's instantiations (WaypointEntry::fn_chunked)
+constexpr int kChunkedWarps[2] = {1, 4};
 struct WaypointEntry {
   int N, R, D, slots;
   WaypointKernel fn;          // one thread per trajectory
@@ -183,16 +199,18 @@ struct WaypointEntry {
   void (*fn_tmem)(const mtg::WaypointParams, const CUtensorMap);  // + shared-memory state, TMA stores
   void (*fn_tmem_fused)(const mtg::WaypointParams, const CUtensorMap);  // + fused Nfabian
   size_t (*tmem_smem)(int K);  // dynamic shared memory of fn_tmem / fn_tmem_fused (mtg::V3Layout)
-  void (*fn_chunked)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap);  // any K (K3)
-  size_t (*chunked_smem)(int C);  // dynamic shared memory of fn_chunked with C resident blocks (mtg::ChunkedLayout)
+  ChunkedKernel fn_chunked[2];      // any K (K3), kChunkedWarps[i] warps per CTA
+  size_t (*chunked_smem[2])(int C);  // dynamic shared memory of fn_chunked[i] with C resident blocks (mtg::ChunkedLayout)
   int chunked_park_slots;         // doubles per thread of one vertex block that fn_chunked parks in global memory
 };
 #define MTG_WP_(N_, R_, D_, V1_)                                                                                  \
   {                                                                                                               \
     N_, R_, D_, mtg::sweep_state_slots<N_, D_>(), V1_, mtg::twisted_solve_kernel<N_, R_, D_>,                     \
         mtg::twisted_tmem_kernel<N_, R_, D_>, mtg::twisted_tmem_kernel<N_, R_, D_, true>,                         \
-        mtg::V3Layout<N_, D_>::bytes, mtg::twisted_chunked_kernel<N_, R_, D_, kRingDepth>,                        \
-        mtg::ChunkedLayout<N_, D_, kRingDepth>::bytes, mtg::ChunkedLayout<N_, D_, kRingDepth>::kPark              \
+        mtg::V3Layout<N_, D_>::bytes,                                                                             \
+        {mtg::twisted_chunked_kernel<N_, R_, D_, kRingDepth, 1>, mtg::twisted_chunked_kernel<N_, R_, D_, kRingDepth, 4>}, \
+        {mtg::ChunkedLayout<N_, D_, kRingDepth, 1>::bytes, mtg::ChunkedLayout<N_, D_, kRingDepth, 4>::bytes},    \
+        mtg::ChunkedLayout<N_, D_, kRingDepth, 4>::kPark                                                          \
   }
 #define MTG_WP(N_, R_, D_) MTG_WP_(N_, R_, D_, (mtg::waypoint_solve_kernel<N_, R_, D_>))
 // v1 (thread per trajectory) is kept for the headline shapes only (cross-check / profiles)
@@ -429,14 +447,61 @@ struct FusedInput {
 // shared memory of an SM that resident CTAs share (H100: 228 KB; every CTA also reserves 1 KB of it)
 constexpr int kSmemPerSm = 228 * 1024;
 
-// Resident CTAs per SM of a kTmemThreads-thread kernel with `smem` bytes of dynamic shared memory: limited by its
+// Resident CTAs per SM of a `threads`-thread kernel with `smem` bytes of dynamic shared memory: limited by its
 // registers, by shared memory and by `cap`; 0 when `smem` exceeds the per-block opt-in limit.
-int resident_ctas(mtg_handle* h, const void* fn, size_t smem, int cap, int* ctas) {
+int resident_ctas(mtg_handle* h, const void* fn, size_t smem, int cap, int threads, int* ctas) {
   int n_regs = 0;
   const int rc = kernel_regs(h, fn, &n_regs);
   if (rc != MTG_OK) return rc;
-  const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * mtg::kTmemThreads));
+  const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * threads));
   *ctas = smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024))), cap);
+  return MTG_OK;
+}
+
+// Set the shared memory carveout of `fn` (percent of the SM's maximum), unless it already has that value.
+int set_carveout(mtg_handle* h, const void* fn, int percent) {
+  for (auto& kv : h->carveout_set)
+    if (kv.first == fn) {
+      if (kv.second != percent) MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, percent));
+      kv.second = percent;
+      return MTG_OK;
+    }
+  MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, percent));
+  h->carveout_set.emplace_back(fn, percent);
+  return MTG_OK;
+}
+
+// Resident CTAs per SM of the chunked kernel `fn` (`threads` per CTA, `smem` bytes of dynamic shared memory, at most
+// `cap`) and the shared memory carveout those CTAs need (*carveout, percent): the rest of the SM's 256 KB stays L1,
+// which serves the 8-byte cp.async input reads.  On the first use of a configuration the hand-computed residency is
+// checked against the occupancy calculator at that carveout, so that the planned warps per SM are the ones that run.
+int chunked_residency(mtg_handle* h, const void* fn, size_t smem, int cap, int threads, int* ctas, int* carveout) {
+  for (const auto& pl : h->chunked_plans)
+    if (pl.fn == fn && pl.smem == smem && pl.cap == cap) {
+      *ctas = pl.ctas;
+      *carveout = pl.carveout;
+      return MTG_OK;
+    }
+  mtg_handle::ChunkedPlan np;
+  np.fn = fn;
+  np.smem = smem;
+  np.cap = cap;
+  int rc = resident_ctas(h, fn, smem, cap, threads, &np.ctas);
+  if (rc != MTG_OK) return rc;
+  if (np.ctas > 0) {
+    rc = ensure_dyn_smem(h, fn, smem);
+    if (rc != MTG_OK) return rc;
+    const size_t need = size_t(np.ctas) * (smem + 1024);
+    np.carveout = int(std::min<size_t>(100, (need * 100 + kSmemPerSm - 1) / kSmemPerSm));
+    rc = set_carveout(h, fn, np.carveout);
+    if (rc != MTG_OK) return rc;
+    int occ = 0;
+    MTG_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, threads, smem));
+    np.ctas = std::min(np.ctas, occ);
+  }
+  h->chunked_plans.push_back(np);
+  *ctas = np.ctas;
+  *carveout = np.carveout;
   return MTG_OK;
 }
 
@@ -445,51 +510,80 @@ int resident_ctas(mtg_handle* h, const void* fn, size_t smem, int cap, int* ctas
 int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, const mtg::WaypointParams& prm,
                    double* coeffs, int64_t B, cudaStream_t stream, int slot) {
   const int nmax = (p->K + 1) / 2 - 1;
-  int best_ctas = 0, best_C = 0;
+  // Auto: one-warp CTAs (shared memory then comes in 31-52 KB steps instead of 124-206 KB ones), no L2 hints, at
+  // most kAutoParkWarps warps per SM while any block is parked and as many as fit otherwise; among the chunks up to
+  // the auto chunk, the one with the most warps, the largest on a tie.  The auto chunk is 5 while that parks at most
+  // kAutoParkedMax blocks per lane (K <= 16 at N = 10), 4 beyond.  Each resident block takes 3.2 KB of shared
+  // memory per warp away from L1 and saves one round trip of a parked block through L2: it pays while the parked
+  // blocks are few.  Measured with tools/k3_sweep.py on an H100 SXM at N = 10, D = 3, 4 warps per SM (ms per solve,
+  // 700 W power limit, spread of the round medians <= 0.02 ms):
+  //   K = 16  (1 048 576): C = 3 2.93, C = 4 2.72, C = 5 2.60, C = 6 2.98
+  //   K = 50  (246 272):   C = 3 3.15, C = 4 3.09, C = 5 3.10, C = 6 3.48
+  //   K = 100 (113 664):   C = 3 3.11, C = 4 3.08, C = 5 3.14, C = 6 3.60
+  // More warps pay only when nothing is parked (400 W: K = 8, C = 3 runs 1.28 ms at 6-7 warps against 1.51 ms at 4);
+  // with parked blocks they lose (C = 3, K = 16: 2.93 ms at 4 warps, 3.52 at 7), with or without evict-first hints on
+  // the streamed data, and the hints themselves cost 2-20 %.  Four-warp CTAs at the same warps run 1-3 % slower.
+  constexpr int kAutoParkWarps = 4;
+  constexpr int kAutoParkedMax = 2;
+  const int auto_chunk = nmax - 5 <= kAutoParkedMax ? 5 : 4;
+  const int cmax = std::max(1, std::min(nmax, h->chunk_blocks > 0 ? 24 : auto_chunk));
+  int best_warps = 0, best_C = 0, best_i = 0, best_ctas = 0, best_carveout = 0;
   size_t best_smem = 0;
-  // Auto: the largest chunk up to kAutoChunk that fits.  Measured on H100 at N = 10, D = 3 (K = 16, 50, 100): C = 3
-  // at one CTA per SM runs 20-35 % faster than C = 2 at two CTAs per SM -- the second CTA's warps hide less than
-  // its doubled parking area and halved L1 cost -- and C = 4 is level with C = 3, while C = 5 and 6 lose again as
-  // shared memory crowds out L1.
-  constexpr int kAutoChunk = 3;
-  const int cmax = std::max(1, std::min(nmax, h->chunk_blocks > 0 ? 24 : kAutoChunk));
-  for (int C = cmax; C >= 1 && best_ctas == 0; --C) {
+  for (int C = cmax; C >= 1; --C) {
     if (h->chunk_blocks > 0 && C != std::min(h->chunk_blocks, cmax)) continue;
-    const size_t smem = e->chunked_smem(C);
-    int ctas = 0;
-    const int rc_ctas = resident_ctas(h, (const void*)e->fn_chunked, smem, 8, &ctas);
-    if (rc_ctas != MTG_OK) return rc_ctas;
-    best_ctas = ctas;
-    best_C = C;
-    best_smem = smem;
+    for (int i = 0; i < 2; ++i) {
+      const int W = kChunkedWarps[i];
+      if (h->chunk_warps > 0 ? W != h->chunk_warps : W != 1) continue;
+      // cap on resident warps per SM
+      const int wcap = h->ctas_per_sm > 0 ? h->ctas_per_sm : (nmax > C ? kAutoParkWarps : 64);
+      const size_t smem = e->chunked_smem[i](C);
+      int ctas = 0, carveout = 0;
+      const int rc =
+          chunked_residency(h, (const void*)e->fn_chunked[i], smem, std::max(1, wcap / W), 32 * W, &ctas, &carveout);
+      if (rc != MTG_OK) return rc;
+      if (ctas * W > best_warps) {
+        best_warps = ctas * W;
+        best_ctas = ctas;
+        best_carveout = carveout;
+        best_C = C;
+        best_i = i;
+        best_smem = smem;
+      }
+    }
   }
-  if (best_ctas == 0) {
+  if (best_warps == 0) {
     h->error = "chunked kernel: no launch configuration fits";
     return MTG_ERR_ALLOC;
   }
-  const int64_t ctiles = (B + 63) / 64;
+  const int W = kChunkedWarps[best_i];
+  const void* fn = (const void*)e->fn_chunked[best_i];
+  const int threads = 32 * W;
+  const int64_t ctiles = (B + 16 * W - 1) / (16 * W);
   const int64_t blocks = std::min<int64_t>(ctiles, int64_t(best_ctas) * h->sm_count);
   const int npark = nmax - best_C;  // parked vertex blocks per lane
   mtg::ChunkedLaunch cl;
   cl.chunk = best_C;
   cl.ckpt = nullptr;
+  cl.evict_first = h->l2_hints;
   mtg_handle::Arena& ar = h->scratch[slot];
   if (npark > 0) {
-    const size_t bytes = size_t(npark) * e->chunked_park_slots * size_t(blocks) * mtg::kTmemThreads * sizeof(double);
+    const size_t bytes = size_t(npark) * e->chunked_park_slots * size_t(blocks) * threads * sizeof(double);
     const int rc = arena_acquire(h, ar, bytes, stream);
     if (rc != MTG_OK) return rc;
     cl.ckpt = ar.p;
   }
   {
-    const int rc_smem = ensure_dyn_smem(h, (const void*)e->fn_chunked, size_t(best_smem));
-    if (rc_smem != MTG_OK) return rc_smem;
+    int rc = ensure_dyn_smem(h, fn, best_smem);
+    if (rc != MTG_OK) return rc;
+    rc = set_carveout(h, fn, best_carveout);
+    if (rc != MTG_OK) return rc;
   }
   CUtensorMap tmap;
   {
     const int rc = encode_coeff_tmap(h, &tmap, coeffs, B, p);
     if (rc != MTG_OK) return rc;
   }
-  e->fn_chunked<<<(unsigned)blocks, mtg::kTmemThreads, best_smem, stream>>>(prm, cl, tmap);
+  e->fn_chunked[best_i]<<<(unsigned)blocks, threads, best_smem, stream>>>(prm, cl, tmap);
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
   if (npark > 0) return arena_release(h, ar, stream);
@@ -569,7 +663,7 @@ int launch_cost_fused(mtg_handle* h, const mtg_problem* p, CachedTopology* topo,
   const size_t smem = ce->smem(p->K);
   int ctas = 0;
   {
-    const int rc_ctas = resident_ctas(h, (const void*)ce->fn, smem, 16, &ctas);
+    const int rc_ctas = resident_ctas(h, (const void*)ce->fn, smem, 16, mtg::kTmemThreads, &ctas);
     if (rc_ctas != MTG_OK) return rc_ctas;
   }
   if (ctas < 2) return MTG_ERR_ALLOC;  // large K: unfused path (chunked kernel + cost kernel)
@@ -654,7 +748,7 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
         for (int nbuf = 2; nbuf >= 1; --nbuf) {
           const size_t smem = (fused ? e5->smem_fused : e5->smem)(p->K, L.n_fixed, nbuf);
           int ctas = 0;
-          const int rc_ctas = resident_ctas(h, (const void*)fn5, smem, 8, &ctas);
+          const int rc_ctas = resident_ctas(h, (const void*)fn5, smem, 8, mtg::kTmemThreads, &ctas);
           if (rc_ctas != MTG_OK) return rc_ctas;
           // more resident CTAs first; then double buffering
           if (ctas > best_ctas) {
@@ -715,7 +809,7 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
         const size_t best_smem = e4->smem(p->K);
         int best_ctas = 0;
         {
-          const int rc_ctas = resident_ctas(h, (const void*)fn, best_smem, 8, &best_ctas);
+          const int rc_ctas = resident_ctas(h, (const void*)fn, best_smem, 8, mtg::kTmemThreads, &best_ctas);
           if (rc_ctas != MTG_OK) return rc_ctas;
         }
         if (best_ctas >= (h->waypoint_variant == 4 ? 1 : 2)) {  // as for v5: a forced v4 runs whenever one CTA fits
@@ -765,7 +859,7 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
         np.entry = (const void*)e;
         np.K = p->K;
         np.smem = e->tmem_smem(p->K);
-        const int rc_ctas = resident_ctas(h, (const void*)e->fn_tmem, np.smem, 16, &np.ctas);
+        const int rc_ctas = resident_ctas(h, (const void*)e->fn_tmem, np.smem, 16, mtg::kTmemThreads, &np.ctas);
         if (rc_ctas != MTG_OK) return rc_ctas;
         h->plans.push_back(np);
         plan = &h->plans.back();
@@ -962,6 +1056,14 @@ int mtg_set_option(mtg_handle* h, int key, int value) {
   }
   if (key == MTG_OPT_CHUNK_BLOCKS && value >= 0 && value <= 64) {
     h->chunk_blocks = value;
+    return MTG_OK;
+  }
+  if (key == MTG_OPT_CHUNK_WARPS && (value == 0 || value == 1 || value == 4)) {
+    h->chunk_warps = value;
+    return MTG_OK;
+  }
+  if (key == MTG_OPT_L2_HINTS && (value == 0 || value == 1)) {
+    h->l2_hints = value;
     return MTG_OK;
   }
   if (key == MTG_OPT_TMA_INPUTS && value >= 0 && value <= 2) {

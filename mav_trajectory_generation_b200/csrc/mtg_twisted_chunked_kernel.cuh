@@ -4,8 +4,8 @@
 //
 // The resident kernels keep the factor of every eliminated vertex in shared memory, which caps the number of
 // trajectories in flight per SM as K grows (25 doubles per lane and eliminated vertex at N = 10, D = 3).  Here
-// only the C innermost vertex blocks of a lane stay in shared memory -- the host picks C for the most resident CTAs
-// per SM -- and the outer ones are PARKED in global memory.  One pass per tile:
+// only the C innermost vertex blocks of a lane stay in shared memory -- the host picks C and the warps per SM
+// (launch_chunked) -- and the outer ones are PARKED in global memory.  One pass per tile:
 //
 //   forward   sweep over all own vertices 1..n (n = ceil(K/2)-1); the block of vertex v <= n-C (its pack() slots
 //             and the step's segment time) goes to the parking area, the innermost C blocks to shared slot
@@ -16,12 +16,13 @@
 //
 // Cost: no recomputation -- every vertex is factorised once, as in the resident kernels.  Extra global traffic
 // 2 * (n-C) * (kSlots+1) * 8 bytes per lane (written once, read once); CTAs are persistent (static tile
-// assignment), so the parking area is bounded by the number of resident threads, not by the batch (about 1 KB per
-// thread at K = 16, C = 3: it stays in L2; at K = 50 it spills to HBM).  Every thread owns one column of it,
+// assignment), so the parking area is bounded by the number of resident threads, not by the batch (about 0.4 KB
+// per thread at K = 16, C = 5: it stays in L2; at K = 50 it spills to HBM).  Every thread owns one column of it,
 // laid out [block][slot][thread] so that a warp stores or loads one slot as 256 contiguous bytes.  As in v4, the
 // next tile's prologue inputs are prefetched into the dead state region at the end of the outward sweep, and the
 // fixed end derivatives of the final emission into the idle input ring.  Arithmetic per vertex is exactly the
-// v4 sequence: results are bitwise equal to v4 and independent of C (tests force tiny chunks on K = 16 to prove it).
+// v4 sequence: results are bitwise equal to v4 and independent of C (tests force tiny chunks on K = 16 to prove it),
+// of the warps per CTA, of the warps per SM and of the L2 hints.
 #pragma once
 
 #include "mtg_twisted_tmem_v4_kernel.cuh"
@@ -30,13 +31,16 @@ namespace mtg {
 
 struct ChunkedLaunch {
   int chunk;          // C: vertex blocks resident per lane (in shared memory)
-  double* ckpt;       // parking area [n-C][kPark][gridDim.x * 128]: the outer vertex blocks of the sweep
+  double* ckpt;       // parking area [n-C][kPark][gridDim.x * blockDim.x]: the outer vertex blocks of the sweep
+  int evict_first;    // inputs and coefficient stores marked evict-first in L2, so that the parking area stays there
 };
 
 // Dynamic shared memory of K3 behind the staging tiles, in per-thread slots:
 // [input ring RD x (1+D)][times C][stash D+1][region: C blocks with the vertex position, or the next tile's prologue]
-template <int N, int D, int RD>
+// for a CTA of W warps
+template <int N, int D, int RD, int W>
 struct ChunkedLayout {
+  static constexpr int kThreads = 32 * W;
   static constexpr int kSlots = sweep_state_slots<N, D, true>();
   static constexpr int kPark = kSlots + 1;                   // a parked block: pack() slots, then the segment time
   static constexpr int kPro = 2 * D + (N / 2 - 1) * D + 1;  // x0, x1, u0[m], T0
@@ -49,7 +53,7 @@ struct ChunkedLayout {
     return size_t(C) * kSlots > size_t(kPro) ? size_t(C) * kSlots : size_t(kPro);
   }
   __host__ __device__ static constexpr size_t bytes(int C) {
-    return tmem_stage_bytes<N, D>() + tmem_slot_bytes(region(C) + region_slots(C));
+    return tmem_stage_bytes<N, D, kThreads>() + tmem_slot_bytes(region(C) + region_slots(C), kThreads);
   }
 };
 
@@ -62,24 +66,29 @@ __device__ __forceinline__ void cp_async_wait_at_most(int pending) {
   else cp_async_wait_group<3>();
 }
 
-template <int N, int R, int D, int RD>
-__global__ void __launch_bounds__(kTmemThreads, 2)
+// W warps per CTA.  The warps of a CTA share nothing but the CTA's shared memory allocation (each has its own staging
+// tile, tiles, parking column and TMA group; there is no __syncthreads), so W only sets the granularity in which
+// shared memory is allocated: at N = 10, D = 3 one-warp CTAs fit 7 warps per SM at C = 3 where four-warp CTAs
+// fit 4.
+// Both launch bounds give a register cap of 255.
+template <int N, int R, int D, int RD, int W>
+__global__ void __launch_bounds__(32 * W, 8 / W)
     twisted_chunked_kernel(const WaypointParams prm, const ChunkedLaunch cl, const __grid_constant__ CUtensorMap tmap) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
-  using Lay = ChunkedLayout<N, D, RD>;
+  using Lay = ChunkedLayout<N, D, RD, W>;
   constexpr int kSlots = Lay::kSlots;
   constexpr int kPark = Lay::kPark;
   constexpr int kPro = Lay::kPro;
-  constexpr int kWarps = kTmemThreads / 32;
+  constexpr int kThreads = Lay::kThreads;
   static_assert(RD >= 2, "ring depth");
   using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
   using S = sweep::Sweep<N, D, G>;
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int lane = threadIdx.x & 31;
-  const int warp = threadIdx.x >> 5;
+  const int lane = W == 1 ? int(threadIdx.x) : int(threadIdx.x & 31);
+  const int warp = W == 1 ? 0 : int(threadIdx.x >> 5);
   const int half = lane & 1;
   const int K = prm.K;
   const int nf = prm.n_fixed;
@@ -90,22 +99,22 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   const int npark = n - C;  // vertices 1..npark are parked (none when C >= n)
 
   double2* stage = reinterpret_cast<double2*>(smem_raw) + size_t(warp) * 32 * (D * h);
-  double* base = reinterpret_cast<double*>(smem_raw + tmem_stage_bytes<N, D>()) + threadIdx.x;
-  auto PF = [&](int buf, int slot) -> double* { return base + (size_t(buf) * (1 + D) + slot) * kTmemThreads; };
-  double* thist = base + size_t(Lay::kHist) * kTmemThreads;
-  auto HT = [&](int b) -> double* { return thist + size_t(b) * kTmemThreads; };  // time of the step that made block b
-  double* stash = thist + size_t(Lay::hist_slots(C)) * kTmemThreads;  // x0[D], T0
-  double* region = stash + size_t(Lay::kStash) * kTmemThreads;        // state blocks; next tile's prologue inputs
-  auto SP = [&](int blk, int slot) -> double* { return region + (size_t(blk) * kSlots + slot) * kTmemThreads; };
-  auto PRO = [&](int slot) -> double* { return region + size_t(slot) * kTmemThreads; };
+  double* base = reinterpret_cast<double*>(smem_raw + tmem_stage_bytes<N, D, kThreads>()) + threadIdx.x;
+  auto PF = [&](int buf, int slot) -> double* { return base + (size_t(buf) * (1 + D) + slot) * kThreads; };
+  double* thist = base + size_t(Lay::kHist) * kThreads;
+  auto HT = [&](int b) -> double* { return thist + size_t(b) * kThreads; };  // time of the step that made block b
+  double* stash = thist + size_t(Lay::hist_slots(C)) * kThreads;  // x0[D], T0
+  double* region = stash + size_t(Lay::kStash) * kThreads;        // state blocks; next tile's prologue inputs
+  auto SP = [&](int blk, int slot) -> double* { return region + (size_t(blk) * kSlots + slot) * kThreads; };
+  auto PRO = [&](int slot) -> double* { return region + size_t(slot) * kThreads; };
 
   const sweep::Frame<N> fr{K, half};
   const int e0 = fr.e0();
 
   const long long n_wtiles = (prm.B + 15) >> 4;
-  const long long wt_stride = (long long)gridDim.x * kWarps;
-  const long long gthreads = (long long)gridDim.x * kTmemThreads;
-  double* __restrict__ pk = cl.ckpt ? cl.ckpt + ((long long)blockIdx.x * kTmemThreads + threadIdx.x) : nullptr;
+  const long long wt_stride = (long long)gridDim.x * W;
+  const long long gthreads = (long long)gridDim.x * kThreads;
+  double* __restrict__ pk = cl.ckpt ? cl.ckpt + ((long long)blockIdx.x * kThreads + threadIdx.x) : nullptr;
   auto PK = [&](int b, int slot) -> double* { return pk + ((long long)b * kPark + slot) * gthreads; };
 
   // pointers of a warp tile's trajectory for this lane
@@ -129,24 +138,24 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
   auto pro_issue = [&](const Ptrs& p) {
 #pragma unroll
     for (int d = 0; d < D; ++d) {
-      cp_async8(PRO(d), xaddr(p, 0, d));
-      cp_async8(PRO(D + d), xaddr(p, 1, d));
+      cp_async8_stream(PRO(d), xaddr(p, 0, d), cl.evict_first);
+      cp_async8_stream(PRO(D + d), xaddr(p, 1, d), cl.evict_first);
 #pragma unroll
-      for (int b = 0; b < m; ++b) cp_async8(PRO(2 * D + b * D + d), p.fx + d * nf + e0 + b);
+      for (int b = 0; b < m; ++b) cp_async8_stream(PRO(2 * D + b * D + d), p.fx + d * nf + e0 + b, cl.evict_first);
     }
-    cp_async8(PRO(kPro - 1), p.tt + fr.seg(0));
+    cp_async8_stream(PRO(kPro - 1), p.tt + fr.seg(0), cl.evict_first);
   };
   // inputs of inward step v (time of own segment v, position of own vertex v+1) -> ring buffer v % RD
   auto ring_issue = [&](const Ptrs& p, int v) {
     const int j = v < K ? v : K - 1;
     const int vn = v + 1 <= K ? v + 1 : K;
     const int buf = v % RD;
-    cp_async8(PF(buf, 0), p.tt + fr.seg(j));
+    cp_async8_stream(PF(buf, 0), p.tt + fr.seg(j), cl.evict_first);
 #pragma unroll
-    for (int d = 0; d < D; ++d) cp_async8(PF(buf, 1 + d), xaddr(p, vn, d));
+    for (int d = 0; d < D; ++d) cp_async8_stream(PF(buf, 1 + d), xaddr(p, vn, d), cl.evict_first);
   };
 
-  long long wt = (long long)blockIdx.x * kWarps + warp;
+  long long wt = (long long)blockIdx.x * W + warp;
   if (wt < n_wtiles) {
     pro_issue(tile_ptrs(wt));
     cp_async_commit();
@@ -154,7 +163,7 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
 
   double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
   const int nhF = M - 1, nhB = K - M - 1;
-  const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB};
+  const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB, cl.evict_first != 0};
 
   for (; wt < n_wtiles; wt += wt_stride) {
     const long long wt_next = wt + wt_stride;  // its prologue is prefetched at the end of this tile
@@ -179,10 +188,10 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
       for (int d = 0; d < D; ++d) {
         xm[d] = *PRO(d);
         xc[d] = *PRO(D + d);
-        stash[size_t(d) * kTmemThreads] = xm[d];
+        stash[size_t(d) * kThreads] = xm[d];
       }
       const double T0 = *PRO(kPro - 1);
-      stash[size_t(D) * kTmemThreads] = T0;
+      stash[size_t(D) * kThreads] = T0;
       if (!(T0 > 0.0)) stat |= kStatusBadTime;
       const double iT0 = fast_rcp(T0);
       double pw[N - 1];
@@ -268,7 +277,7 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
 #pragma unroll
       for (int d = 0; d < D; ++d)
 #pragma unroll
-        for (int b = 0; b < m; ++b) cp_async8(base + size_t(b * D + d) * kTmemThreads, P.fx + d * nf + e0 + b);
+        for (int b = 0; b < m; ++b) cp_async8_stream(base + size_t(b * D + d) * kThreads, P.fx + d * nf + e0 + b, cl.evict_first);
       cp_async_commit();
     }
     // the next tile's prologue inputs go to the state region: issued once every state block has been read back
@@ -326,17 +335,17 @@ __global__ void __launch_bounds__(kTmemThreads, 2)
       }
 #pragma unroll
       for (int d = 0; d < D; ++d) {
-        sd[0][d] = stash[size_t(d) * kTmemThreads];
+        sd[0][d] = stash[size_t(d) * kThreads];
 #pragma unroll
         for (int b = 0; b < m; ++b) {
           if constexpr (kEndInRing) {
-            sd[1 + b][d] = fr.sgn(b) * base[size_t(b * D + d) * kTmemThreads];
+            sd[1 + b][d] = fr.sgn(b) * base[size_t(b * D + d) * kThreads];
           } else {
             sd[1 + b][d] = fr.sgn(b) * __ldg(P.fx + d * nf + e0 + b);
           }
         }
       }
-      const double T = stash[size_t(D) * kTmemThreads];
+      const double T = stash[size_t(D) * kThreads];
       const double iT = fast_rcp(T);
       __syncwarp();
       out.emit(0, 0, T, iT, sd, ed, traj0);

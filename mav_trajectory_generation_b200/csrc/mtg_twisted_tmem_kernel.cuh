@@ -28,14 +28,16 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast
 
 constexpr int kTmemThreads = 128;
 
-// coefficient staging tiles of the four warps of a CTA at the start of dynamic shared memory: one whole segment (D*N
+// coefficient staging tiles of the warps of a CTA at the start of dynamic shared memory: one whole segment (D*N
 // contiguous output doubles) per lane, i.e. two 16-row TMA boxes per warp
-template <int N, int D>
+template <int N, int D, int kThreads = kTmemThreads>
 __host__ __device__ constexpr size_t tmem_stage_bytes() {
-  return size_t(kTmemThreads / 32) * 32 * D * (N / 2) * 16;
+  return size_t(kThreads / 32) * 32 * D * (N / 2) * 16;
 }
-// bytes of `slots` per-thread doubles (slot s of thread t at double s * kTmemThreads + t)
-__host__ __device__ constexpr size_t tmem_slot_bytes(size_t slots) { return slots * kTmemThreads * 8; }
+// bytes of `slots` per-thread doubles (slot s of thread t at double s * kThreads + t)
+__host__ __device__ constexpr size_t tmem_slot_bytes(size_t slots, int kThreads = kTmemThreads) {
+  return slots * kThreads * 8;
+}
 
 // Dynamic shared memory of v3 (and its cost-only instantiation) behind the staging tiles, in per-thread slots:
 // [prefetch ring 2 x (1+D)][time history nmax+1][sweep state: nmax blocks with the vertex position]
@@ -53,6 +55,18 @@ struct V3Layout {
 __device__ __forceinline__ void cp_async8(const double* smem_dst, const double* gsrc) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
+// cp_async8 that, when `evict_first`, marks the line evict-first in L2: for inputs read once, so that they do not
+// push out data that is read again (the chunked kernel's parking area)
+__device__ __forceinline__ void cp_async8_stream(const double* smem_dst, const double* gsrc, int evict_first) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 pol;\n\t"
+      "setp.ne.b32 p, %2, 0;\n\t"
+      "createpolicy.fractional.L2::evict_first.b64 pol, 1.0;\n\t"
+      "@p cp.async.ca.shared.global.L2::cache_hint [%0], [%1], 8, pol;\n\t"
+      "@!p cp.async.ca.shared.global [%0], [%1], 8;\n\t}" ::"r"(smem_u32(smem_dst)),
+      "l"(gsrc), "r"(evict_first)
+      : "memory");
+}
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 // TMA tensor store of a [16 rows][D*N doubles] shared-memory box to coeffs viewed as a 2-D tensor
 // [B trajectories][K*D*N doubles]: (c0 = first double inside the trajectory, c1 = first trajectory).  Rows
@@ -62,6 +76,16 @@ __device__ __forceinline__ void tma_store_box(const CUtensorMap* tmap, const voi
                    reinterpret_cast<uint64_t>(tmap)),
                "r"(smem_u32(ssrc)), "r"(c0), "r"(c1)
                : "memory");
+}
+// the same store with the written lines marked evict-first in L2 (the output is not read again by the kernel)
+__device__ __forceinline__ void tma_store_box_evict_first(const CUtensorMap* tmap, const void* ssrc, int c0, int c1) {
+  asm volatile(
+      "{\n\t.reg .b64 pol;\n\t"
+      "createpolicy.fractional.L2::evict_first.b64 pol, 1.0;\n\t"
+      "cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], pol;\n\t}" ::"l"(
+          reinterpret_cast<uint64_t>(tmap)),
+      "r"(smem_u32(ssrc)), "r"(c0), "r"(c1)
+      : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
@@ -79,6 +103,11 @@ struct TmaEmitter {
   double2* my_row;  // this lane's row of it
   int lane, K;
   int nhF, nhB;  // a half is active in sweep step v iff v <= its nh
+  bool evict_first = false;  // stores marked evict-first in L2 (the chunked kernel keeps its parking area in L2)
+  __device__ __forceinline__ void store(const void* ssrc, int c0, int c1) const {
+    if (evict_first) tma_store_box_evict_first(tmap, ssrc, c0, c1);
+    else tma_store_box(tmap, ssrc, c0, c1);
+  }
   // emit own-frame segment j for every lane of the warp at once (convergent); v_step: the sweep step (0 = final).
   // Rows of lanes that are not active in v_step are not stored.
   __device__ __forceinline__ void emit(int j, int v_step, double T, double iT, const double (&sd)[h][D],
@@ -101,8 +130,8 @@ struct TmaEmitter {
     fence_proxy_async();
     __syncwarp();
     if (lane == 0) {
-      if (v_step <= nhF) tma_store_box(tmap, stage, j * (D * N), (int)traj0);
-      if (v_step <= nhB) tma_store_box(tmap, stage + 16 * (D * h), (K - 1 - j) * (D * N), (int)traj0);
+      if (v_step <= nhF) store(stage, j * (D * N), (int)traj0);
+      if (v_step <= nhB) store(stage + 16 * (D * h), (K - 1 - j) * (D * N), (int)traj0);
       bulk_commit();
     }
   }
