@@ -122,7 +122,8 @@ __global__ void __launch_bounds__(128, 2)
     for (int v = 0; v <= K; ++v) {
       if (v < K) {
         const double T = __ldg(tt + v);
-        if (!(T > 0.0)) stat |= kStatusBadTime;
+        if (!(T > 0.0) || isinf(T)) stat |= kStatusBadTime;  // +inf too: a segment between two fully fixed
+                                                              // vertices reaches no pivot
         seg_powers(T, pwc);
         mn = free_mask(v + 1);
       } else {
@@ -194,7 +195,7 @@ __global__ void __launch_bounds__(128, 2)
         double s = Dp[j][j];
 #pragma unroll
         for (int k = 0; k < j; ++k) s = fma(-Dp[j][k], Dp[j][k], s);
-        if (!(s > 0.0)) stat |= kStatusNotSpd;
+        if (!(s > 0.0) || isinf(s)) stat |= kStatusNotSpd;
         inv[j] = fast_rsqrt(s);
 #pragma unroll
         for (int i = j + 1; i < h; ++i) {
