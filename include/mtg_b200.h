@@ -191,6 +191,41 @@ int mtg_evaluate_range_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D,
                                  const int32_t* derivs, int32_t max_samples, double* out, int32_t* n_samples,
                                  double* sampling_times, void* stream);
 
+/* computeMaximumOfMagnitude (impl/polynomial_optimization_linear_impl.h:465-497), B trajectories x n_derivs orders.
+ * Candidates per segment are 0, T and every real root in [0, T] of sum_d p_d^(k) p_d^(k+1) (p^(k+1) for D = 1;
+ * src/segment.cpp:83-184); the largest |p^(k)(t)| wins, the first one on a tie; all zero gives Extremum() = (0, 0, 0).
+ * N even in [2, 12].  derivs: HOST array, n_derivs <= 8, each in [0, N-2].  value/time/segment: [B][n_derivs]; time is
+ * relative to the segment start (Extremum::time); time, segment, status nullable.  A segment time <= 0 or non-finite:
+ * status MTG_STATUS_BAD_TIME, value and time NaN, segment -1. */
+int mtg_max_magnitude_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                const double* coeffs, int32_t n_derivs, const int32_t* derivs, double* value,
+                                double* time, int32_t* segment, int32_t* status, void* stream);
+
+/* The soft constraints and time cost of PolynomialOptimizationNonLinear (impl/polynomial_optimization_nonlinear_impl.h). */
+typedef struct mtg_soft_constraint {
+  int32_t derivative; /* in [0, N-2] */
+  double max_value;   /* > 0 and finite (the reference would divide by 0 at max_value == 0) */
+} mtg_soft_constraint;
+typedef struct mtg_time_objective {
+  int32_t time_cost;             /* 0: penalty * T_total^2 (kSquaredTime*), 1: penalty * T_total (kRichterTime*) */
+  double time_penalty;           /* reference default 500 */
+  double soft_constraint_weight; /* reference default 100 */
+  double maximum_cost;           /* clamp of each soft term: 1e12 in the objectives, 1e9 in getTotalCostWithSoftConstraints */
+  int32_t n_constraints;         /* 0..8; 0 = use_soft_constraints == false */
+  const mtg_soft_constraint* constraints; /* HOST array, summed in array order like inequality_constraints_ */
+} mtg_time_objective;
+
+/* objectiveFunctionTime (nonlinear_impl.h:556-615) when d_free == NULL: the solve of mtg_solve_linear_batch_f64 at
+ * seg_times; else objectiveFunctionTimeAndConstraints (:660-742): setFreeConstraints with d_free [B][D][n_free], as
+ * mtg_coeffs_from_constraints_batch_f64.  coeffs [B][K][D][N] is a required output (the extrema read it).
+ * objective[b] = computeCost() + time cost + sum_c min(maximum_cost, exp((max_c - max_value_c) / max_value_c * weight))
+ * (evaluateMaximumMagnitudeAsSoftConstraint, :766-795), summed in that order; the time sum runs left to right.
+ * terms [B][3] nullable = (trajectory cost, time cost, soft cost).  status [B] nullable; a trajectory with status != 0
+ * (MTG_STATUS_BAD_TIME, MTG_STATUS_NOT_SPD) has objective NaN. */
+int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                 const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
+                                 double* coeffs, double* objective, double* terms, int32_t* status, void* stream);
+
 /* ---- the hot path, HOST pointers (what PolynomialOptimization<N>::solveLinear() calls) ---- */
 /* Same contract with host buffers; H2D, kernels and D2H are pipelined over internal streams and
  * the call returns when the results are in the host buffers.  Pinned buffers (mtg_host_alloc)
@@ -214,6 +249,12 @@ int mtg_evaluate_range_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32
                                       const double* coeffs, double t_start, double t_end, double dt, int32_t n_derivs,
                                       const int32_t* derivs, int32_t max_samples, double* out, int32_t* n_samples,
                                       double* sampling_times);
+int mtg_max_magnitude_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                     const double* coeffs, int32_t n_derivs, const int32_t* derivs, double* value,
+                                     double* time, int32_t* segment, int32_t* status);
+int mtg_time_objective_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                      const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
+                                      double* coeffs, double* objective, double* terms, int32_t* status);
 
 /* ---- memory helpers (so host code above the ABI needs no CUDA headers) -------------------- */
 void* mtg_host_alloc(mtg_handle* h, uint64_t bytes);   /* pinned */

@@ -34,7 +34,10 @@ EXPORTED_SYMBOLS = [
     "mtg_cost_gradient_mellinger_batch_f64", "mtg_evaluate_batch_f64", "mtg_evaluate_range_batch_f64",
     "mtg_cost_gradient_mellinger_batch_host_f64", "mtg_evaluate_range_batch_host_f64",
     "mtg_memcpy_d2d", "mtg_ipc_export", "mtg_ipc_import", "mtg_ipc_close",
+    "mtg_max_magnitude_batch_f64", "mtg_time_objective_batch_f64", "mtg_max_magnitude_batch_host_f64",
+    "mtg_time_objective_batch_host_f64",
 ]
+TIME_COST_SQUARED, TIME_COST_RICHTER = 0, 1
 
 
 class MtgProblem(C.Structure):
@@ -44,6 +47,26 @@ class MtgProblem(C.Structure):
 
 class MtgLayout(C.Structure):
     _fields_ = [("n_all", C.c_int32), ("n_fixed", C.c_int32), ("n_free", C.c_int32), ("kernel", C.c_int32)]
+
+
+class MtgSoftConstraint(C.Structure):
+    _fields_ = [("derivative", C.c_int32), ("max_value", C.c_double)]
+
+
+class MtgTimeObjective(C.Structure):
+    _fields_ = [("time_cost", C.c_int32), ("time_penalty", C.c_double), ("soft_constraint_weight", C.c_double),
+                ("maximum_cost", C.c_double), ("n_constraints", C.c_int32),
+                ("constraints", C.POINTER(MtgSoftConstraint))]
+
+
+def time_objective_params(time_cost=TIME_COST_SQUARED, time_penalty=500.0, soft_constraint_weight=100.0,
+                          maximum_cost=1e12, constraints=()):
+    """mtg_time_objective for `constraints` = [(derivative, max_value), ...] (reference defaults otherwise)."""
+    arr = (MtgSoftConstraint * max(len(constraints), 1))(*[MtgSoftConstraint(int(k), float(v)) for k, v in constraints])
+    obj = MtgTimeObjective(int(time_cost), float(time_penalty), float(soft_constraint_weight), float(maximum_cost),
+                           len(constraints), C.cast(arr, C.POINTER(MtgSoftConstraint)))
+    obj._keep = arr  # the array must outlive the call
+    return obj
 
 
 _lib = None
@@ -100,6 +123,15 @@ def load():
                                                              C.c_double, C.c_double, C.c_double, dp, dp, dp]
     L.mtg_solve_waypoints_nfabian_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, i64, dp,
                                                         C.c_double, C.c_double, C.c_double, dp, dp, dp, vp]
+    i32p = C.POINTER(C.c_int32)
+    L.mtg_max_magnitude_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, C.c_int32, i32p, dp, dp,
+                                              dp, dp, vp]
+    L.mtg_max_magnitude_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, C.c_int32, i32p,
+                                                   dp, dp, dp, dp]
+    L.mtg_time_objective_batch_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dp, C.POINTER(MtgTimeObjective),
+                                               dp, dp, dp, dp, vp]
+    L.mtg_time_objective_batch_host_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dp,
+                                                    C.POINTER(MtgTimeObjective), dp, dp, dp, dp]
     for name in EXPORTED_SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export what the header declares
     _lib = L
@@ -269,6 +301,45 @@ class Solver:
         self._check(rc, "mtg_cost_gradient_mellinger_batch_f64")
         return cost, grad
 
+    def max_magnitude(self, seg_times, coeffs, derivs=(1, 2), stream=None):
+        """Batched computeMaximumOfMagnitude: (value, time, segment) [B][len(derivs)] and status [B] (int32)."""
+        import torch
+        B, K, D, N = coeffs.shape
+        derivs = [int(x) for x in derivs]
+        arr = (C.c_int32 * max(len(derivs), 1))(*derivs)
+        dev = coeffs.device
+        value = torch.empty((B, len(derivs)), dtype=torch.float64, device=dev)
+        time = torch.empty((B, len(derivs)), dtype=torch.float64, device=dev)
+        segment = torch.empty((B, len(derivs)), dtype=torch.int32, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.mtg_max_magnitude_batch_f64(self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(),
+                                                  len(derivs), arr, value.data_ptr(), time.data_ptr(),
+                                                  segment.data_ptr(), status.data_ptr(), s)
+        self._check(rc, "mtg_max_magnitude_batch_f64")
+        return value, time, segment, status
+
+    def time_objective(self, prob, seg_times, d_fixed, d_free=None, constraints=(), time_cost=TIME_COST_SQUARED,
+                       time_penalty=500.0, soft_constraint_weight=100.0, maximum_cost=1e12, stream=None):
+        """Batched objectiveFunctionTime (d_free None) / objectiveFunctionTimeAndConstraints: (objective [B],
+        terms [B][3] = (trajectory, time, soft), coeffs [B][K][D][N], status [B]).  constraints: [(derivative,
+        max_value), ...]."""
+        import torch
+        B = seg_times.shape[0]
+        dev = seg_times.device
+        obj = time_objective_params(time_cost, time_penalty, soft_constraint_weight, maximum_cost, constraints)
+        coeffs = torch.empty((B, prob.K, prob.D, prob.N), dtype=torch.float64, device=dev)
+        objective = torch.empty((B,), dtype=torch.float64, device=dev)
+        terms = torch.empty((B, 3), dtype=torch.float64, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.mtg_time_objective_batch_f64(
+            self.h, C.byref(prob.c), B, seg_times.data_ptr(), d_fixed.data_ptr(),
+            d_free.data_ptr() if d_free is not None else None, C.byref(obj), coeffs.data_ptr(), objective.data_ptr(),
+            terms.data_ptr(), status.data_ptr(), s)
+        self._check(rc, "mtg_time_objective_batch_f64")
+        return objective, terms, coeffs, status
+
     def coeffs_from_constraints(self, prob, seg_times, d_fixed, d_free, coeffs=None, stream=None):
         import torch
         B = seg_times.shape[0]
@@ -335,3 +406,22 @@ class Solver:
                                                       self._hptr(coeffs), self._hptr(cost))
         self._check(rc, "mtg_compute_cost_batch_host_f64")
         return cost
+
+    def max_magnitude_host(self, seg_times, coeffs, derivs, value, time=None, segment=None, status=None):
+        B, K, D, N = coeffs.shape
+        derivs = [int(x) for x in derivs]
+        arr = (C.c_int32 * max(len(derivs), 1))(*derivs)
+        rc = self.lib.mtg_max_magnitude_batch_host_f64(self.h, N, K, D, B, self._hptr(seg_times), self._hptr(coeffs),
+                                                       len(derivs), arr, self._hptr(value), self._hptr(time),
+                                                       self._hptr(segment), self._hptr(status))
+        self._check(rc, "mtg_max_magnitude_batch_host_f64")
+        return value
+
+    def time_objective_host(self, prob, seg_times, d_fixed, d_free, obj, coeffs, objective, terms=None, status=None):
+        """obj: time_objective_params(...)."""
+        B = seg_times.shape[0]
+        rc = self.lib.mtg_time_objective_batch_host_f64(
+            self.h, C.byref(prob.c), B, self._hptr(seg_times), self._hptr(d_fixed), self._hptr(d_free), C.byref(obj),
+            self._hptr(coeffs), self._hptr(objective), self._hptr(terms), self._hptr(status))
+        self._check(rc, "mtg_time_objective_batch_host_f64")
+        return objective

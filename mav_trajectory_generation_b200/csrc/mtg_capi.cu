@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
@@ -11,6 +12,7 @@
 #include <vector>
 
 #include "../../include/mtg_b200.h"
+#include "mtg_extrema_kernel.cuh"
 #include "mtg_generic_kernel.cuh"
 #include "mtg_twisted_kernel.cuh"
 #include "mtg_twisted_tmem_kernel.cuh"
@@ -1448,6 +1450,146 @@ int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
   return arena_release(h, ar, s);
 }
 
+// computeMaximumOfMagnitude: N even in [2, 12], 1..8 derivative orders, each in [0, N-2] (linear_impl.h:401 CHECKs
+// N - k - 1 > 0)
+static bool valid_extrema_args(int32_t N, int32_t K, int32_t D, int64_t B, int32_t n_derivs, const int32_t* derivs) {
+  if (N < 2 || N > MTG_MAX_N || (N & 1) || K < 1 || D < 1 || B < 0) return false;
+  if (n_derivs < 1 || n_derivs > mtg::kExtremaMaxDerivs || !derivs) return false;
+  for (int q = 0; q < n_derivs; ++q)
+    if (derivs[q] < 0 || derivs[q] > N - 2) return false;
+  return true;
+}
+
+static int launch_max_magnitude(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                const double* coeffs, int32_t n_derivs, const int32_t* derivs, double* value,
+                                double* time, int32_t* segment, int32_t* status, cudaStream_t s) {
+  mtg::ExtremaParams ep;
+  ep.K = K;
+  ep.D = D;
+  ep.n_derivs = n_derivs;
+  for (int q = 0; q < mtg::kExtremaMaxDerivs; ++q) ep.derivs[q] = q < n_derivs ? derivs[q] : 0;
+  ep.B = B;
+  ep.times = seg_times;
+  ep.coeffs = coeffs;
+  ep.value = value;
+  ep.time = time;
+  ep.segment = segment;
+  ep.status = status;
+  const int tpb = std::max(1, mtg::kExtremaThreads / K);
+  const size_t smem = size_t(2) * tpb * K * n_derivs * sizeof(double);
+  if (smem > h->smem_optin) {
+    h->error = "mtg_max_magnitude_batch_f64: K * n_derivs too large";
+    return MTG_ERR_BAD_ARG;
+  }
+  typedef void (*ExtremaFn)(const mtg::ExtremaParams, const int);
+  static const ExtremaFn kExtrema[MTG_MAX_N / 2] = {mtg::max_magnitude_kernel<2>, mtg::max_magnitude_kernel<4>,
+                                                    mtg::max_magnitude_kernel<6>, mtg::max_magnitude_kernel<8>,
+                                                    mtg::max_magnitude_kernel<10>, mtg::max_magnitude_kernel<12>};
+  const ExtremaFn fn = kExtrema[N / 2 - 1];
+  {
+    const int rc_smem = ensure_dyn_smem(h, (const void*)fn, smem);
+    if (rc_smem != MTG_OK) return rc_smem;
+  }
+  const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
+  fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(ep, tpb);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  return MTG_OK;
+}
+
+int mtg_max_magnitude_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                const double* coeffs, int32_t n_derivs, const int32_t* derivs, double* value,
+                                double* time, int32_t* segment, int32_t* status, void* stream) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid_extrema_args(N, K, D, B, n_derivs, derivs) || (B > 0 && (!seg_times || !coeffs || !value))) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (B == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  (void)cudaGetLastError();
+  return launch_max_magnitude(h, N, K, D, B, seg_times, coeffs, n_derivs, derivs, value, time, segment, status,
+                              (cudaStream_t)stream);
+}
+
+static bool valid_objective(const mtg_problem* p, const mtg_time_objective* obj) {
+  if (!obj || (obj->time_cost != 0 && obj->time_cost != 1)) return false;
+  if (obj->n_constraints < 0 || obj->n_constraints > mtg::kExtremaMaxDerivs) return false;
+  if (obj->n_constraints > 0 && !obj->constraints) return false;
+  for (int q = 0; q < obj->n_constraints; ++q) {
+    const mtg_soft_constraint& c = obj->constraints[q];
+    // max_value == 0 would divide by zero in the reference (nonlinear_impl.h:785)
+    if (c.derivative < 0 || c.derivative > p->N - 2 || !(c.max_value > 0.0) || !std::isfinite(c.max_value)) return false;
+  }
+  return true;
+}
+
+int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                 const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
+                                 double* coeffs, double* objective, double* terms, int32_t* status, void* stream) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid_problem(p) || B < 0 || !valid_objective(p, obj) ||
+      (B > 0 && (!seg_times || !d_fixed || !coeffs || !objective))) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (B == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  CachedTopology* topo = get_topology(h, p);
+  if (!topo) return MTG_ERR_CUDA;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int nc = obj->n_constraints;
+  // scratch: computeCost [B], maxima [B][nc], solve status [B]
+  const size_t o_max = align_doubles(size_t(B)), o_st = o_max + align_doubles(size_t(B) * nc),
+               need = (o_st + align_doubles((size_t(B) + 1) / 2)) * 8;
+  mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
+  int rc = arena_acquire(h, ar, need, s);
+  if (rc != MTG_OK) return rc;
+  double* cost = ar.p;
+  double* maxima = ar.p + o_max;
+  int32_t* solve_status = reinterpret_cast<int32_t*>(ar.p + o_st);
+  MTG_CUDA(h, cudaMemsetAsync(solve_status, 0, sizeof(int32_t) * size_t(B), s));
+  // the same launches as mtg_solve_linear_batch_f64 / mtg_coeffs_from_constraints_batch_f64
+  if (!d_free)
+    rc = launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, solve_status, s, false);
+  else
+    rc = launch_solve(h, p, topo, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, s, true);
+  if (rc != MTG_OK) return rc;
+  rc = mtg_compute_cost_batch_f64(h, p, B, seg_times, coeffs, cost, s);
+  if (rc != MTG_OK) return rc;
+  mtg::ObjectiveParams op;
+  op.K = p->K;
+  op.n_constraints = nc;
+  op.richter = obj->time_cost;
+  op.time_penalty = obj->time_penalty;
+  op.weight = obj->soft_constraint_weight;
+  op.maximum_cost = obj->maximum_cost;
+  if (nc > 0) {
+    int32_t derivs[mtg::kExtremaMaxDerivs];
+    for (int q = 0; q < nc; ++q) {
+      derivs[q] = obj->constraints[q].derivative;
+      op.max_value[q] = obj->constraints[q].max_value;
+    }
+    rc = launch_max_magnitude(h, p->N, p->K, p->D, B, seg_times, coeffs, nc, derivs, maxima, nullptr, nullptr, nullptr,
+                              s);
+    if (rc != MTG_OK) return rc;
+  }
+  op.B = B;
+  op.times = seg_times;
+  op.cost = cost;
+  op.maxima = maxima;
+  op.solve_status = solve_status;
+  op.objective = objective;
+  op.terms = terms;
+  op.status = status;
+  const int threads = 128;
+  const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
+  mtg::time_objective_kernel<<<(unsigned)blocks, threads, 0, s>>>(op);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  return arena_release(h, ar, s);
+}
+
 // ---- host-pointer variants: chunked H2D -> kernel -> D2H over kPipe streams ---------------
 // Every exit of a host-pointer entry point -- error returns included -- waits for all pipeline streams:
 // copies into caller-owned (possibly pinned) buffers must not be in flight when the caller gets control back.
@@ -1661,6 +1803,80 @@ int mtg_evaluate_range_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32
   MTG_CUDA(h, cudaMemcpyAsync(n_samples, base + o_n, b_n, cudaMemcpyDeviceToHost, s));
   if (sampling_times && max_samples > 0)
     MTG_CUDA(h, cudaMemcpyAsync(sampling_times, base + o_s, b_s, cudaMemcpyDeviceToHost, s));
+  MTG_CUDA(h, cudaStreamSynchronize(s));
+  return MTG_OK;
+}
+
+int mtg_max_magnitude_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                     const double* coeffs, int32_t n_derivs, const int32_t* derivs, double* value,
+                                     double* time, int32_t* segment, int32_t* status) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid_extrema_args(N, K, D, B, n_derivs, derivs) || (B > 0 && (!seg_times || !coeffs || !value))) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (B == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  const size_t b_t = size_t(K) * 8 * B, b_c = size_t(K) * D * N * 8 * B, b_v = size_t(n_derivs) * 8 * B,
+               b_s = size_t(n_derivs) * 4 * B;
+  const size_t o_c = align_up(b_t), o_v = align_up(o_c + b_c), o_t = align_up(o_v + b_v), o_s = align_up(o_t + b_v),
+               o_st = align_up(o_s + b_s);
+  int rc = ensure_pipe(h, 0, o_st + 4 * size_t(B));
+  if (rc != MTG_OK) return rc;
+  cudaStream_t s = h->streams[0];
+  char* base = static_cast<char*>(h->dev_buf[0]);
+  PipeSyncGuard sync_on_exit{h};
+  MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, b_t, cudaMemcpyHostToDevice, s));
+  MTG_CUDA(h, cudaMemcpyAsync(base + o_c, coeffs, b_c, cudaMemcpyHostToDevice, s));
+  rc = mtg_max_magnitude_batch_f64(h, N, K, D, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_c),
+                                   n_derivs, derivs, reinterpret_cast<double*>(base + o_v),
+                                   time ? reinterpret_cast<double*>(base + o_t) : nullptr,
+                                   segment ? reinterpret_cast<int32_t*>(base + o_s) : nullptr,
+                                   status ? reinterpret_cast<int32_t*>(base + o_st) : nullptr, s);
+  if (rc != MTG_OK) return rc;
+  MTG_CUDA(h, cudaMemcpyAsync(value, base + o_v, b_v, cudaMemcpyDeviceToHost, s));
+  if (time) MTG_CUDA(h, cudaMemcpyAsync(time, base + o_t, b_v, cudaMemcpyDeviceToHost, s));
+  if (segment) MTG_CUDA(h, cudaMemcpyAsync(segment, base + o_s, b_s, cudaMemcpyDeviceToHost, s));
+  if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_st, 4 * size_t(B), cudaMemcpyDeviceToHost, s));
+  MTG_CUDA(h, cudaStreamSynchronize(s));
+  return MTG_OK;
+}
+
+int mtg_time_objective_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                      const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
+                                      double* coeffs, double* objective, double* terms, int32_t* status) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid_problem(p) || B < 0 || !valid_objective(p, obj) ||
+      (B > 0 && (!seg_times || !d_fixed || !coeffs || !objective))) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (B == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  CachedTopology* topo = get_topology(h, p);
+  if (!topo) return MTG_ERR_CUDA;
+  const size_t K = p->K, D = p->D, N = p->N, nf = topo->layout.n_fixed, np = topo->layout.n_free;
+  const size_t b_t = K * 8 * B, b_f = D * nf * 8 * B, b_p = d_free ? D * np * 8 * B : 0, b_c = K * D * N * 8 * B;
+  const size_t o_f = align_up(b_t), o_p = align_up(o_f + b_f), o_c = align_up(o_p + b_p), o_o = align_up(o_c + b_c),
+               o_m = align_up(o_o + 8 * B), o_s = align_up(o_m + (terms ? 24 * B : 0));
+  int rc = ensure_pipe(h, 0, o_s + 4 * B);
+  if (rc != MTG_OK) return rc;
+  cudaStream_t s = h->streams[0];
+  char* base = static_cast<char*>(h->dev_buf[0]);
+  PipeSyncGuard sync_on_exit{h};
+  MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, b_t, cudaMemcpyHostToDevice, s));
+  MTG_CUDA(h, cudaMemcpyAsync(base + o_f, d_fixed, b_f, cudaMemcpyHostToDevice, s));
+  if (d_free && b_p) MTG_CUDA(h, cudaMemcpyAsync(base + o_p, d_free, b_p, cudaMemcpyHostToDevice, s));
+  rc = mtg_time_objective_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_f),
+                                    d_free ? reinterpret_cast<double*>(base + o_p) : nullptr, obj,
+                                    reinterpret_cast<double*>(base + o_c), reinterpret_cast<double*>(base + o_o),
+                                    terms ? reinterpret_cast<double*>(base + o_m) : nullptr,
+                                    status ? reinterpret_cast<int32_t*>(base + o_s) : nullptr, s);
+  if (rc != MTG_OK) return rc;
+  MTG_CUDA(h, cudaMemcpyAsync(coeffs, base + o_c, b_c, cudaMemcpyDeviceToHost, s));
+  MTG_CUDA(h, cudaMemcpyAsync(objective, base + o_o, 8 * B, cudaMemcpyDeviceToHost, s));
+  if (terms) MTG_CUDA(h, cudaMemcpyAsync(terms, base + o_m, 24 * B, cudaMemcpyDeviceToHost, s));
+  if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_s, 4 * B, cudaMemcpyDeviceToHost, s));
   MTG_CUDA(h, cudaStreamSynchronize(s));
   return MTG_OK;
 }

@@ -9,6 +9,7 @@
 
 #include <cstdint>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "mav_trajectory_generation/segment.h"
@@ -78,6 +79,15 @@ class LinearCore {
   void unpack(const std::vector<double>& coeffs);
 };
 
+// The time objective of PolynomialOptimizationNonLinear (reference NonlinearOptimizationParameters fields and defaults)
+struct TimeObjectiveParameters {
+  bool richter_time = false;  // kRichterTime*: time_penalty * T_total; otherwise time_penalty * T_total^2
+  double time_penalty = 500.0;
+  double soft_constraint_weight = 100.0;
+  double maximum_cost = 1e12;  // clamp of each soft term (1e9 in getTotalCostWithSoftConstraints)
+  std::vector<std::pair<int, double> > soft_constraints;  // (derivative, max value > 0), summed in this order; <= 8
+};
+
 class BatchCore {
  public:
   BatchCore(int N, size_t dimension);
@@ -98,6 +108,12 @@ class BatchCore {
   void evaluateRange(double t_start, double t_end, double dt, const std::vector<int>& derivatives, int max_samples,
                      std::vector<double>* samples, std::vector<int32_t>* n_samples,
                      std::vector<double>* sampling_times) const;
+  // batched computeMaximumOfMagnitude of the current coefficients (maxima: [B][n_derivs])
+  void computeMaximaOfMagnitude(const std::vector<int>& derivatives, std::vector<Extremum>* maxima) const;
+  // objectiveFunctionTime (d_free == nullptr) / objectiveFunctionTimeAndConstraints at the current segment times;
+  // the solved coefficients replace coeffs_ (objective: [B], terms: [B][3] or nullptr)
+  bool timeObjective(const TimeObjectiveParameters& params, const double* d_free, std::vector<double>* objective,
+                     std::vector<double>* terms);
   void getSegments(size_t b, Segment::Vector* segments) const;
 
   int N_;

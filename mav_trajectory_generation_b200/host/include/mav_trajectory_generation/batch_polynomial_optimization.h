@@ -78,6 +78,20 @@ class BatchPolynomialOptimization {
                      std::vector<double>* sampling_times = nullptr) const {
     core_.evaluateRange(t_start, t_end, dt, derivatives, max_samples, samples, n_samples, sampling_times);
   }
+  // PolynomialOptimization::computeMaximumOfMagnitude (reference impl/polynomial_optimization_linear_impl.h:465-497) of
+  // every trajectory for each derivative order (each in [0, N-2], at most 8): maxima[b * derivatives.size() + q].
+  void computeMaximaOfMagnitude(const std::vector<int>& derivatives, std::vector<Extremum>* maxima) const {
+    core_.computeMaximaOfMagnitude(derivatives, maxima);
+  }
+  // The nonlinear optimiser's objective for every problem at its current segment times (reference
+  // impl/polynomial_optimization_nonlinear_impl.h): objectiveFunctionTime when d_free is nullptr (solve), otherwise
+  // objectiveFunctionTimeAndConstraints with d_free [B][D][n_free] (setFreeConstraints).  objective[b] is NaN where
+  // status()[b] != 0; terms[3 * b + {0, 1, 2}] = trajectory, time and soft-constraint cost.  The evaluated
+  // trajectories replace coefficients().
+  bool timeObjective(const b200::TimeObjectiveParameters& params, const double* d_free, std::vector<double>* objective,
+                     std::vector<double>* terms = nullptr) {
+    return core_.timeObjective(params, d_free, objective, terms);
+  }
 
  private:
   b200::BatchCore core_;

@@ -567,6 +567,44 @@ void BatchCore::evaluateRange(double t_start, double t_end, double dt, const std
   CHECK_EQ(rc, MTG_OK) << mtg_last_error(h);
 }
 
+void BatchCore::computeMaximaOfMagnitude(const std::vector<int>& derivatives, std::vector<Extremum>* maxima) const {
+  CHECK(!derivatives.empty() && derivatives.size() <= 8);
+  const size_t nd = derivatives.size();
+  std::vector<int32_t> ders(derivatives.begin(), derivatives.end());
+  std::vector<double> value(B_ * nd), time(B_ * nd);
+  std::vector<int32_t> segment(B_ * nd);
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_max_magnitude_batch_host_f64(h, N_, topo_.K, topo_.D, static_cast<int64_t>(B_), times_, coeffs_,
+                                                  static_cast<int32_t>(nd), ders.data(), value.data(), time.data(),
+                                                  segment.data(), nullptr);
+  CHECK_EQ(rc, MTG_OK) << mtg_last_error(h);
+  CHECK_NOTNULL(maxima)->resize(B_ * nd);
+  for (size_t i = 0; i < B_ * nd; ++i) (*maxima)[i] = Extremum(time[i], value[i], segment[i]);
+}
+
+bool BatchCore::timeObjective(const TimeObjectiveParameters& params, const double* d_free, std::vector<double>* objective,
+                              std::vector<double>* terms) {
+  CHECK_GT(B_, 0u) << "setup first";
+  CHECK_LE(params.soft_constraints.size(), 8u);
+  std::vector<mtg_soft_constraint> cons;
+  for (const auto& c : params.soft_constraints) cons.push_back({c.first, c.second});
+  mtg_time_objective obj = {params.richter_time ? 1 : 0, params.time_penalty, params.soft_constraint_weight,
+                            params.maximum_cost, static_cast<int32_t>(cons.size()), cons.data()};
+  CHECK_NOTNULL(objective)->assign(B_, 0.0);
+  if (terms) terms->assign(3 * B_, 0.0);
+  mtg_problem p = {N_, topo_.r, topo_.K, topo_.D, topo_.mask.data()};
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_time_objective_batch_host_f64(h, &p, static_cast<int64_t>(B_), times_, d_fixed_, d_free, &obj,
+                                                   coeffs_, objective->data(), terms ? terms->data() : nullptr, status_);
+  if (rc != MTG_OK) {
+    LOG(ERROR) << "mtg_time_objective_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+    return false;
+  }
+  return true;
+}
+
 void BatchCore::getSegments(size_t b, Segment::Vector* segments) const {
   CHECK_LT(b, B_);
   unpackSegments(topo_, coeffs_ + b * size_t(topo_.K) * topo_.D * N_, times_ + b * topo_.K, segments);
