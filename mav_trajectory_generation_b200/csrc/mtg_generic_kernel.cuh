@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(128) backsub_kernel(const GenericParams prm) {
     const int nf = prm.n_fixed, np = prm.n_free;
     int stat = 0;
     for (int i = 0; i < prm.K; ++i)
-      if (!(prm.times[traj * prm.K + i] > 0.0)) stat |= kStatusBadTime;
+      if (bad_segment_time(prm.times[traj * prm.K + i])) stat |= kStatusBadTime;
     back_substitute(prm, traj, [&](int col, int d) -> double {
       return col < nf ? fx[d * nf + col] : fr[d * np + (col - nf)];
     });
@@ -138,7 +138,7 @@ __global__ void __launch_bounds__(128) generic_solve_kernel(const GenericParams 
     // ---- assemble R_pp (banded lower) and -R_pf d_f
     for (int i = 0; i < K; ++i) {
       const double T = prm.times[traj * K + i];
-      if (!(T > 0.0)) stat |= kStatusBadTime;
+      if (bad_segment_time(T)) stat |= kStatusBadTime;
       const double iT = 1.0 / T;
       double sp[MTG_MAX_N_HALF];
       sp[0] = 1.0;
@@ -173,7 +173,7 @@ __global__ void __launch_bounds__(128) generic_solve_kernel(const GenericParams 
         if (j < i) {
           BAND(i, i - j) = s * BAND(j, 0);
         } else {
-          if (!(s > 0.0)) stat |= kStatusNotSpd;
+          if (!(s > 0.0) || isinf(s)) stat |= kStatusNotSpd;
           BAND(i, 0) = rsqrt(s);
         }
       }

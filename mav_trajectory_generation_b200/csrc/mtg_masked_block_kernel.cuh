@@ -122,8 +122,8 @@ __global__ void __launch_bounds__(128, 2)
     for (int v = 0; v <= K; ++v) {
       if (v < K) {
         const double T = __ldg(tt + v);
-        if (!(T > 0.0) || isinf(T)) stat |= kStatusBadTime;  // +inf too: a segment between two fully fixed
-                                                              // vertices reaches no pivot
+        if (bad_segment_time(T)) stat |= kStatusBadTime;  // +inf too: a segment between two fully fixed
+                                                          // vertices reaches no pivot
         seg_powers(T, pwc);
         mn = free_mask(v + 1);
       } else {

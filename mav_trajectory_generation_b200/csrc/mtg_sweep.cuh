@@ -133,7 +133,8 @@ struct Sweep {
     assemble_impl<true>(pw, Cee, cps, cpe, bcar, Wp, yp, xm, xc, xn, Dp, E, bb);
   }
 
-  // Cholesky of a symmetric block (lower triangle read) with inverse pivots; a pivot that is not > 0 sets kStatusNotSpd
+  // Cholesky of a symmetric block (lower triangle read) with inverse pivots; a pivot that is not > 0 or is infinite sets
+  // kStatusNotSpd
   static __device__ __forceinline__ void cholesky(const double (&A)[m][m], double (&L)[m][m], double (&inv)[m],
                                                   int& stat) {
 #pragma unroll
@@ -141,7 +142,7 @@ struct Sweep {
       double s = A[j][j];
 #pragma unroll
       for (int k = 0; k < j; ++k) s = fma(-L[j][k], L[j][k], s);
-      if (!(s > 0.0)) stat |= kStatusNotSpd;
+      if (!(s > 0.0) || isinf(s)) stat |= kStatusNotSpd;
       inv[j] = fast_rsqrt(s);
 #pragma unroll
       for (int i = j + 1; i < m; ++i) {

@@ -192,7 +192,7 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
       }
       const double T0 = *PRO(kPro - 1);
       stash[size_t(D) * kThreads] = T0;
-      if (!(T0 > 0.0)) stat |= kStatusBadTime;
+      if (bad_segment_time(T0)) stat |= kStatusBadTime;
       const double iT0 = fast_rcp(T0);
       double pw[N - 1];
       segment_powers<N, R>(T0, iT0, pw);
@@ -213,7 +213,7 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
         T = *PF(v % RD, 0);
         if (v + RD - 1 <= nh) ring_issue(P, v + RD - 1);  // nothing is left in flight after the last own step
         cp_async_commit();
-        if (!(T > 0.0)) stat |= kStatusBadTime;
+        if (bad_segment_time(T)) stat |= kStatusBadTime;
         const double iT = fast_rcp(T);
         double pw[N - 1];
         segment_powers<N, R>(T, iT, pw);

@@ -54,7 +54,7 @@ __global__ void __launch_bounds__(32) twisted_solve_kernel(const WaypointParams 
   double xnn[D];   // prefetched position of own-frame vertex v+1 for the next iteration
   {
     const double T0 = __ldg(tt + fr.seg(0));
-    if (!(T0 > 0.0)) stat |= kStatusBadTime;
+    if (bad_segment_time(T0)) stat |= kStatusBadTime;
     const double iT0 = fast_rcp(T0);
     double pw[N - 1];
     segment_powers<N, R>(T0, iT0, pw);
@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(32) twisted_solve_kernel(const WaypointParams 
 #pragma unroll
         for (int d = 0; d < D; ++d) xnn[d] = __ldg(fx + d * nf + pn);
       }
-      if (!(T > 0.0)) stat |= kStatusBadTime;
+      if (bad_segment_time(T)) stat |= kStatusBadTime;
       const double iT = fast_rcp(T);
       double pw[N - 1];
       segment_powers<N, R>(T, iT, pw);

@@ -285,7 +285,7 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
     } else {
       T0 = time_of(T0e, fr.seg(0));
     }
-    if (!(T0 > 0.0)) stat |= kStatusBadTime;
+    if (bad_segment_time(T0)) stat |= kStatusBadTime;
     HT(0) = T0;
     const double iT0 = fast_rcp(T0);
     double pw[N - 1];
@@ -314,7 +314,7 @@ __global__ void __launch_bounds__(kTmemThreads, (N <= 8 ? 3 : 2))
         const int vn = v + 2 <= K ? v + 2 : K;
         pf_issue((v + 1) & 1, jn, vn);
       }
-      if (!(T > 0.0)) stat |= kStatusBadTime;
+      if (bad_segment_time(T)) stat |= kStatusBadTime;
       const double iT = fast_rcp(T);
       double pw[N - 1];
       segment_powers<N, R>(T, iT, pw);

@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       } else {
         T0 = *PRO(kPro - 1);
       }
-      if (!(T0 > 0.0)) stat |= kStatusBadTime;
+      if (bad_segment_time(T0)) stat |= kStatusBadTime;
       HT(0) = T0;
       const double iT0 = fast_rcp(T0);
       double pw[N - 1];
@@ -211,7 +211,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         HT(v) = T;
         if (v + RD - 1 <= nh) ring_issue(P, v + RD - 1);  // nothing is left in flight after the last own step
         cp_async_commit();
-        if (!(T > 0.0)) stat |= kStatusBadTime;
+        if (bad_segment_time(T)) stat |= kStatusBadTime;
         const double iT = fast_rcp(T);
         double pw[N - 1];
         segment_powers<N, R>(T, iT, pw);

@@ -222,7 +222,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       } else {
         T0 = in_T(0);
       }
-      if (!(T0 > 0.0)) stat |= kStatusBadTime;
+      if (bad_segment_time(T0)) stat |= kStatusBadTime;
       const double iT0 = fast_rcp(T0);
       double pw[N - 1];
       segment_powers<N, R>(T0, iT0, pw);
@@ -244,7 +244,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         } else {
           T = in_T(v);
         }
-        if (!(T > 0.0)) stat |= kStatusBadTime;
+        if (bad_segment_time(T)) stat |= kStatusBadTime;
         const double iT = fast_rcp(T);
         double pw[N - 1];
         segment_powers<N, R>(T, iT, pw);

@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(32) waypoint_solve_kernel(const WaypointParams
   double xm[D], xc[D];
   {
     const double T0 = __ldg(tt);
-    if (!(T0 > 0.0)) stat |= kStatusBadTime;
+    if (bad_segment_time(T0)) stat |= kStatusBadTime;
     const double iT0 = fast_rcp(T0);
     double pw[N - 1];
     segment_powers<N, R>(T0, iT0, pw);
@@ -193,7 +193,7 @@ __global__ void __launch_bounds__(32) waypoint_solve_kernel(const WaypointParams
 
   for (int v = 1; v < K; ++v) {
     const double T = __ldg(tt + v);
-    if (!(T > 0.0)) stat |= kStatusBadTime;
+    if (bad_segment_time(T)) stat |= kStatusBadTime;
     const double iT = fast_rcp(T);
     double pw[N - 1];
     segment_powers<N, R>(T, iT, pw);
