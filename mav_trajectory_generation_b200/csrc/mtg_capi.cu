@@ -51,12 +51,10 @@ struct mtg_handle {
   std::string error;
   int64_t launches = 0;
   int waypoint_variant = 0;  // MTG_OPT_WAYPOINT_VARIANT
-  int ring_depth = 3;        // MTG_OPT_RING_DEPTH (v4 kernel: cp.async input ring buffers, 2..4)
   int early_steps = 0;       // MTG_OPT_EARLY_REFILL (v5, single tile buffer): 0 = on (kV5Early steps of lead), -1 = off
   int ctas_per_sm = 0;       // MTG_OPT_CTAS_PER_SM (v4 kernel: 0 = as many as fit, 9 = one CTA per tile, not persistent;
                              // chunked kernel: cap on resident warps per SM)
-  int stagger_us = 0;        // MTG_OPT_STAGGER_US (v4 kernel: CTA start times spread over this many microseconds)
-  int tma_inputs = 2;        // MTG_OPT_TMA_INPUTS (default routing prefers the TMA-input kernel v5 when eligible)
+  int tma_inputs = 2;       // MTG_OPT_TMA_INPUTS (default routing prefers the TMA-input kernel v5 when eligible)
   int mellinger_unfused = 0; // MTG_OPT_MELLINGER_UNFUSED (1 = expand + solve + cost kernels, the round-1 path)
   int generic_variant = 0;   // MTG_OPT_GENERIC_VARIANT (0 = masked block kernel, 1 = banded kernel in global scratch)
   int chunk_blocks = 0;      // MTG_OPT_CHUNK_BLOCKS (chunked kernel: resident vertex blocks per lane, 0 = auto)
@@ -80,18 +78,16 @@ struct mtg_handle {
   Arena pack[kPipe + 1];     // times + d_fixed produced by nfabian_pack_kernel; Mellinger expansion
   Arena counters[kPipe + 1]; // dynamic tile counter of the persistent kernels (event-ordered like the scratch arenas: two
                              // launches of one slot on different caller streams must not share a live counter)
-  // cached launch plans of the v3 kernel (per waypoint entry and K): attributes are set once
-  struct TmemPlan {
-    const void* entry = nullptr;
-    int K = 0;
-    int ctas = 0;
-    size_t smem = 0;
+  // What is known about each kernel function launched so far, queried or set once per function so that a repeated
+  // B = 1 solveLinear() call makes no attribute call.  The dynamic shared memory limit is a property of the function
+  // (shared by every K routed to it): only ever raised.
+  struct FnInfo {
+    const void* fn;
+    int regs;             // cudaFuncGetAttributes().numRegs
+    size_t max_dyn_smem;  // cudaFuncAttributeMaxDynamicSharedMemorySize as last set (0: never)
+    int carveout;         // cudaFuncAttributePreferredSharedMemoryCarveout as last set (-1: never)
   };
-  std::vector<TmemPlan> plans;
-  // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of the FUNCTION (shared by every K routed to it):
-  // remember the largest value set so far and only ever raise it
-  std::vector<std::pair<const void*, size_t>> smem_set;
-  std::vector<std::pair<const void*, int>> regs_of;  // cudaFuncGetAttributes().numRegs, queried once per function
+  std::vector<FnInfo> fns;
   // cached residency of the chunked kernel per (function, dynamic shared memory, CTA cap)
   struct ChunkedPlan {
     const void* fn = nullptr;
@@ -101,12 +97,11 @@ struct mtg_handle {
     int carveout = 0;  // cudaFuncAttributePreferredSharedMemoryCarveout for these CTAs
   };
   std::vector<ChunkedPlan> chunked_plans;
-  std::vector<std::pair<const void*, int>> carveout_set;  // carveout last set per function
-  // last encoded tensor map (B = 1 solveLinear() calls re-use the same output buffer)
+  // last encoded coefficient tensor map (B = 1 solveLinear() calls re-use the same output buffer)
   struct TmapKey {
     const void* base = nullptr;
     int64_t B = 0;
-    int K = 0, D = 0, N = 0;
+    int K = 0, D = 0, N = 0, box = 0;
   } tmap_key;
   CUtensorMap tmap_cached;
   cudaStream_t streams[kPipe] = {nullptr, nullptr, nullptr};
@@ -126,6 +121,13 @@ bool set_err(mtg_handle* h, const char* what, cudaError_t e) {
   do {                                            \
     cudaError_t e__ = (call);                     \
     if (set_err(h, #call, e__)) return MTG_ERR_CUDA; \
+  } while (0)
+
+// return the status of `expr` unless it is MTG_OK
+#define MTG_TRY(expr)                  \
+  do {                                 \
+    const int rc__ = (expr);           \
+    if (rc__ != MTG_OK) return rc__;   \
   } while (0)
 
 bool valid_problem(const mtg_problem* p) {
@@ -187,119 +189,104 @@ void compute_layout(int N, int K, const std::vector<uint8_t>& mask, Layout* L) {
   L->waypoint = wp && h >= 2;
 }
 
-// ---- waypoint kernel registry ---------------------------------------------------------
+// ---- waypoint kernel table: one row per compiled (N, r, D) -----------------------------------
 // depth of the cp.async input ring of the v4 and chunked instantiations (their layouts depend on it)
 constexpr int kRingDepth = 3;
-typedef void (*WaypointKernel)(const mtg::WaypointParams);
-typedef void (*ChunkedKernel)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap);
-// warps per CTA of the chunked kernel's instantiations (WaypointEntry::fn_chunked)
-constexpr int kChunkedWarps[2] = {1, 4};
-struct WaypointEntry {
-  int N, R, D, slots;
-  WaypointKernel fn;          // one thread per trajectory
-  WaypointKernel fn_twisted;  // two lanes per trajectory (twisted factorisation)
-  void (*fn_tmem)(const mtg::WaypointParams, const CUtensorMap);  // + shared-memory state, TMA stores
-  void (*fn_tmem_fused)(const mtg::WaypointParams, const CUtensorMap);  // + fused Nfabian
-  size_t (*tmem_smem)(int K);  // dynamic shared memory of fn_tmem / fn_tmem_fused (mtg::V3Layout)
-  ChunkedKernel fn_chunked[2];      // any K (K3), kChunkedWarps[i] warps per CTA
-  size_t (*chunked_smem[2])(int C);  // dynamic shared memory of fn_chunked[i] with C resident blocks (mtg::ChunkedLayout)
-  int chunked_park_slots;         // doubles per thread of one vertex block that fn_chunked parks in global memory
-};
-#define MTG_WP_(N_, R_, D_, V1_)                                                                                  \
-  {                                                                                                               \
-    N_, R_, D_, mtg::sweep_state_slots<N_, D_>(), V1_, mtg::twisted_solve_kernel<N_, R_, D_>,                     \
-        mtg::twisted_tmem_kernel<N_, R_, D_>, mtg::twisted_tmem_kernel<N_, R_, D_, true>,                         \
-        mtg::V3Layout<N_, D_>::bytes,                                                                             \
-        {mtg::twisted_chunked_kernel<N_, R_, D_, kRingDepth, 1>, mtg::twisted_chunked_kernel<N_, R_, D_, kRingDepth, 4>}, \
-        {mtg::ChunkedLayout<N_, D_, kRingDepth, 1>::bytes, mtg::ChunkedLayout<N_, D_, kRingDepth, 4>::bytes},    \
-        mtg::ChunkedLayout<N_, D_, kRingDepth, 4>::kPark                                                          \
-  }
-#define MTG_WP(N_, R_, D_) MTG_WP_(N_, R_, D_, (mtg::waypoint_solve_kernel<N_, R_, D_>))
-// v1 (thread per trajectory) is kept for the headline shapes only (cross-check / profiles)
-#define MTG_WP2(N_, R_, D_) MTG_WP_(N_, R_, D_, nullptr)
-const WaypointEntry kWaypointKernels[] = {
-    MTG_WP(10, 4, 3),  MTG_WP(10, 4, 1),  MTG_WP2(10, 4, 2), MTG_WP2(10, 4, 4),   // min snap, N = 10
-    MTG_WP(10, 3, 3),  MTG_WP2(10, 3, 1), MTG_WP(10, 2, 3),  MTG_WP2(10, 2, 1),   // jerk / acceleration on N = 10
-    MTG_WP(8, 3, 3),   MTG_WP(8, 3, 1),   MTG_WP2(8, 3, 2),  MTG_WP2(8, 3, 4),    // min jerk, N = 8
-    MTG_WP(12, 5, 3),  MTG_WP2(12, 5, 1), MTG_WP2(12, 5, 4),                      // N = 12 (feasibility tests)
-    MTG_WP2(6, 2, 3),  MTG_WP2(6, 2, 1),                                          // min acceleration, N = 6
-};
-
-// ---- cost-only kernels (computeCost of the solution without writing coefficients; Mellinger expansion on the fly)
-typedef void (*TmemKernel)(const mtg::WaypointParams, const CUtensorMap);
-struct CostEntry {
-  int N, R, D;
-  TmemKernel fn;
-  size_t (*smem)(int K);
-};
-#define MTG_COST(N_, R_, D_) {N_, R_, D_, mtg::twisted_tmem_kernel<N_, R_, D_, false, true>, mtg::V3Layout<N_, D_>::bytes}
-const CostEntry kCostKernels[] = {MTG_COST(10, 4, 3), MTG_COST(10, 4, 1), MTG_COST(10, 4, 4), MTG_COST(10, 3, 3),
-                                  MTG_COST(10, 2, 3), MTG_COST(8, 3, 3),  MTG_COST(12, 5, 3)};
-const CostEntry* find_cost(const mtg_problem* p) {
-  for (const auto& e : kCostKernels)
-    if (e.N == p->N && e.R == p->r && e.D == p->D) return &e;
-  return nullptr;
-}
-
-// ---- v4 (persistent, deep input prefetch) kernels: the default for short trajectories (K <= 8), where the per-tile
-// prologue of the per-tile kernel is a large share of a tile
-typedef void (*V4Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV4, const CUtensorMap);
-struct V4Entry {
-  int N, R, D;
-  V4Kernel fn, fn_fused;
-  size_t (*smem)(int K);
-};
-#define MTG_V4(N_, R_, D_, MB_)                                                                    \
-  {                                                                                                \
-    N_, R_, D_, mtg::twisted_tmem_v4_kernel<N_, R_, D_, false, kRingDepth, MB_>,                  \
-        mtg::twisted_tmem_v4_kernel<N_, R_, D_, true, kRingDepth, MB_>,                            \
-        mtg::V4Layout<N_, D_, kRingDepth>::bytes                                                   \
-  }
-const V4Entry kV4Kernels[] = {MTG_V4(10, 4, 3, 2), MTG_V4(8, 3, 3, 3), MTG_V4(10, 4, 1, 2), MTG_V4(10, 3, 3, 2),
-                              MTG_V4(10, 2, 3, 2), MTG_V4(12, 5, 3, 2)};
-constexpr int kV4MaxK = 8;
-
-// ---- v5: v4 with the inputs moved by TMA bulk copies (whole 16-trajectory tiles, double buffered when two fit)
-typedef void (*V5Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV5, const CUtensorMap);
-// lead (outward-sweep steps) of the single-buffer tile refill
+// lead (outward-sweep steps) of v5's single-buffer tile refill
 constexpr int kV5Early = 2;
-struct V5Entry {
+// v4 is the default for short trajectories (K <= 8), where the per-tile prologue of v3 is a large share of a tile
+constexpr int kV4MaxK = 8;
+// warps per CTA of the chunked kernel's instantiations (WaypointEntry::k3)
+constexpr int kChunkedWarps[2] = {1, 4};
+typedef void (*SweepKernel)(const mtg::WaypointParams);                    // v1, v2
+typedef void (*TmemKernel)(const mtg::WaypointParams, const CUtensorMap);  // v3, cost-only
+typedef void (*V4Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV4, const CUtensorMap);
+typedef void (*V5Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV5, const CUtensorMap);
+typedef void (*ChunkedKernel)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap);
+struct WaypointEntry {
   int N, R, D;
-  V5Kernel fn, fn_fused;
-  V5Kernel fn_early, fn_fused_early;  // the EARLY = kV5Early instantiations
-  size_t (*smem)(int K, int nf, int nbuf), (*smem_fused)(int K, int nf, int nbuf);
-  bool (*early_fits)(int K);  // the EARLY instantiations may run for this K
+  SweepKernel v2;                 // two lanes per trajectory (twisted factorisation), state in shared memory
+  size_t (*v2_smem)(int K);
+  TmemKernel v3, v3_fused;        // + 128-thread CTAs, TMA tensor stores; fused Nfabian
+  size_t (*v3_smem)(int K);
+  ChunkedKernel k3[2];            // K3: any K, kChunkedWarps[i] warps per CTA
+  size_t (*k3_smem[2])(int C);    // with C resident blocks per lane
+  int k3_park;                    // doubles per thread of one vertex block that K3 parks in global memory
+  // null where the shape has no such instantiation
+  SweepKernel v1;                 // one thread per trajectory (cross-checks and profiles)
+  size_t (*v1_smem)(int K);
+  V4Kernel v4, v4_fused;          // persistent, deep input prefetch
+  size_t (*v4_smem)(int K);
+  V5Kernel v5, v5_fused;          // v4 with the inputs moved by TMA bulk copies
+  V5Kernel v5_early, v5_fused_early;  // the EARLY = kV5Early instantiations
+  size_t (*v5_smem)(int K, int nf, int nbuf), (*v5_fused_smem)(int K, int nf, int nbuf);
+  bool (*early_fits)(int K);      // the EARLY instantiations may run for this K
+  TmemKernel cost;                // computeCost of the solution without writing coefficients (v3 layout)
 };
-#define MTG_V5(N_, R_, D_, MB_)                                                                                       \
-  {N_, R_, D_, mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, false>, mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, true>, \
-   mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, false, kV5Early>, mtg::twisted_tmem_v5_kernel<N_, R_, D_, MB_, true, kV5Early>, \
-   mtg::V5Layout<N_, D_, false>::bytes, mtg::V5Layout<N_, D_, true>::bytes,                                          \
-   mtg::V5Layout<N_, D_, false>::early_fits<kV5Early>}
-const V5Entry kV5Kernels[] = {MTG_V5(10, 4, 3, 2), MTG_V5(8, 3, 3, 3),  MTG_V5(10, 4, 1, 2),
-                              MTG_V5(10, 3, 3, 2), MTG_V5(10, 2, 3, 2), MTG_V5(12, 5, 3, 2)};
-const V5Entry* find_v5(const mtg_problem* p) {
-  for (const auto& e : kV5Kernels)
-    if (e.N == p->N && e.R == p->r && e.D == p->D) return &e;
-  return nullptr;
+enum : int { kV1 = 1, kCost = 2 };
+// The row of (N, R, D).  FLAGS adds v1 and the cost-only kernel; MINB > 0 adds v4 and v5 with MINB blocks per SM in
+// their launch bounds.
+template <int N, int R, int D, int FLAGS = 0, int MINB = 0>
+WaypointEntry waypoint_row() {
+  WaypointEntry e{};
+  e.N = N;
+  e.R = R;
+  e.D = D;
+  e.v2 = mtg::twisted_solve_kernel<N, R, D>;
+  e.v2_smem = mtg::V2Layout<N, D>::bytes;
+  e.v3 = mtg::twisted_tmem_kernel<N, R, D>;
+  e.v3_fused = mtg::twisted_tmem_kernel<N, R, D, true>;
+  e.v3_smem = mtg::V3Layout<N, D>::bytes;
+  e.k3[0] = mtg::twisted_chunked_kernel<N, R, D, kRingDepth, 1>;
+  e.k3[1] = mtg::twisted_chunked_kernel<N, R, D, kRingDepth, 4>;
+  e.k3_smem[0] = mtg::ChunkedLayout<N, D, kRingDepth, 1>::bytes;
+  e.k3_smem[1] = mtg::ChunkedLayout<N, D, kRingDepth, 4>::bytes;
+  e.k3_park = mtg::ChunkedLayout<N, D, kRingDepth, 4>::kPark;
+  if constexpr ((FLAGS & kV1) != 0) {
+    e.v1 = mtg::waypoint_solve_kernel<N, R, D>;
+    e.v1_smem = mtg::V1Layout<N, D>::bytes;
+  }
+  if constexpr (MINB > 0) {
+    e.v4 = mtg::twisted_tmem_v4_kernel<N, R, D, false, kRingDepth, MINB>;
+    e.v4_fused = mtg::twisted_tmem_v4_kernel<N, R, D, true, kRingDepth, MINB>;
+    e.v4_smem = mtg::V4Layout<N, D, kRingDepth>::bytes;
+    e.v5 = mtg::twisted_tmem_v5_kernel<N, R, D, MINB, false>;
+    e.v5_fused = mtg::twisted_tmem_v5_kernel<N, R, D, MINB, true>;
+    e.v5_early = mtg::twisted_tmem_v5_kernel<N, R, D, MINB, false, kV5Early>;
+    e.v5_fused_early = mtg::twisted_tmem_v5_kernel<N, R, D, MINB, true, kV5Early>;
+    e.v5_smem = mtg::V5Layout<N, D, false>::bytes;
+    e.v5_fused_smem = mtg::V5Layout<N, D, true>::bytes;
+    e.early_fits = mtg::V5Layout<N, D, false>::template early_fits<kV5Early>;
+  }
+  if constexpr ((FLAGS & kCost) != 0) e.cost = mtg::twisted_tmem_kernel<N, R, D, false, true>;
+  return e;
 }
+const WaypointEntry kWaypoints[] = {
+    // min snap, N = 10
+    waypoint_row<10, 4, 3, kV1 | kCost, 2>(), waypoint_row<10, 4, 1, kV1 | kCost, 2>(), waypoint_row<10, 4, 2>(),
+    waypoint_row<10, 4, 4, kCost>(),
+    // jerk / acceleration on N = 10
+    waypoint_row<10, 3, 3, kV1 | kCost, 2>(), waypoint_row<10, 3, 1>(), waypoint_row<10, 2, 3, kV1 | kCost, 2>(),
+    waypoint_row<10, 2, 1>(),
+    // min jerk, N = 8
+    waypoint_row<8, 3, 3, kV1 | kCost, 3>(), waypoint_row<8, 3, 1, kV1>(), waypoint_row<8, 3, 2>(),
+    waypoint_row<8, 3, 4>(),
+    // N = 12 (feasibility tests)
+    waypoint_row<12, 5, 3, kV1 | kCost, 2>(), waypoint_row<12, 5, 1>(), waypoint_row<12, 5, 4>(),
+    // min acceleration, N = 6
+    waypoint_row<6, 2, 3>(), waypoint_row<6, 2, 1>(),
+};
 
-const V4Entry* find_v4(const mtg_problem* p) {
-  for (const auto& e : kV4Kernels)
-    if (e.N == p->N && e.R == p->r && e.D == p->D) return &e;
-  return nullptr;
-}
-
-const WaypointEntry* find_waypoint(const mtg_handle* h, const mtg_problem* p, const Layout& L) {
+const WaypointEntry* find_waypoint(const mtg_problem* p, const Layout& L) {
   if (!L.waypoint) return nullptr;
-  for (const auto& e : kWaypointKernels)
+  for (const auto& e : kWaypoints)
     if (e.N == p->N && e.R == p->r && e.D == p->D) return &e;  // any K: the chunked kernel has a fixed footprint
-  (void)h;
   return nullptr;
 }
 
-int route(const mtg_handle* h, const mtg_problem* p, const Layout& L) {
+int route(const mtg_problem* p, const Layout& L) {
   if (L.n_free == 0) return MTG_KERNEL_NOFREE;
-  if (find_waypoint(h, p, L)) return MTG_KERNEL_WAYPOINT;
+  if (find_waypoint(p, L)) return MTG_KERNEL_WAYPOINT;
   return MTG_KERNEL_GENERIC;
 }
 
@@ -359,38 +346,39 @@ int arena_release(mtg_handle* h, mtg_handle::Arena& a, cudaStream_t stream) {
 // zeroed dynamic-tile counter of pipeline slot `slot`, ordered after the previous launch that used it
 int tile_counter_acquire(mtg_handle* h, int slot, cudaStream_t stream, unsigned long long** out) {
   mtg_handle::Arena& a = h->counters[slot];
-  const int rc = arena_acquire(h, a, 256, stream);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(arena_acquire(h, a, 256, stream));
   *out = reinterpret_cast<unsigned long long*>(a.p);
   MTG_CUDA(h, cudaMemsetAsync(*out, 0, sizeof(unsigned long long), stream));
   return MTG_OK;
 }
 
+// The cached facts of `fn`: its registers are queried on first use.  Null (and h->error set) when the query fails.
+mtg_handle::FnInfo* fn_info(mtg_handle* h, const void* fn) {
+  for (auto& f : h->fns)
+    if (f.fn == fn) return &f;
+  cudaFuncAttributes attr;
+  if (set_err(h, "cudaFuncGetAttributes", cudaFuncGetAttributes(&attr, fn))) return nullptr;
+  h->fns.push_back({fn, attr.numRegs, 0, -1});
+  return &h->fns.back();
+}
+
 // Make sure `fn` may be launched with `bytes` of dynamic shared memory (raises the function attribute when needed).
 int ensure_dyn_smem(mtg_handle* h, const void* fn, size_t bytes) {
-  for (auto& kv : h->smem_set)
-    if (kv.first == fn) {
-      if (kv.second >= bytes) return MTG_OK;
-      MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-      kv.second = bytes;
-      return MTG_OK;
-    }
+  mtg_handle::FnInfo* f = fn_info(h, fn);
+  if (!f) return MTG_ERR_CUDA;
+  if (bytes <= f->max_dyn_smem) return MTG_OK;
   MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  h->smem_set.emplace_back(fn, bytes);
+  f->max_dyn_smem = bytes;
   return MTG_OK;
 }
 
-// registers per thread of a kernel (cached: a B = 1 solveLinear() call must not pay an attribute query)
-int kernel_regs(mtg_handle* h, const void* fn, int* out) {
-  for (auto& kv : h->regs_of)
-    if (kv.first == fn) {
-      *out = kv.second;
-      return MTG_OK;
-    }
-  cudaFuncAttributes attr;
-  MTG_CUDA(h, cudaFuncGetAttributes(&attr, fn));
-  h->regs_of.emplace_back(fn, attr.numRegs);
-  *out = attr.numRegs;
+// Set the shared memory carveout of `fn` (percent of the SM's maximum), unless it already has that value.
+int set_carveout(mtg_handle* h, const void* fn, int percent) {
+  mtg_handle::FnInfo* f = fn_info(h, fn);
+  if (!f) return MTG_ERR_CUDA;
+  if (f->carveout == percent) return MTG_OK;
+  MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, percent));
+  f->carveout = percent;
   return MTG_OK;
 }
 
@@ -406,9 +394,9 @@ struct DeviceGuard {
   }
 };
 
-// coeffs as a 2-D fp64 tensor [B][K*D*N] for the TMA stores (box = 16 trajectories x one segment)
-int encode_coeff_tmap(mtg_handle* h, CUtensorMap* out, double* coeffs, int64_t B, const mtg_problem* p,
-                      int box_inner = 0) {
+// coeffs as a 2-D fp64 tensor [B][K*D*N] for the TMA stores (box = 16 trajectories x `box` doubles of one segment).
+// The last encoded map is kept: repeated calls on the same output buffer encode it once.
+int coeff_tmap(mtg_handle* h, double* coeffs, int64_t B, const mtg_problem* p, int box, const CUtensorMap** out) {
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -421,6 +409,11 @@ int encode_coeff_tmap(mtg_handle* h, CUtensorMap* out, double* coeffs, int64_t B
       return nullptr;
     return reinterpret_cast<EncodeFn>(fp);
   }();
+  mtg_handle::TmapKey& key = h->tmap_key;
+  *out = &h->tmap_cached;
+  if (key.base == coeffs && key.B == B && key.K == p->K && key.D == p->D && key.N == p->N && key.box == box)
+    return MTG_OK;
+  key.base = nullptr;
   if (!encode) {
     h->error = "cuTensorMapEncodeTiled is not available from the driver";
     return MTG_ERR_CUDA;
@@ -428,15 +421,16 @@ int encode_coeff_tmap(mtg_handle* h, CUtensorMap* out, double* coeffs, int64_t B
   const cuuint64_t row = cuuint64_t(p->K) * p->D * p->N;
   const cuuint64_t dims[2] = {row, cuuint64_t(B)};
   const cuuint64_t strides[1] = {row * sizeof(double)};
-  const cuuint32_t box[2] = {cuuint32_t(box_inner > 0 ? box_inner : p->D * p->N), 16u};
+  const cuuint32_t boxdim[2] = {cuuint32_t(box), 16u};
   const cuuint32_t estr[2] = {1u, 1u};
-  const CUresult cr = encode(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, coeffs, dims, strides, box, estr,
+  const CUresult cr = encode(&h->tmap_cached, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, coeffs, dims, strides, boxdim, estr,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                              CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (cr != CUDA_SUCCESS) {
     h->error = "cuTensorMapEncodeTiled failed (" + std::to_string(int(cr)) + ")";
     return MTG_ERR_CUDA;
   }
+  key = {coeffs, B, p->K, p->D, p->N, box};
   return MTG_OK;
 }
 
@@ -452,24 +446,19 @@ constexpr int kSmemPerSm = 228 * 1024;
 // Resident CTAs per SM of a `threads`-thread kernel with `smem` bytes of dynamic shared memory: limited by its
 // registers, by shared memory and by `cap`; 0 when `smem` exceeds the per-block opt-in limit.
 int resident_ctas(mtg_handle* h, const void* fn, size_t smem, int cap, int threads, int* ctas) {
-  int n_regs = 0;
-  const int rc = kernel_regs(h, fn, &n_regs);
-  if (rc != MTG_OK) return rc;
-  const int by_regs = std::max(1, 65536 / (std::max(n_regs, 1) * threads));
+  const mtg_handle::FnInfo* f = fn_info(h, fn);
+  if (!f) return MTG_ERR_CUDA;
+  const int by_regs = std::max(1, 65536 / (std::max(f->regs, 1) * threads));
   *ctas = smem > h->smem_optin ? 0 : std::min(std::min<int>(by_regs, int(kSmemPerSm / (smem + 1024))), cap);
   return MTG_OK;
 }
 
-// Set the shared memory carveout of `fn` (percent of the SM's maximum), unless it already has that value.
-int set_carveout(mtg_handle* h, const void* fn, int percent) {
-  for (auto& kv : h->carveout_set)
-    if (kv.first == fn) {
-      if (kv.second != percent) MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, percent));
-      kv.second = percent;
-      return MTG_OK;
-    }
-  MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, percent));
-  h->carveout_set.emplace_back(fn, percent);
+// v3 and its cost-only form run while their factor leaves at least two CTAs of `fn` per SM (of at most 16); beyond,
+// the chunked kernel (K3) takes the solve.
+int v3_fits(mtg_handle* h, const void* fn, size_t smem, bool* fits) {
+  int ctas = 0;
+  MTG_TRY(resident_ctas(h, fn, smem, 16, mtg::kTmemThreads, &ctas));
+  *fits = ctas >= 2;
   return MTG_OK;
 }
 
@@ -488,15 +477,12 @@ int chunked_residency(mtg_handle* h, const void* fn, size_t smem, int cap, int t
   np.fn = fn;
   np.smem = smem;
   np.cap = cap;
-  int rc = resident_ctas(h, fn, smem, cap, threads, &np.ctas);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(resident_ctas(h, fn, smem, cap, threads, &np.ctas));
   if (np.ctas > 0) {
-    rc = ensure_dyn_smem(h, fn, smem);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(ensure_dyn_smem(h, fn, smem));
     const size_t need = size_t(np.ctas) * (smem + 1024);
     np.carveout = int(std::min<size_t>(100, (need * 100 + kSmemPerSm - 1) / kSmemPerSm));
-    rc = set_carveout(h, fn, np.carveout);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(set_carveout(h, fn, np.carveout));
     int occ = 0;
     MTG_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, threads, smem));
     np.ctas = std::min(np.ctas, occ);
@@ -507,10 +493,25 @@ int chunked_residency(mtg_handle* h, const void* fn, size_t smem, int cap, int t
   return MTG_OK;
 }
 
+// ---- waypoint launches: plan_waypoint() decides, launch_waypoint() launches -------------------
+enum class Family { Sweep, Tmem, V4, V5, Chunked };  // v1 and v2, v3, v4, v5, K3: fixes the argument list
+struct WaypointPlan {
+  Family family = Family::Sweep;
+  const void* fn = nullptr;
+  int64_t blocks = 0;
+  int threads = 0;
+  size_t smem = 0;            // dynamic shared memory
+  int n_buffers = 0;          // v5: input tile buffers per warp
+  bool tile_counter = false;  // v4, v5: warps draw their tiles from a zeroed global counter
+  int chunk = 0;              // K3: vertex blocks resident per lane
+  size_t park_bytes = 0;      // K3: parking area of the outer vertex blocks (0: nothing is parked)
+  int carveout = -1;          // K3: shared memory carveout in percent (-1: left as it is)
+  int evict_first = 0;        // K3: streamed data marked evict-first in L2
+};
+
 // K3: the chunked twisted kernel -- any K, fixed on-chip footprint; the vertex blocks beyond the C resident ones
 // are parked in global memory.
-int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, const mtg::WaypointParams& prm,
-                   double* coeffs, int64_t B, cudaStream_t stream, int slot) {
+int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, int64_t B, WaypointPlan* pl) {
   const int nmax = (p->K + 1) / 2 - 1;
   // Auto: one-warp CTAs (shared memory then comes in 31-52 KB steps instead of 124-206 KB ones), no L2 hints, at
   // most kAutoParkWarps warps per SM while any block is parked and as many as fit otherwise; among the chunks up to
@@ -538,11 +539,9 @@ int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, 
       if (h->chunk_warps > 0 ? W != h->chunk_warps : W != 1) continue;
       // cap on resident warps per SM
       const int wcap = h->ctas_per_sm > 0 ? h->ctas_per_sm : (nmax > C ? kAutoParkWarps : 64);
-      const size_t smem = e->chunked_smem[i](C);
+      const size_t smem = e.k3_smem[i](C);
       int ctas = 0, carveout = 0;
-      const int rc =
-          chunked_residency(h, (const void*)e->fn_chunked[i], smem, std::max(1, wcap / W), 32 * W, &ctas, &carveout);
-      if (rc != MTG_OK) return rc;
+      MTG_TRY(chunked_residency(h, (const void*)e.k3[i], smem, std::max(1, wcap / W), 32 * W, &ctas, &carveout));
       if (ctas * W > best_warps) {
         best_warps = ctas * W;
         best_ctas = ctas;
@@ -558,38 +557,165 @@ int launch_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry* e, 
     return MTG_ERR_ALLOC;
   }
   const int W = kChunkedWarps[best_i];
-  const void* fn = (const void*)e->fn_chunked[best_i];
-  const int threads = 32 * W;
-  const int64_t ctiles = (B + 16 * W - 1) / (16 * W);
-  const int64_t blocks = std::min<int64_t>(ctiles, int64_t(best_ctas) * h->sm_count);
+  pl->family = Family::Chunked;
+  pl->fn = (const void*)e.k3[best_i];
+  pl->threads = 32 * W;
+  pl->smem = best_smem;
+  pl->blocks = std::min<int64_t>((B + 16 * W - 1) / (16 * W), int64_t(best_ctas) * h->sm_count);
+  pl->chunk = best_C;
   const int npark = nmax - best_C;  // parked vertex blocks per lane
-  mtg::ChunkedLaunch cl;
-  cl.chunk = best_C;
-  cl.ckpt = nullptr;
-  cl.evict_first = h->l2_hints;
-  mtg_handle::Arena& ar = h->scratch[slot];
-  if (npark > 0) {
-    const size_t bytes = size_t(npark) * e->chunked_park_slots * size_t(blocks) * threads * sizeof(double);
-    const int rc = arena_acquire(h, ar, bytes, stream);
-    if (rc != MTG_OK) return rc;
-    cl.ckpt = ar.p;
+  if (npark > 0) pl->park_bytes = size_t(npark) * e.k3_park * size_t(pl->blocks) * pl->threads * sizeof(double);
+  pl->carveout = best_carveout;
+  pl->evict_first = h->l2_hints;
+  return MTG_OK;
+}
+
+// Waypoint routing.  a16 = 16-byte aligned, V = MTG_OPT_WAYPOINT_VARIANT.  Every kernel here stores coefficients in
+// 16-byte units (TMA tensor stores / double2), so a plain call whose output is not a16 (e.g. a tensor slice) has
+// already gone to the banded generic kernel, which stores scalar doubles.  The first rule that applies decides:
+//  1. A fused call whose output is not a16: no fused kernel; the caller packs the inputs and solves.
+//  2. V = 5, plain call: K3.
+//  3. v5 when V = 6, or V = 0 and TMA_INPUTS != 0, with B % 16 == 0, a16 inputs and a v5 instantiation.  Of two and
+//     one input tile buffers per warp, the one with more resident CTAs per SM wins (at most 8; two on a tie).  V = 6
+//     takes it at >= 1 CTA; V = 0 at >= 2 CTAs (with fewer, K3 keeps more warps in flight) and with two buffers, or
+//     with one when TMA_INPUTS = 2.  One buffer is refilled early (EARLY instantiation) unless EARLY_REFILL = -1,
+//     where K leaves room for it and the EARLY kernel's registers keep as many CTAs resident.
+//  4. v4 when V = 4, or V = 0 and K <= 8, with a v4 instantiation, at >= 2 resident CTAs per SM of at most 8 (V = 4:
+//     >= 1), then at most CTAS_PER_SM; CTAS_PER_SM = 9 launches one CTA per tile instead of persistent CTAs.
+//  5. For V in {0, 3, 4, 5, 6}, every fused call, V = 2 when v2's state does not fit in shared memory and V = 1 when
+//     neither v1's nor v2's does: v3 while its factor leaves >= 2 CTAs per SM (counted with the plain kernel's
+//     registers, fused calls too); beyond, K3 for a plain call and no fused kernel for a fused one.
+//  6. V = 1 where v1 is compiled and fits: v1.  Otherwise v2.
+// v5 and v4 draw tiles from a global counter when DYNAMIC_TILES = 1, and in auto mode when every warp has many tiles
+// (v5: >= 8 and K > 8; v4: >= 16), where the counter balances the tail; otherwise tiles go round-robin, since the
+// counter's round trip to L2 is not small against a short tile or amortised over few.  CTAS_PER_SM also caps K3's
+// resident warps (plan_chunked), and has no effect on v5.
+int plan_waypoint(mtg_handle* h, const mtg_problem* p, const Layout& L, const WaypointEntry& e,
+                  const mtg::WaypointParams& prm, bool fused, WaypointPlan* pl) {
+  const auto a16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
+  const int V = h->waypoint_variant, K = p->K;
+  const int64_t B = prm.B;
+  if (!a16(prm.coeffs)) return MTG_ERR_ALLOC;
+  if (V == 5 && !fused) return plan_chunked(h, p, e, B, pl);
+  const bool inputs_a16 = fused ? a16(prm.positions) : a16(prm.times) && a16(prm.dfix);
+  if ((V == 6 || (V == 0 && h->tma_inputs != 0)) && B % 16 == 0 && inputs_a16 && e.v5) {
+    const void* fn = (const void*)(fused ? e.v5_fused : e.v5);
+    int ctas = 0, nbuf = 0;
+    size_t smem = 0;
+    for (int nb = 2; nb >= 1; --nb) {
+      const size_t s = (fused ? e.v5_fused_smem : e.v5_smem)(K, L.n_fixed, nb);
+      int c = 0;
+      MTG_TRY(resident_ctas(h, fn, s, 8, mtg::kTmemThreads, &c));
+      if (c > ctas) {
+        ctas = c;
+        nbuf = nb;
+        smem = s;
+      }
+    }
+    if (ctas >= (V == 6 ? 1 : 2) && (V == 6 || nbuf == 2 || h->tma_inputs == 2)) {
+      pl->family = Family::V5;
+      pl->fn = fn;
+      pl->threads = mtg::kTmemThreads;
+      pl->smem = smem;
+      pl->n_buffers = nbuf;
+      if (nbuf == 1 && h->early_steps >= 0 && e.early_fits(K)) {
+        const void* fe = (const void*)(fused ? e.v5_fused_early : e.v5_early);
+        const mtg_handle::FnInfo* f = fn_info(h, fe);
+        if (!f) return MTG_ERR_CUDA;
+        if (65536 / (std::max(f->regs, 1) * mtg::kTmemThreads) >= ctas) pl->fn = fe;
+      }
+      pl->blocks = std::min<int64_t>((B + 63) / 64, int64_t(ctas) * h->sm_count);
+      const int64_t tiles_per_warp = (B / 16) / std::max<int64_t>(1, pl->blocks * 4);
+      pl->tile_counter = h->dynamic_tiles == 1 || (h->dynamic_tiles == 0 && tiles_per_warp >= 8 && K > kV4MaxK);
+      return MTG_OK;
+    }
   }
-  {
-    int rc = ensure_dyn_smem(h, fn, best_smem);
-    if (rc != MTG_OK) return rc;
-    rc = set_carveout(h, fn, best_carveout);
-    if (rc != MTG_OK) return rc;
+  if ((V == 4 || (V == 0 && K <= kV4MaxK)) && e.v4) {
+    const void* fn = (const void*)(fused ? e.v4_fused : e.v4);
+    const size_t smem = e.v4_smem(K);
+    int ctas = 0;
+    MTG_TRY(resident_ctas(h, fn, smem, 8, mtg::kTmemThreads, &ctas));
+    if (ctas >= (V == 4 ? 1 : 2)) {
+      const bool per_tile = h->ctas_per_sm == 9;
+      if (h->ctas_per_sm > 0 && !per_tile) ctas = std::min(ctas, h->ctas_per_sm);
+      const int64_t tiles = (B + 63) / 64;
+      const int64_t tiles_per_warp = ((B + 15) / 16) / std::max<int64_t>(1, int64_t(ctas) * h->sm_count * 4);
+      pl->family = Family::V4;
+      pl->fn = fn;
+      pl->threads = mtg::kTmemThreads;
+      pl->smem = smem;
+      pl->blocks = per_tile ? tiles : std::min<int64_t>(tiles, int64_t(ctas) * h->sm_count);
+      pl->tile_counter = !per_tile && (h->dynamic_tiles == 1 || (h->dynamic_tiles == 0 && tiles_per_warp >= 16));
+      return MTG_OK;
+    }
   }
-  CUtensorMap tmap;
-  {
-    const int rc = encode_coeff_tmap(h, &tmap, coeffs, B, p);
-    if (rc != MTG_OK) return rc;
+  const bool v1_fits = e.v1 && e.v1_smem(K) <= h->smem_optin;
+  const bool v2_fits = e.v2_smem(K) <= h->smem_optin;
+  if (fused || (V != 1 && V != 2) || (V == 2 && !v2_fits) || (V == 1 && !v1_fits && !v2_fits)) {
+    const size_t smem = e.v3_smem(K);
+    bool fits = false;
+    MTG_TRY(v3_fits(h, (const void*)e.v3, smem, &fits));
+    if (!fits) return fused ? MTG_ERR_ALLOC : plan_chunked(h, p, e, B, pl);
+    pl->family = Family::Tmem;
+    pl->fn = (const void*)(fused ? e.v3_fused : e.v3);
+    pl->blocks = (B + 63) / 64;
+    pl->threads = mtg::kTmemThreads;
+    pl->smem = smem;
+  } else if (V == 1 && v1_fits) {
+    pl->fn = (const void*)e.v1;
+    pl->blocks = (B + 31) / 32;
+    pl->threads = 32;
+    pl->smem = e.v1_smem(K);
+  } else {
+    pl->fn = (const void*)e.v2;
+    pl->blocks = (B + 15) / 16;
+    pl->threads = 32;
+    pl->smem = e.v2_smem(K);
   }
-  e->fn_chunked[best_i]<<<(unsigned)blocks, threads, best_smem, stream>>>(prm, cl, tmap);
+  return MTG_OK;
+}
+
+// The one launch site of the waypoint kernels: tile counter or parking area, function attributes, tensor map,
+// launch, and the release that orders the next user of the counter or parking area after this launch.
+int launch_waypoint(mtg_handle* h, const mtg_problem* p, const WaypointPlan& pl, const mtg::WaypointParams& prm,
+                    cudaStream_t stream, int slot) {
+  mtg_handle::Arena* held = nullptr;
+  unsigned long long* counter = nullptr;
+  if (pl.tile_counter) {
+    MTG_TRY(tile_counter_acquire(h, slot, stream, &counter));
+    held = &h->counters[slot];
+  }
+  if (pl.park_bytes > 0) {
+    held = &h->scratch[slot];
+    MTG_TRY(arena_acquire(h, *held, pl.park_bytes, stream));
+  }
+  MTG_TRY(ensure_dyn_smem(h, pl.fn, pl.smem));
+  if (pl.carveout >= 0) MTG_TRY(set_carveout(h, pl.fn, pl.carveout));
+  const CUtensorMap* tmap = nullptr;
+  if (pl.family != Family::Sweep) MTG_TRY(coeff_tmap(h, prm.coeffs, prm.B, p, p->D * p->N, &tmap));
+  const unsigned grid = (unsigned)pl.blocks;
+  switch (pl.family) {
+    case Family::Sweep:
+      ((SweepKernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm);
+      break;
+    case Family::Tmem:
+      ((TmemKernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm, *tmap);
+      break;
+    case Family::V4:
+      ((V4Kernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm, mtg::TmemLaunchV4{counter}, *tmap);
+      break;
+    case Family::V5:
+      ((V5Kernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm, mtg::TmemLaunchV5{pl.n_buffers, counter}, *tmap);
+      break;
+    case Family::Chunked: {
+      const mtg::ChunkedLaunch cl{pl.chunk, pl.park_bytes > 0 ? held->p : nullptr, pl.evict_first};
+      ((ChunkedKernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm, cl, *tmap);
+      break;
+    }
+  }
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
-  if (npark > 0) return arena_release(h, ar, stream);
-  return MTG_OK;
+  return held ? arena_release(h, *held, stream) : MTG_OK;
 }
 
 // ---- K4: masked block-tridiagonal kernel, any mask; N in {2..12}, dimension groups of 1..4
@@ -627,27 +753,21 @@ int launch_masked(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int
     MaskedKernel fn = kMaskedKernels[p->N / 2 - 1][dg - 1];
     const int kslots = hh * (hh + 1) / 2 + hh * dg;
     const size_t smem = size_t(4) * 32 * dg * p->N * sizeof(double);  // staging tiles of the four warps
-    {
-        const int rc_smem = ensure_dyn_smem(h, (const void*)fn, size_t(smem));
-        if (rc_smem != MTG_OK) return rc_smem;
-      }
+    MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
     int per_sm = 0;
     MTG_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)fn, 128, smem));
     per_sm = std::max(per_sm, 1);
     const int64_t blocks = std::min<int64_t>((B + 127) / 128, int64_t(per_sm) * h->sm_count);
     const size_t bytes = size_t(p->K + 1) * kslots * size_t(blocks) * 128 * sizeof(double);
-    int rc = arena_acquire(h, ar, bytes, stream);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(arena_acquire(h, ar, bytes, stream));
     prm.lifo = ar.p;
     prm.d0 = d0;
-    CUtensorMap tmap;
-    rc = encode_coeff_tmap(h, &tmap, coeffs, B, p, dg * p->N);
-    if (rc != MTG_OK) return rc;
-    fn<<<(unsigned)blocks, 128, smem, stream>>>(prm, tmap);
+    const CUtensorMap* tmap = nullptr;
+    MTG_TRY(coeff_tmap(h, coeffs, B, p, dg * p->N, &tmap));
+    fn<<<(unsigned)blocks, 128, smem, stream>>>(prm, *tmap);
     MTG_CUDA(h, cudaGetLastError());
     h->launches++;
-    rc = arena_release(h, ar, stream);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(arena_release(h, ar, stream));
     d0 += dg;
   }
   return MTG_OK;
@@ -659,39 +779,26 @@ int launch_masked(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int
 int launch_cost_fused(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t nx, const double* times,
                       const double* dfix, double* cost_x, int mel_k1, double inc, double lower, cudaStream_t stream) {
   const Layout& L = topo->layout;
-  const CostEntry* ce = find_cost(p);
-  const WaypointEntry* e = L.waypoint ? find_waypoint(h, p, L) : nullptr;
-  if (!ce || !e || L.n_free == 0) return MTG_ERR_ALLOC;
-  const size_t smem = ce->smem(p->K);
-  int ctas = 0;
-  {
-    const int rc_ctas = resident_ctas(h, (const void*)ce->fn, smem, 16, mtg::kTmemThreads, &ctas);
-    if (rc_ctas != MTG_OK) return rc_ctas;
-  }
-  if (ctas < 2) return MTG_ERR_ALLOC;  // large K: unfused path (chunked kernel + cost kernel)
-  mtg::WaypointParams prm;
+  const WaypointEntry* e = find_waypoint(p, L);
+  if (!e || !e->cost || L.n_free == 0) return MTG_ERR_ALLOC;
+  const size_t smem = e->v3_smem(p->K);
+  bool fits = false;
+  MTG_TRY(v3_fits(h, (const void*)e->cost, smem, &fits));
+  if (!fits) return MTG_ERR_ALLOC;  // large K: unfused path (chunked kernel + cost kernel)
+  mtg::WaypointParams prm{};  // no coefficient output, no fused inputs
   prm.K = p->K;
   prm.n_fixed = L.n_fixed;
   prm.B = nx;
   prm.times = times;
   prm.dfix = dfix;
-  prm.coeffs = nullptr;
-  prm.dfree = nullptr;
-  prm.status = nullptr;
-  prm.positions = nullptr;
-  prm.v_max = prm.a_max = prm.magic = 0.0;
-  prm.times_out = nullptr;
   prm.cost = cost_x;
   prm.mel_k1 = mel_k1;
   prm.mel_inc = inc;
   prm.mel_lower = lower;
-  {
-        const int rc_smem = ensure_dyn_smem(h, (const void*)ce->fn, smem);
-        if (rc_smem != MTG_OK) return rc_smem;
-      }
+  MTG_TRY(ensure_dyn_smem(h, (const void*)e->cost, smem));
   CUtensorMap tmap;
   std::memset(&tmap, 0, sizeof(tmap));  // unused by the cost-only instantiation
-  ce->fn<<<(unsigned)((nx + 63) / 64), mtg::kTmemThreads, smem, stream>>>(prm, tmap);
+  e->cost<<<(unsigned)((nx + 63) / 64), mtg::kTmemThreads, smem, stream>>>(prm, tmap);
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
   return MTG_OK;
@@ -706,14 +813,13 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
   // clear a stale (non-sticky) error another library of the process may have left behind: the
   // cudaGetLastError() after our launches must report OUR launch only
   (void)cudaGetLastError();
-  int kind = backsub_only ? MTG_KERNEL_NOFREE : route(h, p, L);
+  int kind = backsub_only ? MTG_KERNEL_NOFREE : route(p, L);
   // Every specialised kernel stores coefficients in 16-byte units (TMA tensor stores / double2): an output that
   // is only 8-byte aligned (e.g. a tensor slice) takes the banded generic kernel, which stores scalar doubles.
   const bool out_aligned = (reinterpret_cast<uintptr_t>(coeffs) & 15u) == 0;
   if (kind == MTG_KERNEL_WAYPOINT && !fused && !out_aligned) kind = MTG_KERNEL_GENERIC;
   if (kind == MTG_KERNEL_WAYPOINT) {
-    const WaypointEntry* e = find_waypoint(h, p, L);
-    mtg::WaypointParams prm;
+    mtg::WaypointParams prm{};  // not cost-only
     prm.K = p->K;
     prm.n_fixed = L.n_fixed;
     prm.B = B;
@@ -722,194 +828,16 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
     prm.coeffs = coeffs;
     prm.dfree = dfree;
     prm.status = status;
-    prm.positions = fused ? fused->positions : nullptr;
-    prm.v_max = fused ? fused->v_max : 0.0;
-    prm.a_max = fused ? fused->a_max : 0.0;
-    prm.magic = fused ? fused->magic : 0.0;
-    prm.times_out = fused ? fused->times_out : nullptr;
-    prm.cost = nullptr;
-    prm.mel_k1 = 0;
-    prm.mel_inc = prm.mel_lower = 0.0;
-    const size_t smem_v1 = size_t(p->K - 1) * e->slots * 32 * sizeof(double);
-    const bool use_v1 = h->waypoint_variant == 1 && e->fn != nullptr && smem_v1 <= h->smem_optin;
-    // The TMA tensor stores need a 16-byte aligned output (cuTensorMapEncodeTiled); an 8-byte aligned
-    // caller buffer (e.g. a tensor slice) takes the shared-memory twisted kernel instead of failing.
-    const bool coeffs_aligned = (reinterpret_cast<uintptr_t>(coeffs) & 15u) == 0;
-    if (h->waypoint_variant == 5 && coeffs_aligned && !fused)
-      return launch_chunked(h, p, e, prm, coeffs, B, stream, slot);
-    const bool v5_eligible =
-        coeffs_aligned && (B % 16) == 0 &&
-        (fused ? (reinterpret_cast<uintptr_t>(fused->positions) & 15u) == 0
-               : ((reinterpret_cast<uintptr_t>(times) | reinterpret_cast<uintptr_t>(dfix)) & 15u) == 0);
-    if ((h->waypoint_variant == 6 || (h->waypoint_variant == 0 && h->tma_inputs)) && v5_eligible) {
-      const V5Entry* e5 = find_v5(p);
-      if (e5) {
-        const V5Kernel fn5 = fused ? e5->fn_fused : e5->fn;
-        int best_ctas = 0, best_nbuf = 0;
-        size_t best_smem = 0;
-        for (int nbuf = 2; nbuf >= 1; --nbuf) {
-          const size_t smem = (fused ? e5->smem_fused : e5->smem)(p->K, L.n_fixed, nbuf);
-          int ctas = 0;
-          const int rc_ctas = resident_ctas(h, (const void*)fn5, smem, 8, mtg::kTmemThreads, &ctas);
-          if (rc_ctas != MTG_OK) return rc_ctas;
-          // more resident CTAs first; then double buffering
-          if (ctas > best_ctas) {
-            best_ctas = ctas;
-            best_nbuf = nbuf;
-            best_smem = smem;
-          }
-        }
-        // default routing wants two resident CTAs per SM (otherwise the chunked kernel keeps more warps in flight);
-        // a forced v5 runs whenever one CTA fits
-        const bool take = best_ctas >= (h->waypoint_variant == 6 ? 1 : 2) &&
-                          (h->waypoint_variant == 6 || best_nbuf == 2 || h->tma_inputs == 2);
-        if (take) {
-          mtg::TmemLaunchV5 tl;
-          tl.n_buffers = best_nbuf;
-          tl.tile_counter = nullptr;
-          V5Kernel launch_fn = fn5;
-          if (best_nbuf == 1 && h->early_steps >= 0) {
-            // early refill of the single tile buffer (EARLY instantiation): both lanes must own >= E vertices and the
-            // parking area must lie inside the sweep state, behind the state blocks still needed
-            const V5Kernel fe = fused ? e5->fn_fused_early : e5->fn_early;
-            if (fe != nullptr && e5->early_fits(p->K)) {
-              int regs_e = 0;
-              const int rc_regs = kernel_regs(h, (const void*)fe, &regs_e);
-              if (rc_regs != MTG_OK) return rc_regs;
-              if (65536 / (std::max(regs_e, 1) * mtg::kTmemThreads) >= best_ctas) launch_fn = fe;
-            }
-          }
-          const int64_t blocks = std::min<int64_t>((B + 63) / 64, int64_t(best_ctas) * h->sm_count);
-          // dynamic tile counter for long tiles with several tiles per warp (balances the tail); static round-robin for
-          // short trajectories, where the atomic's round trip is not small against a tile
-          const int64_t tiles_per_warp = (B / 16) / std::max<int64_t>(1, blocks * 4);
-          if (h->dynamic_tiles == 1 || (h->dynamic_tiles == 0 && tiles_per_warp >= 8 && p->K > kV4MaxK)) {
-            const int rc_ctr = tile_counter_acquire(h, slot, stream, &tl.tile_counter);
-            if (rc_ctr != MTG_OK) return rc_ctr;
-          }
-          {
-            const int rc_smem = ensure_dyn_smem(h, (const void*)launch_fn, best_smem);
-            if (rc_smem != MTG_OK) return rc_smem;
-          }
-          CUtensorMap tmap;
-          {
-            const int rc = encode_coeff_tmap(h, &tmap, coeffs, B, p);
-            if (rc != MTG_OK) return rc;
-          }
-          launch_fn<<<(unsigned)blocks, mtg::kTmemThreads, best_smem, stream>>>(prm, tl, tmap);
-          MTG_CUDA(h, cudaGetLastError());
-          h->launches++;
-          if (tl.tile_counter != nullptr) return arena_release(h, h->counters[slot], stream);
-          return MTG_OK;
-        }
-      }
+    if (fused) {
+      prm.positions = fused->positions;
+      prm.v_max = fused->v_max;
+      prm.a_max = fused->a_max;
+      prm.magic = fused->magic;
+      prm.times_out = fused->times_out;
     }
-    if ((h->waypoint_variant == 4 || (h->waypoint_variant == 0 && p->K <= kV4MaxK)) && coeffs_aligned) {
-      const V4Entry* e4 = find_v4(p);
-      if (e4) {
-        V4Kernel fn = fused ? e4->fn_fused : e4->fn;
-        const size_t best_smem = e4->smem(p->K);
-        int best_ctas = 0;
-        {
-          const int rc_ctas = resident_ctas(h, (const void*)fn, best_smem, 8, mtg::kTmemThreads, &best_ctas);
-          if (rc_ctas != MTG_OK) return rc_ctas;
-        }
-        if (best_ctas >= (h->waypoint_variant == 4 ? 1 : 2)) {  // as for v5: a forced v4 runs whenever one CTA fits
-          const bool per_tile = h->ctas_per_sm == 9;
-          if (h->ctas_per_sm > 0 && !per_tile) best_ctas = std::min(best_ctas, h->ctas_per_sm);
-          mtg::TmemLaunchV4 tl;
-          tl.tile_counter = nullptr;
-          // dynamic tile counter when every warp has many tiles to draw (balances the tail); static round-robin for
-          // small batches, where the first draw's round trip to L2 is not amortised (measured: C2 static, C4 dynamic)
-          const int64_t tiles_per_warp = ((B + 15) / 16) / std::max<int64_t>(1, int64_t(best_ctas) * h->sm_count * 4);
-          const bool dyn = h->dynamic_tiles == 1 || (h->dynamic_tiles == 0 && tiles_per_warp >= 16);
-          if (dyn && !per_tile) {
-            const int rc_ctr = tile_counter_acquire(h, slot, stream, &tl.tile_counter);
-            if (rc_ctr != MTG_OK) return rc_ctr;
-          }
-          {
-        const int rc_smem = ensure_dyn_smem(h, (const void*)fn, size_t(best_smem));
-        if (rc_smem != MTG_OK) return rc_smem;
-      }
-          CUtensorMap tmap;
-          {
-            const int rc = encode_coeff_tmap(h, &tmap, coeffs, B, p);
-            if (rc != MTG_OK) return rc;
-          }
-          const int64_t ctiles = (B + 63) / 64;
-          const int64_t blocks = per_tile ? ctiles : std::min<int64_t>(ctiles, int64_t(best_ctas) * h->sm_count);
-          fn<<<(unsigned)blocks, mtg::kTmemThreads, best_smem, stream>>>(prm, tl, tmap);
-          MTG_CUDA(h, cudaGetLastError());
-          h->launches++;
-          if (tl.tile_counter != nullptr) return arena_release(h, h->counters[slot], stream);
-          return MTG_OK;
-        }
-      }
-    }
-    const bool twisted_fits = size_t((p->K + 1) / 2 - 1) * e->slots * 32 * sizeof(double) <= h->smem_optin;
-    const bool want_default = h->waypoint_variant == 0 || h->waypoint_variant >= 3 || fused ||
-                              (h->waypoint_variant == 2 && !twisted_fits) || (h->waypoint_variant == 1 && !use_v1 && !twisted_fits);
-    if (want_default && (coeffs_aligned || fused)) {
-      if (!coeffs_aligned) return MTG_ERR_ALLOC;  // fused entry: caller falls back to pack + solve
-      // ---- launch plan (resident CTAs per SM): computed and the function attributes set ONCE per (kernel, K);
-      // a B = 1 solveLinear() call pays none of it again.
-      mtg_handle::TmemPlan* plan = nullptr;
-      for (auto& pl : h->plans)
-        if (pl.entry == (const void*)e && pl.K == p->K) plan = &pl;
-      if (!plan) {
-        mtg_handle::TmemPlan np;
-        np.entry = (const void*)e;
-        np.K = p->K;
-        np.smem = e->tmem_smem(p->K);
-        const int rc_ctas = resident_ctas(h, (const void*)e->fn_tmem, np.smem, 16, mtg::kTmemThreads, &np.ctas);
-        if (rc_ctas != MTG_OK) return rc_ctas;
-        h->plans.push_back(np);
-        plan = &h->plans.back();
-      }
-      if (plan->ctas < 2 && fused) return MTG_ERR_ALLOC;  // caller falls back to pack + solve
-      if (plan->ctas < 2)  // the whole factor does not fit on chip at two CTAs per SM: checkpoint + recompute (K3)
-        return launch_chunked(h, p, e, prm, coeffs, B, stream, slot);
-      const int64_t blocks = (B + 63) / 64;
-      auto fn = fused ? e->fn_tmem_fused : e->fn_tmem;
-      {
-        const int rc_smem = ensure_dyn_smem(h, (const void*)fn, plan->smem);
-        if (rc_smem != MTG_OK) return rc_smem;
-      }
-      // coeffs as a 2-D fp64 tensor [B][K*D*N] for the TMA stores (box = 16 trajectories x one segment);
-      // the encoded map is cached for repeated calls on the same output buffer
-      if (!(h->tmap_key.base == coeffs && h->tmap_key.B == B && h->tmap_key.K == p->K && h->tmap_key.D == p->D &&
-            h->tmap_key.N == p->N)) {
-        const int rc = encode_coeff_tmap(h, &h->tmap_cached, coeffs, B, p);
-        if (rc != MTG_OK) {
-          h->tmap_key.base = nullptr;
-          return rc;
-        }
-        h->tmap_key.base = coeffs;
-        h->tmap_key.B = B;
-        h->tmap_key.K = p->K;
-        h->tmap_key.D = p->D;
-        h->tmap_key.N = p->N;
-      }
-      fn<<<(unsigned)blocks, mtg::kTmemThreads, plan->smem, stream>>>(prm, h->tmap_cached);
-    } else if (use_v1) {
-      {
-        const int rc_smem = ensure_dyn_smem(h, (const void*)e->fn, size_t(smem_v1));
-        if (rc_smem != MTG_OK) return rc_smem;
-      }
-      const int64_t blocks = (B + 31) / 32;
-      e->fn<<<(unsigned)blocks, 32, smem_v1, stream>>>(prm);
-    } else {
-      const size_t smem = size_t((p->K + 1) / 2 - 1) * e->slots * 32 * sizeof(double);
-      {
-        const int rc_smem = ensure_dyn_smem(h, (const void*)e->fn_twisted, size_t(smem));
-        if (rc_smem != MTG_OK) return rc_smem;
-      }
-      const int64_t blocks = (B + 15) / 16;
-      e->fn_twisted<<<(unsigned)blocks, 32, smem, stream>>>(prm);
-    }
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
-    return MTG_OK;
+    WaypointPlan plan;
+    MTG_TRY(plan_waypoint(h, p, L, *find_waypoint(p, L), prm, fused != nullptr, &plan));
+    return launch_waypoint(h, p, plan, prm, stream, slot);
   }
   if (kind == MTG_KERNEL_GENERIC && out_aligned && h->generic_variant == 0)
     return launch_masked(h, p, topo, B, times, dfix, coeffs, dfree, status, stream, slot);
@@ -945,14 +873,12 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
     const size_t per_thread = size_t(L.n_free) * (L.bw + 1 + p->D);
     const size_t bytes = per_thread * size_t(blocks) * threads * sizeof(double);
     mtg_handle::Arena& ar = h->scratch[slot];
-    int rc = arena_acquire(h, ar, bytes, stream);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(arena_acquire(h, ar, bytes, stream));
     prm.scratch = ar.p;
     prm.scratch_stride = blocks * threads;
     mtg::generic_solve_kernel<<<(unsigned)blocks, threads, 0, stream>>>(prm);
     MTG_CUDA(h, cudaGetLastError());
-    rc = arena_release(h, ar, stream);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(arena_release(h, ar, stream));
   }
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
@@ -1080,16 +1006,12 @@ int mtg_set_option(mtg_handle* h, int key, int value) {
     h->early_steps = value;
     return MTG_OK;
   }
-  if (key == MTG_OPT_RING_DEPTH && value >= 2 && value <= 4) {
-    h->ring_depth = value;
+  // reserved keys: accepted in their documented ranges, no effect
+  if ((key == MTG_OPT_RING_DEPTH && value >= 2 && value <= 4) ||
+      (key == MTG_OPT_STAGGER_US && value >= 0 && value <= 1000))
     return MTG_OK;
-  }
   if (key == MTG_OPT_CTAS_PER_SM && value >= 0 && value <= 9) {
     h->ctas_per_sm = value;
-    return MTG_OK;
-  }
-  if (key == MTG_OPT_STAGGER_US && value >= 0 && value <= 1000) {
-    h->stagger_us = value;
     return MTG_OK;
   }
   if (key == MTG_OPT_DYNAMIC_TILES && value >= 0 && value <= 2) {  // 0 = auto, 1 = always, 2 = never
@@ -1107,10 +1029,7 @@ int mtg_problem_layout(const mtg_problem* p, mtg_layout* out, int32_t* slot_col)
   out->n_all = L.n_all;
   out->n_fixed = L.n_fixed;
   out->n_free = L.n_free;
-  // routing without a device: assume the H100 opt-in shared memory limit (227 KB)
-  mtg_handle fake;
-  fake.smem_optin = 227 * 1024;
-  out->kernel = route(&fake, p, L);
+  out->kernel = route(p, L);
   if (slot_col) std::memcpy(slot_col, L.slot_col.data(), sizeof(int32_t) * L.slot_col.size());
   return MTG_OK;
 }
@@ -1144,7 +1063,7 @@ static int nfabian_device(mtg_handle* h, int32_t N, int32_t r, int32_t K, int32_
   CachedTopology* topo = get_topology(h, &p);
   if (!topo) return MTG_ERR_CUDA;
   const Layout& L = topo->layout;
-  if (route(h, &p, L) == MTG_KERNEL_WAYPOINT) {
+  if (route(&p, L) == MTG_KERNEL_WAYPOINT) {
     FusedInput f = {positions, v_max, a_max, magic, seg_times_out};
     const int rc = launch_solve(h, &p, topo, B, nullptr, nullptr, nullptr, coeffs, nullptr, status, s, false, &f, slot);
     if (rc != MTG_ERR_ALLOC) return rc;
@@ -1152,8 +1071,7 @@ static int nfabian_device(mtg_handle* h, int32_t N, int32_t r, int32_t K, int32_
   // no fused specialisation: pack (times, d_fixed) with a small kernel, then the regular path
   const size_t n_t = align_doubles(size_t(B) * K), n_f = size_t(B) * D * L.n_fixed;
   mtg_handle::Arena& ar = h->pack[slot];
-  int rc = arena_acquire(h, ar, (n_t + n_f) * 8, s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(arena_acquire(h, ar, (n_t + n_f) * 8, s));
   double* t_buf = seg_times_out ? seg_times_out : ar.p;
   double* f_buf = ar.p + n_t;
   mtg::PackParams pk;
@@ -1173,8 +1091,7 @@ static int nfabian_device(mtg_handle* h, int32_t N, int32_t r, int32_t K, int32_
   mtg::nfabian_pack_kernel<<<(unsigned)blocks, threads, 0, s>>>(pk);
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
-  rc = launch_solve(h, &p, topo, B, t_buf, f_buf, nullptr, coeffs, nullptr, status, s, false, nullptr, slot);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(launch_solve(h, &p, topo, B, t_buf, f_buf, nullptr, coeffs, nullptr, status, s, false, nullptr, slot));
   return arena_release(h, ar, s);  // the solve was the last reader of the packed inputs
 }
 
@@ -1227,21 +1144,18 @@ int mtg_compute_cost_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, c
     return MTG_ERR_BAD_ARG;
   }
   typedef void (*CostFn)(const mtg::CostParams, const int);
-  struct CostEntry {
+  struct CostKernelEntry {
     int N, r;
     CostFn fn;
   };
-  static const CostEntry kCost[] = {{10, 4, mtg::cost_kernel<10, 4>}, {10, 3, mtg::cost_kernel<10, 3>},
-                                    {10, 2, mtg::cost_kernel<10, 2>}, {8, 3, mtg::cost_kernel<8, 3>},
-                                    {12, 5, mtg::cost_kernel<12, 5>}, {12, 4, mtg::cost_kernel<12, 4>},
-                                    {6, 2, mtg::cost_kernel<6, 2>},   {4, 1, mtg::cost_kernel<4, 1>}};
+  static const CostKernelEntry kComputeCostKernels[] = {
+      {10, 4, mtg::cost_kernel<10, 4>}, {10, 3, mtg::cost_kernel<10, 3>}, {10, 2, mtg::cost_kernel<10, 2>},
+      {8, 3, mtg::cost_kernel<8, 3>},   {12, 5, mtg::cost_kernel<12, 5>}, {12, 4, mtg::cost_kernel<12, 4>},
+      {6, 2, mtg::cost_kernel<6, 2>},   {4, 1, mtg::cost_kernel<4, 1>}};
   CostFn fn = mtg::cost_kernel<0, 0>;
-  for (const auto& e : kCost)
+  for (const auto& e : kComputeCostKernels)
     if (e.N == p->N && e.r == p->r) fn = e.fn;
-  {
-    const int rc_smem = ensure_dyn_smem(h, (const void*)fn, smem);
-    if (rc_smem != MTG_OK) return rc_smem;
-  }
+  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
   int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
   fn<<<(unsigned)blocks, threads, smem, (cudaStream_t)stream>>>(prm, tpb);
   MTG_CUDA(h, cudaGetLastError());
@@ -1284,10 +1198,7 @@ int mtg_evaluate_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64
       mtg::evaluate_kernel<5>, mtg::evaluate_kernel<6>,  mtg::evaluate_kernel<7>,  mtg::evaluate_kernel<8>,
       mtg::evaluate_kernel<9>, mtg::evaluate_kernel<10>, mtg::evaluate_kernel<11>, mtg::evaluate_kernel<12>};
   const EvalFn fn = kEval[N - 1];
-  {
-    const int rc_smem = ensure_dyn_smem(h, (const void*)fn, smem);
-    if (rc_smem != MTG_OK) return rc_smem;
-  }
+  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
   const int64_t total = B * int64_t(n_samples);
   const int64_t blocks = std::min<int64_t>((total + threads - 1) / threads, int64_t(h->sm_count) * 32);
   fn<<<(unsigned)blocks, threads, smem, (cudaStream_t)stream>>>(ep);
@@ -1317,8 +1228,7 @@ int mtg_evaluate_range_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D,
   const size_t ns = size_t(B) * size_t(std::max(max_samples, 1));
   mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
   const size_t o_idx = align_doubles(ns);  // t_local first (doubles), then seg_idx (int32)
-  int rc = arena_acquire(h, ar, (o_idx + align_doubles((ns + 1) / 2)) * 8, s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(arena_acquire(h, ar, (o_idx + align_doubles((ns + 1) / 2)) * 8, s));
   mtg::RangeParams rp;
   rp.N = N;
   rp.K = K;
@@ -1360,10 +1270,7 @@ int mtg_evaluate_range_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D,
         mtg::range_eval_kernel<5>, mtg::range_eval_kernel<6>,  mtg::range_eval_kernel<7>,  mtg::range_eval_kernel<8>,
         mtg::range_eval_kernel<9>, mtg::range_eval_kernel<10>, mtg::range_eval_kernel<11>, mtg::range_eval_kernel<12>};
     const RangeEval fn = kRangeEval[N - 1];
-    {
-      const int rc_smem = ensure_dyn_smem(h, (const void*)fn, smem);
-      if (rc_smem != MTG_OK) return rc_smem;
-    }
+    MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
     const int64_t total = B * int64_t(max_samples);
     const int64_t blocks = std::min<int64_t>((total + threads - 1) / threads, int64_t(h->sm_count) * 32);
     fn<<<(unsigned)blocks, threads, smem, s>>>(rp);
@@ -1391,9 +1298,8 @@ int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
     // fused path: one cost-only launch over the B*(K+1) expanded problems (expansion generated in the kernel, no
     // perturbed inputs or coefficients ever written), then the finite differences
     mtg_handle::Arena& arf = h->pack[mtg_handle::kPipe];
-    int rc = arena_acquire(h, arf, size_t(B) * (K + 1) * 8, s);
-    if (rc != MTG_OK) return rc;
-    rc = launch_cost_fused(h, p, topo, B * int64_t(K + 1), seg_times, d_fixed, arf.p, int(K + 1), 0.1, 0.1, s);
+    MTG_TRY(arena_acquire(h, arf, size_t(B) * (K + 1) * 8, s));
+    const int rc = launch_cost_fused(h, p, topo, B * int64_t(K + 1), seg_times, d_fixed, arf.p, int(K + 1), 0.1, 0.1, s);
     if (rc == MTG_OK) {
       const int threads = 128;
       const int64_t gb = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
@@ -1412,8 +1318,7 @@ int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
                o_j = o_c + align_doubles(nx_max * K * D * N), need = (o_j + align_doubles(nx_max)) * 8;
   mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
   {
-    const int rc = arena_acquire(h, ar, need, s);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(arena_acquire(h, ar, need, s));
   }
   for (int64_t b0 = 0; b0 < B; b0 += chunk) {
     const int64_t nb = std::min<int64_t>(chunk, B - b0), nx = nb * int64_t(K + 1);
@@ -1437,10 +1342,8 @@ int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
     mtg::mellinger_expand_kernel<<<(unsigned)blocks, threads, 0, s>>>(mp);
     MTG_CUDA(h, cudaGetLastError());
     h->launches++;
-    int rc = launch_solve(h, p, topo, nx, t_x, f_x, nullptr, c_x, nullptr, nullptr, s, false);
-    if (rc != MTG_OK) return rc;
-    rc = mtg_compute_cost_batch_f64(h, p, nx, t_x, c_x, j_x, s);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(launch_solve(h, p, topo, nx, t_x, f_x, nullptr, c_x, nullptr, nullptr, s, false));
+    MTG_TRY(mtg_compute_cost_batch_f64(h, p, nx, t_x, c_x, j_x, s));
     const int64_t gb = std::min<int64_t>((nb + threads - 1) / threads, int64_t(h->sm_count) * 16);
     mtg::mellinger_gradient_kernel<<<(unsigned)gb, threads, 0, s>>>(nb, p->K, j_x, cost ? cost + b0 : nullptr,
                                                                   grad + b0 * K, mp.increment);
@@ -1486,10 +1389,7 @@ static int launch_max_magnitude(mtg_handle* h, int32_t N, int32_t K, int32_t D, 
                                                     mtg::max_magnitude_kernel<6>, mtg::max_magnitude_kernel<8>,
                                                     mtg::max_magnitude_kernel<10>, mtg::max_magnitude_kernel<12>};
   const ExtremaFn fn = kExtrema[N / 2 - 1];
-  {
-    const int rc_smem = ensure_dyn_smem(h, (const void*)fn, smem);
-    if (rc_smem != MTG_OK) return rc_smem;
-  }
+  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
   const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
   fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(ep, tpb);
   MTG_CUDA(h, cudaGetLastError());
@@ -1543,20 +1443,17 @@ int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
   const size_t o_max = align_doubles(size_t(B)), o_st = o_max + align_doubles(size_t(B) * nc),
                need = (o_st + align_doubles((size_t(B) + 1) / 2)) * 8;
   mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
-  int rc = arena_acquire(h, ar, need, s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(arena_acquire(h, ar, need, s));
   double* cost = ar.p;
   double* maxima = ar.p + o_max;
   int32_t* solve_status = reinterpret_cast<int32_t*>(ar.p + o_st);
   MTG_CUDA(h, cudaMemsetAsync(solve_status, 0, sizeof(int32_t) * size_t(B), s));
   // the same launches as mtg_solve_linear_batch_f64 / mtg_coeffs_from_constraints_batch_f64
   if (!d_free)
-    rc = launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, solve_status, s, false);
+    MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, solve_status, s, false));
   else
-    rc = launch_solve(h, p, topo, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, s, true);
-  if (rc != MTG_OK) return rc;
-  rc = mtg_compute_cost_batch_f64(h, p, B, seg_times, coeffs, cost, s);
-  if (rc != MTG_OK) return rc;
+    MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, s, true));
+  MTG_TRY(mtg_compute_cost_batch_f64(h, p, B, seg_times, coeffs, cost, s));
   mtg::ObjectiveParams op;
   op.K = p->K;
   op.n_constraints = nc;
@@ -1570,9 +1467,8 @@ int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
       derivs[q] = obj->constraints[q].derivative;
       op.max_value[q] = obj->constraints[q].max_value;
     }
-    rc = launch_max_magnitude(h, p->N, p->K, p->D, B, seg_times, coeffs, nc, derivs, maxima, nullptr, nullptr, nullptr,
-                              s);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(launch_max_magnitude(h, p->N, p->K, p->D, B, seg_times, coeffs, nc, derivs, maxima, nullptr, nullptr, nullptr,
+                                 s));
   }
   op.B = B;
   op.times = seg_times;
@@ -1625,7 +1521,6 @@ static int host_pipeline(mtg_handle* h, const mtg_problem* p, int64_t B, const d
   // chunk so that the pipeline has work for every stream but stays in a few tens of MB
   int64_t chunk = std::max<int64_t>(1, std::min<int64_t>((B + mtg_handle::kPipe - 1) / mtg_handle::kPipe, 32768));
   if (B <= 4096) chunk = B;
-  int rc = MTG_OK;
   int slot = 0;
   PipeSyncGuard sync_on_exit{h};
   for (int64_t b0 = 0; b0 < B; b0 += chunk, slot = (slot + 1) % mtg_handle::kPipe) {
@@ -1637,8 +1532,7 @@ static int host_pipeline(mtg_handle* h, const mtg_problem* p, int64_t B, const d
     const size_t o_free = align_up(o_coef + b_coef * nb);
     const size_t o_stat = align_up(o_free + (d_free_out ? b_free * nb : 0));
     const size_t total = align_up(o_stat + (status ? 4 * nb : 0));
-    rc = ensure_pipe(h, slot, total);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(ensure_pipe(h, slot, total));
     cudaStream_t s = h->streams[slot];
     char* base = static_cast<char*>(h->dev_buf[slot]);
     MTG_CUDA(h, cudaMemcpyAsync(base + o_times, seg_times + b0 * K, b_times * nb, cudaMemcpyHostToDevice, s));
@@ -1646,13 +1540,12 @@ static int host_pipeline(mtg_handle* h, const mtg_problem* p, int64_t B, const d
     if (need_free_in)
       MTG_CUDA(h, cudaMemcpyAsync(base + o_freein, d_free_in + b0 * D * L.n_free, b_free * nb,
                                   cudaMemcpyHostToDevice, s));
-    rc = launch_solve(h, p, topo, nb, reinterpret_cast<double*>(base + o_times),
-                      reinterpret_cast<double*>(base + o_fix),
-                      need_free_in ? reinterpret_cast<double*>(base + o_freein) : nullptr,
-                      reinterpret_cast<double*>(base + o_coef),
-                      d_free_out ? reinterpret_cast<double*>(base + o_free) : nullptr,
-                      status ? reinterpret_cast<int32_t*>(base + o_stat) : nullptr, s, backsub_only, nullptr, slot);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(launch_solve(h, p, topo, nb, reinterpret_cast<double*>(base + o_times),
+                         reinterpret_cast<double*>(base + o_fix),
+                         need_free_in ? reinterpret_cast<double*>(base + o_freein) : nullptr,
+                         reinterpret_cast<double*>(base + o_coef),
+                         d_free_out ? reinterpret_cast<double*>(base + o_free) : nullptr,
+                         status ? reinterpret_cast<int32_t*>(base + o_stat) : nullptr, s, backsub_only, nullptr, slot));
     MTG_CUDA(h, cudaMemcpyAsync(coeffs + b0 * K * D * N, base + o_coef, b_coef * nb, cudaMemcpyDeviceToHost, s));
     if (d_free_out && L.n_free > 0)
       MTG_CUDA(h, cudaMemcpyAsync(d_free_out + b0 * D * L.n_free, base + o_free, b_free * nb,
@@ -1691,15 +1584,13 @@ int mtg_solve_waypoints_nfabian_batch_host_f64(mtg_handle* h, int32_t N, int32_t
   for (int64_t b0 = 0; b0 < B; b0 += chunk, slot = (slot + 1) % mtg_handle::kPipe) {
     const int64_t nb = std::min<int64_t>(chunk, B - b0);
     const size_t o_coef = align_up(b_pos * nb), o_t = align_up(o_coef + b_coef * nb), o_stat = align_up(o_t + b_t * nb);
-    int rc = ensure_pipe(h, slot, align_up(o_stat + 4 * nb));
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(ensure_pipe(h, slot, align_up(o_stat + 4 * nb)));
     cudaStream_t s = h->streams[slot];
     char* base = static_cast<char*>(h->dev_buf[slot]);
     MTG_CUDA(h, cudaMemcpyAsync(base, positions + b0 * (K + 1) * D, b_pos * nb, cudaMemcpyHostToDevice, s));
-    rc = nfabian_device(h, N, r, K, D, nb, reinterpret_cast<double*>(base), v_max, a_max, magic,
-                        reinterpret_cast<double*>(base + o_coef), reinterpret_cast<double*>(base + o_t),
-                        reinterpret_cast<int32_t*>(base + o_stat), s, slot);
-    if (rc != MTG_OK) return rc;
+    MTG_TRY(nfabian_device(h, N, r, K, D, nb, reinterpret_cast<double*>(base), v_max, a_max, magic,
+                           reinterpret_cast<double*>(base + o_coef), reinterpret_cast<double*>(base + o_t),
+                           reinterpret_cast<int32_t*>(base + o_stat), s, slot));
     MTG_CUDA(h, cudaMemcpyAsync(coeffs + b0 * K * D * N, base + o_coef, b_coef * nb, cudaMemcpyDeviceToHost, s));
     if (seg_times_out)
       MTG_CUDA(h, cudaMemcpyAsync(seg_times_out + b0 * K, base + o_t, b_t * nb, cudaMemcpyDeviceToHost, s));
@@ -1729,15 +1620,13 @@ int mtg_compute_cost_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t
   DeviceGuard g(h->device);
   const size_t K = p->K, D = p->D, N = p->N;
   const size_t o_coef = align_up(K * 8 * B), o_cost = align_up(o_coef + K * D * N * 8 * B);
-  int rc = ensure_pipe(h, 0, o_cost + 8 * B);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(ensure_pipe(h, 0, o_cost + 8 * B));
   cudaStream_t s = h->streams[0];
   char* base = static_cast<char*>(h->dev_buf[0]);
   MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, K * 8 * B, cudaMemcpyHostToDevice, s));
   MTG_CUDA(h, cudaMemcpyAsync(base + o_coef, coeffs, K * D * N * 8 * B, cudaMemcpyHostToDevice, s));
-  rc = mtg_compute_cost_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_coef),
-                                  reinterpret_cast<double*>(base + o_cost), s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(mtg_compute_cost_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_coef),
+                                     reinterpret_cast<double*>(base + o_cost), s));
   MTG_CUDA(h, cudaMemcpyAsync(cost, base + o_cost, 8 * B, cudaMemcpyDeviceToHost, s));
   MTG_CUDA(h, cudaStreamSynchronize(s));
   return MTG_OK;
@@ -1756,16 +1645,14 @@ int mtg_cost_gradient_mellinger_batch_host_f64(mtg_handle* h, const mtg_problem*
   if (!topo) return MTG_ERR_CUDA;
   const size_t K = p->K, D = p->D, nf = topo->layout.n_fixed;
   const size_t o_f = align_up(K * 8 * B), o_c = align_up(o_f + D * nf * 8 * B), o_g = align_up(o_c + 8 * B);
-  int rc = ensure_pipe(h, 0, o_g + K * 8 * B);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(ensure_pipe(h, 0, o_g + K * 8 * B));
   cudaStream_t s = h->streams[0];
   char* base = static_cast<char*>(h->dev_buf[0]);
   PipeSyncGuard sync_on_exit{h};
   MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, K * 8 * B, cudaMemcpyHostToDevice, s));
   MTG_CUDA(h, cudaMemcpyAsync(base + o_f, d_fixed, D * nf * 8 * B, cudaMemcpyHostToDevice, s));
-  rc = mtg_cost_gradient_mellinger_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_f),
-                                             reinterpret_cast<double*>(base + o_c), reinterpret_cast<double*>(base + o_g), s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(mtg_cost_gradient_mellinger_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_f),
+                                                reinterpret_cast<double*>(base + o_c), reinterpret_cast<double*>(base + o_g), s));
   if (cost) MTG_CUDA(h, cudaMemcpyAsync(cost, base + o_c, 8 * B, cudaMemcpyDeviceToHost, s));
   MTG_CUDA(h, cudaMemcpyAsync(grad, base + o_g, K * 8 * B, cudaMemcpyDeviceToHost, s));
   MTG_CUDA(h, cudaStreamSynchronize(s));
@@ -1787,18 +1674,16 @@ int mtg_evaluate_range_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32
   const size_t b_t = size_t(K) * 8 * B, b_c = size_t(K) * D * N * 8 * B, b_o = size_t(max_samples) * n_derivs * D * 8 * B,
                b_n = 4 * size_t(B), b_s = size_t(max_samples) * 8 * B;
   const size_t o_c = align_up(b_t), o_o = align_up(o_c + b_c), o_n = align_up(o_o + b_o), o_s = align_up(o_n + b_n);
-  int rc = ensure_pipe(h, 0, o_s + b_s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(ensure_pipe(h, 0, o_s + b_s));
   cudaStream_t s = h->streams[0];
   char* base = static_cast<char*>(h->dev_buf[0]);
   PipeSyncGuard sync_on_exit{h};
   MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, b_t, cudaMemcpyHostToDevice, s));
   MTG_CUDA(h, cudaMemcpyAsync(base + o_c, coeffs, b_c, cudaMemcpyHostToDevice, s));
-  rc = mtg_evaluate_range_batch_f64(h, N, K, D, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_c),
-                                    t_start, t_end, dt, n_derivs, derivs, max_samples, reinterpret_cast<double*>(base + o_o),
-                                    reinterpret_cast<int32_t*>(base + o_n),
-                                    sampling_times ? reinterpret_cast<double*>(base + o_s) : nullptr, s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(mtg_evaluate_range_batch_f64(h, N, K, D, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_c),
+                                       t_start, t_end, dt, n_derivs, derivs, max_samples, reinterpret_cast<double*>(base + o_o),
+                                       reinterpret_cast<int32_t*>(base + o_n),
+                                       sampling_times ? reinterpret_cast<double*>(base + o_s) : nullptr, s));
   if (max_samples > 0) MTG_CUDA(h, cudaMemcpyAsync(out, base + o_o, b_o, cudaMemcpyDeviceToHost, s));
   MTG_CUDA(h, cudaMemcpyAsync(n_samples, base + o_n, b_n, cudaMemcpyDeviceToHost, s));
   if (sampling_times && max_samples > 0)
@@ -1821,19 +1706,17 @@ int mtg_max_magnitude_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_
                b_s = size_t(n_derivs) * 4 * B;
   const size_t o_c = align_up(b_t), o_v = align_up(o_c + b_c), o_t = align_up(o_v + b_v), o_s = align_up(o_t + b_v),
                o_st = align_up(o_s + b_s);
-  int rc = ensure_pipe(h, 0, o_st + 4 * size_t(B));
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(ensure_pipe(h, 0, o_st + 4 * size_t(B)));
   cudaStream_t s = h->streams[0];
   char* base = static_cast<char*>(h->dev_buf[0]);
   PipeSyncGuard sync_on_exit{h};
   MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, b_t, cudaMemcpyHostToDevice, s));
   MTG_CUDA(h, cudaMemcpyAsync(base + o_c, coeffs, b_c, cudaMemcpyHostToDevice, s));
-  rc = mtg_max_magnitude_batch_f64(h, N, K, D, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_c),
-                                   n_derivs, derivs, reinterpret_cast<double*>(base + o_v),
-                                   time ? reinterpret_cast<double*>(base + o_t) : nullptr,
-                                   segment ? reinterpret_cast<int32_t*>(base + o_s) : nullptr,
-                                   status ? reinterpret_cast<int32_t*>(base + o_st) : nullptr, s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(mtg_max_magnitude_batch_f64(h, N, K, D, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_c),
+                                      n_derivs, derivs, reinterpret_cast<double*>(base + o_v),
+                                      time ? reinterpret_cast<double*>(base + o_t) : nullptr,
+                                      segment ? reinterpret_cast<int32_t*>(base + o_s) : nullptr,
+                                      status ? reinterpret_cast<int32_t*>(base + o_st) : nullptr, s));
   MTG_CUDA(h, cudaMemcpyAsync(value, base + o_v, b_v, cudaMemcpyDeviceToHost, s));
   if (time) MTG_CUDA(h, cudaMemcpyAsync(time, base + o_t, b_v, cudaMemcpyDeviceToHost, s));
   if (segment) MTG_CUDA(h, cudaMemcpyAsync(segment, base + o_s, b_s, cudaMemcpyDeviceToHost, s));
@@ -1859,20 +1742,18 @@ int mtg_time_objective_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64
   const size_t b_t = K * 8 * B, b_f = D * nf * 8 * B, b_p = d_free ? D * np * 8 * B : 0, b_c = K * D * N * 8 * B;
   const size_t o_f = align_up(b_t), o_p = align_up(o_f + b_f), o_c = align_up(o_p + b_p), o_o = align_up(o_c + b_c),
                o_m = align_up(o_o + 8 * B), o_s = align_up(o_m + (terms ? 24 * B : 0));
-  int rc = ensure_pipe(h, 0, o_s + 4 * B);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(ensure_pipe(h, 0, o_s + 4 * B));
   cudaStream_t s = h->streams[0];
   char* base = static_cast<char*>(h->dev_buf[0]);
   PipeSyncGuard sync_on_exit{h};
   MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, b_t, cudaMemcpyHostToDevice, s));
   MTG_CUDA(h, cudaMemcpyAsync(base + o_f, d_fixed, b_f, cudaMemcpyHostToDevice, s));
   if (d_free && b_p) MTG_CUDA(h, cudaMemcpyAsync(base + o_p, d_free, b_p, cudaMemcpyHostToDevice, s));
-  rc = mtg_time_objective_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_f),
-                                    d_free ? reinterpret_cast<double*>(base + o_p) : nullptr, obj,
-                                    reinterpret_cast<double*>(base + o_c), reinterpret_cast<double*>(base + o_o),
-                                    terms ? reinterpret_cast<double*>(base + o_m) : nullptr,
-                                    status ? reinterpret_cast<int32_t*>(base + o_s) : nullptr, s);
-  if (rc != MTG_OK) return rc;
+  MTG_TRY(mtg_time_objective_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_f),
+                                       d_free ? reinterpret_cast<double*>(base + o_p) : nullptr, obj,
+                                       reinterpret_cast<double*>(base + o_c), reinterpret_cast<double*>(base + o_o),
+                                       terms ? reinterpret_cast<double*>(base + o_m) : nullptr,
+                                       status ? reinterpret_cast<int32_t*>(base + o_s) : nullptr, s));
   MTG_CUDA(h, cudaMemcpyAsync(coeffs, base + o_c, b_c, cudaMemcpyDeviceToHost, s));
   MTG_CUDA(h, cudaMemcpyAsync(objective, base + o_o, 8 * B, cudaMemcpyDeviceToHost, s));
   if (terms) MTG_CUDA(h, cudaMemcpyAsync(terms, base + o_m, 24 * B, cudaMemcpyDeviceToHost, s));

@@ -20,6 +20,15 @@
 
 namespace mtg {
 
+// Dynamic shared memory of v2 for a 32-thread CTA: the sweep state of each lane's (K+1)/2-1 vertices,
+// [vertex][slot][lane]
+template <int N, int D>
+struct V2Layout {
+  __host__ __device__ static constexpr size_t bytes(int K) {
+    return size_t((K + 1) / 2 - 1) * sweep_state_slots<N, D>() * 32 * sizeof(double);
+  }
+};
+
 template <int N, int R, int D>
 __global__ void __launch_bounds__(32) twisted_solve_kernel(const WaypointParams prm) {
   constexpr int h = N / 2;

@@ -143,6 +143,14 @@ __device__ __forceinline__ void emit_segment(double T, double invT, const double
   }
 }
 
+// Dynamic shared memory of v1 for a 32-thread CTA: the sweep state of the K-1 interior vertices, [vertex][slot][lane]
+template <int N, int D>
+struct V1Layout {
+  __host__ __device__ static constexpr size_t bytes(int K) {
+    return size_t(K - 1) * sweep_state_slots<N, D>() * 32 * sizeof(double);
+  }
+};
+
 template <int N, int R, int D>
 __global__ void __launch_bounds__(32) waypoint_solve_kernel(const WaypointParams prm) {
   constexpr int h = N / 2;
