@@ -226,6 +226,36 @@ int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
                                  const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
                                  double* coeffs, double* objective, double* terms, int32_t* status, void* stream);
 
+/* Trajectory::scaleSegmentTimesToMeetConstraints (src/trajectory.cpp:382-429, Liu et al., RA-L 2017) for B
+ * trajectories: up to 20 times, find max |v| and max |a| (as mtg_max_magnitude_batch_f64 with derivs {1, 2}), stop
+ * when v / v_max <= 1.001 and a / a_max <= 1.001, else stretch every segment time by
+ * s = std::max(1, std::max(v / v_max, sqrt(a / a_max))) and scale coefficient n by (1 / s)^n
+ * (Polynomial::scalePolynomialInTime, src/polynomial.cpp:199-205), with the reference's arithmetic.  The whole loop
+ * runs in one kernel launch.
+ *   seg_times [B][K], coeffs [B][K][D][N] -> seg_times_out, coeffs_out; the outputs may be the input buffers (in-place
+ *   use, as the reference mutates its Trajectory), but must not overlap them otherwise.
+ *   within_range [B] int32: the reference's return value (1 = the last check met both limits; 0 after 20 stretches).
+ *   maxima [B][2] = (max |v|, max |a|) at the last check.  status [B]: MTG_STATUS_BAD_TIME.  All three nullable.
+ * N even in [4, 12]; v_max, a_max > 0 (not NaN), +inf = no limit on that order.  A row with a segment time <= 0 or
+ * non-finite gets status MTG_STATUS_BAD_TIME, within_range 0, maxima NaN, and its times and coefficients unchanged.
+ * A NaN violation (an infinite maximum against an infinite limit) gives s = 1 every round, as std::max does in the
+ * reference: 20 unchanged rounds, within_range 0. */
+int mtg_scale_to_constraints_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                       const double* seg_times, const double* coeffs, double v_max, double a_max,
+                                       double* seg_times_out, double* coeffs_out, int32_t* within_range,
+                                       double* maxima, int32_t* status, void* stream);
+
+/* PolynomialOptimizationNonLinear::scaleSegmentTimesWithViolation (impl/polynomial_optimization_nonlinear_impl.h:
+ * 366-406): solve at seg_times (as mtg_solve_linear_batch_f64), stretch as mtg_scale_to_constraints_batch_f64, then
+ * solve again at the stretched times seg_times_out (may be seg_times) into coeffs [B][K][D][N].  The limits follow
+ * mtg_scale_to_constraints_batch_f64 (+inf where the reference passes 0 for a missing constraint, :373-381).  A row
+ * whose first solve fails keeps its input times and gets within_range 0 and maxima NaN.  status [B] is the OR of the
+ * three steps' status bits.  within_range, maxima, status nullable. */
+int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                             const double* d_fixed, double v_max, double a_max, double* coeffs,
+                                             double* seg_times_out, int32_t* within_range, double* maxima,
+                                             int32_t* status, void* stream);
+
 /* ---- the hot path, HOST pointers (what PolynomialOptimization<N>::solveLinear() calls) ---- */
 /* Same contract with host buffers; H2D, kernels and D2H are pipelined over internal streams and
  * the call returns when the results are in the host buffers.  Pinned buffers (mtg_host_alloc)
@@ -255,6 +285,14 @@ int mtg_max_magnitude_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_
 int mtg_time_objective_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                       const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
                                       double* coeffs, double* objective, double* terms, int32_t* status);
+int mtg_scale_to_constraints_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                            const double* seg_times, const double* coeffs, double v_max, double a_max,
+                                            double* seg_times_out, double* coeffs_out, int32_t* within_range,
+                                            double* maxima, int32_t* status);
+int mtg_scale_times_with_violation_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
+                                                  const double* seg_times, const double* d_fixed, double v_max,
+                                                  double a_max, double* coeffs, double* seg_times_out,
+                                                  int32_t* within_range, double* maxima, int32_t* status);
 
 /* ---- memory helpers (so host code above the ABI needs no CUDA headers) -------------------- */
 void* mtg_host_alloc(mtg_handle* h, uint64_t bytes);   /* pinned */

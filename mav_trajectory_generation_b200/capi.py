@@ -35,7 +35,9 @@ EXPORTED_SYMBOLS = [
     "mtg_cost_gradient_mellinger_batch_host_f64", "mtg_evaluate_range_batch_host_f64",
     "mtg_memcpy_d2d", "mtg_ipc_export", "mtg_ipc_import", "mtg_ipc_close",
     "mtg_max_magnitude_batch_f64", "mtg_time_objective_batch_f64", "mtg_max_magnitude_batch_host_f64",
-    "mtg_time_objective_batch_host_f64",
+    "mtg_time_objective_batch_host_f64", "mtg_scale_to_constraints_batch_f64",
+    "mtg_scale_times_with_violation_batch_f64", "mtg_scale_to_constraints_batch_host_f64",
+    "mtg_scale_times_with_violation_batch_host_f64",
 ]
 TIME_COST_SQUARED, TIME_COST_RICHTER = 0, 1
 
@@ -132,6 +134,15 @@ def load():
                                                dp, dp, dp, dp, vp]
     L.mtg_time_objective_batch_host_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dp,
                                                     C.POINTER(MtgTimeObjective), dp, dp, dp, dp]
+    dbl = C.c_double
+    L.mtg_scale_to_constraints_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, dbl, dbl, dp,
+                                                     dp, dp, dp, dp, vp]
+    L.mtg_scale_to_constraints_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, dbl, dbl,
+                                                          dp, dp, dp, dp, dp]
+    L.mtg_scale_times_with_violation_batch_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dbl, dbl, dp, dp,
+                                                           dp, dp, dp, vp]
+    L.mtg_scale_times_with_violation_batch_host_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dbl, dbl, dp,
+                                                                dp, dp, dp, dp]
     for name in EXPORTED_SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export what the header declares
     _lib = L
@@ -340,6 +351,46 @@ class Solver:
         self._check(rc, "mtg_time_objective_batch_f64")
         return objective, terms, coeffs, status
 
+    def scale_to_constraints(self, seg_times, coeffs, v_max, a_max, seg_times_out=None, coeffs_out=None, stream=None):
+        """Batched Trajectory::scaleSegmentTimesToMeetConstraints: (seg_times_out [B][K], coeffs_out [B][K][D][N],
+        within_range [B] int32, maxima [B][2] = (max |v|, max |a|) at the last check, status [B] int32).  Pass the
+        input tensors as the outputs to stretch in place; v_max / a_max = inf means no limit on that order."""
+        import torch
+        B, K, D, N = coeffs.shape
+        dev = coeffs.device
+        if seg_times_out is None:
+            seg_times_out = torch.empty_like(seg_times)
+        if coeffs_out is None:
+            coeffs_out = torch.empty_like(coeffs)
+        within = torch.empty((B,), dtype=torch.int32, device=dev)
+        maxima = torch.empty((B, 2), dtype=torch.float64, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.mtg_scale_to_constraints_batch_f64(
+            self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(), float(v_max), float(a_max),
+            seg_times_out.data_ptr(), coeffs_out.data_ptr(), within.data_ptr(), maxima.data_ptr(), status.data_ptr(), s)
+        self._check(rc, "mtg_scale_to_constraints_batch_f64")
+        return seg_times_out, coeffs_out, within, maxima, status
+
+    def scale_times_with_violation(self, prob, seg_times, d_fixed, v_max, a_max, seg_times_out=None, stream=None):
+        """Batched PolynomialOptimizationNonLinear::scaleSegmentTimesWithViolation: solve, stretch, re-solve at the
+        stretched times.  -> (coeffs [B][K][D][N], seg_times_out [B][K], within_range [B], maxima [B][2], status [B])."""
+        import torch
+        B = seg_times.shape[0]
+        dev = seg_times.device
+        coeffs = torch.empty((B, prob.K, prob.D, prob.N), dtype=torch.float64, device=dev)
+        if seg_times_out is None:
+            seg_times_out = torch.empty_like(seg_times)
+        within = torch.empty((B,), dtype=torch.int32, device=dev)
+        maxima = torch.empty((B, 2), dtype=torch.float64, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.mtg_scale_times_with_violation_batch_f64(
+            self.h, C.byref(prob.c), B, seg_times.data_ptr(), d_fixed.data_ptr(), float(v_max), float(a_max),
+            coeffs.data_ptr(), seg_times_out.data_ptr(), within.data_ptr(), maxima.data_ptr(), status.data_ptr(), s)
+        self._check(rc, "mtg_scale_times_with_violation_batch_f64")
+        return coeffs, seg_times_out, within, maxima, status
+
     def coeffs_from_constraints(self, prob, seg_times, d_fixed, d_free, coeffs=None, stream=None):
         import torch
         B = seg_times.shape[0]
@@ -425,3 +476,23 @@ class Solver:
             self._hptr(coeffs), self._hptr(objective), self._hptr(terms), self._hptr(status))
         self._check(rc, "mtg_time_objective_batch_host_f64")
         return objective
+
+    def scale_to_constraints_host(self, seg_times, coeffs, v_max, a_max, seg_times_out, coeffs_out, within_range=None,
+                                  maxima=None, status=None):
+        B, K, D, N = coeffs.shape
+        rc = self.lib.mtg_scale_to_constraints_batch_host_f64(
+            self.h, N, K, D, B, self._hptr(seg_times), self._hptr(coeffs), float(v_max), float(a_max),
+            self._hptr(seg_times_out), self._hptr(coeffs_out), self._hptr(within_range), self._hptr(maxima),
+            self._hptr(status))
+        self._check(rc, "mtg_scale_to_constraints_batch_host_f64")
+        return seg_times_out
+
+    def scale_times_with_violation_host(self, prob, seg_times, d_fixed, v_max, a_max, coeffs, seg_times_out,
+                                        within_range=None, maxima=None, status=None):
+        B = seg_times.shape[0]
+        rc = self.lib.mtg_scale_times_with_violation_batch_host_f64(
+            self.h, C.byref(prob.c), B, self._hptr(seg_times), self._hptr(d_fixed), float(v_max), float(a_max),
+            self._hptr(coeffs), self._hptr(seg_times_out), self._hptr(within_range), self._hptr(maxima),
+            self._hptr(status))
+        self._check(rc, "mtg_scale_times_with_violation_batch_host_f64")
+        return coeffs

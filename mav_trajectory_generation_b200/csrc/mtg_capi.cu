@@ -1486,6 +1486,106 @@ int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
   return arena_release(h, ar, s);
 }
 
+// scaleSegmentTimesToMeetConstraints: N even in [4, 12] (N = 2 has no acceleration), limits > 0 (+inf = no limit)
+static bool valid_scale_args(int32_t N, int32_t K, int32_t D, int64_t B, double v_max, double a_max) {
+  return N >= 4 && N <= MTG_MAX_N && !(N & 1) && K >= 1 && D >= 1 && B >= 0 && v_max > 0.0 && a_max > 0.0;
+}
+
+static int launch_scale_to_constraints(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                       const double* seg_times, const double* coeffs, double v_max, double a_max,
+                                       double* seg_times_out, double* coeffs_out, const int32_t* skip,
+                                       int32_t* within_range, double* maxima, int32_t* status, cudaStream_t s) {
+  mtg::ScaleParams sp;
+  sp.K = K;
+  sp.D = D;
+  sp.B = B;
+  sp.v_max = v_max;
+  sp.a_max = a_max;
+  sp.times = seg_times;
+  sp.coeffs = coeffs;
+  sp.times_out = seg_times_out;
+  sp.coeffs_out = coeffs_out;
+  sp.skip = skip;
+  sp.within = within_range;
+  sp.maxima = maxima;
+  sp.status = status;
+  const int tpb = std::max(1, mtg::kExtremaThreads / K);
+  const size_t smem = size_t(2) * tpb * K * sizeof(double) + size_t(tpb) * (sizeof(double) + sizeof(int));
+  if (smem > h->smem_optin) {
+    h->error = "mtg_scale_to_constraints_batch_f64: K too large";
+    return MTG_ERR_BAD_ARG;
+  }
+  typedef void (*ScaleFn)(const mtg::ScaleParams, const int);
+  static const ScaleFn kScale[MTG_MAX_N / 2 - 1] = {
+      mtg::scale_to_constraints_kernel<4>, mtg::scale_to_constraints_kernel<6>, mtg::scale_to_constraints_kernel<8>,
+      mtg::scale_to_constraints_kernel<10>, mtg::scale_to_constraints_kernel<12>};
+  const ScaleFn fn = kScale[N / 2 - 2];
+  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
+  const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
+  fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(sp, tpb);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  return MTG_OK;
+}
+
+int mtg_scale_to_constraints_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                       const double* seg_times, const double* coeffs, double v_max, double a_max,
+                                       double* seg_times_out, double* coeffs_out, int32_t* within_range,
+                                       double* maxima, int32_t* status, void* stream) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid_scale_args(N, K, D, B, v_max, a_max) ||
+      (B > 0 && (!seg_times || !coeffs || !seg_times_out || !coeffs_out))) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (B == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  (void)cudaGetLastError();
+  return launch_scale_to_constraints(h, N, K, D, B, seg_times, coeffs, v_max, a_max, seg_times_out, coeffs_out,
+                                     nullptr, within_range, maxima, status, (cudaStream_t)stream);
+}
+
+int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                             const double* d_fixed, double v_max, double a_max, double* coeffs,
+                                             double* seg_times_out, int32_t* within_range, double* maxima,
+                                             int32_t* status, void* stream) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid_problem(p) || !valid_scale_args(p->N, p->K, p->D, B, v_max, a_max) ||
+      (B > 0 && (!seg_times || !d_fixed || !coeffs || !seg_times_out))) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (B == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  CachedTopology* topo = get_topology(h, p);
+  if (!topo) return MTG_ERR_CUDA;
+  cudaStream_t s = (cudaStream_t)stream;
+  // scratch: status of the first solve [B], of the scaling [B], of the re-solve [B]
+  const size_t o_sc = align_doubles((size_t(B) + 1) / 2), o_re = 2 * o_sc;
+  mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
+  MTG_TRY(arena_acquire(h, ar, 3 * o_sc * 8, s));
+  int32_t* st_solve = reinterpret_cast<int32_t*>(ar.p);
+  int32_t* st_scale = reinterpret_cast<int32_t*>(ar.p + o_sc);
+  int32_t* st_resolve = reinterpret_cast<int32_t*>(ar.p + o_re);
+  MTG_CUDA(h, cudaMemsetAsync(st_solve, 0, sizeof(int32_t) * size_t(B), s));
+  MTG_CUDA(h, cudaMemsetAsync(st_resolve, 0, sizeof(int32_t) * size_t(B), s));
+  // nonlinear_impl.h:366-406: the solve at the given times (trajectory_.scaleSegmentTimesToMeetConstraints acts on
+  // the solved trajectory), the stretch in place on coeffs, then solveLinear() at the stretched times
+  MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, st_solve, s, false));
+  MTG_TRY(launch_scale_to_constraints(h, p->N, p->K, p->D, B, seg_times, coeffs, v_max, a_max, seg_times_out, coeffs,
+                                      st_solve, within_range, maxima, st_scale, s));
+  MTG_TRY(launch_solve(h, p, topo, B, seg_times_out, d_fixed, nullptr, coeffs, nullptr, st_resolve, s, false));
+  if (status) {
+    MTG_CUDA(h, cudaMemcpyAsync(status, st_scale, sizeof(int32_t) * size_t(B), cudaMemcpyDeviceToDevice, s));
+    const int threads = 128;
+    const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
+    mtg::or_status_kernel<<<(unsigned)blocks, threads, 0, s>>>(B, st_resolve, status);
+    MTG_CUDA(h, cudaGetLastError());
+    h->launches++;
+  }
+  return arena_release(h, ar, s);
+}
+
 // ---- host-pointer variants: chunked H2D -> kernel -> D2H over kPipe streams ---------------
 // Every exit of a host-pointer entry point -- error returns included -- waits for all pipeline streams:
 // copies into caller-owned (possibly pinned) buffers must not be in flight when the caller gets control back.
@@ -1757,6 +1857,83 @@ int mtg_time_objective_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64
   MTG_CUDA(h, cudaMemcpyAsync(coeffs, base + o_c, b_c, cudaMemcpyDeviceToHost, s));
   MTG_CUDA(h, cudaMemcpyAsync(objective, base + o_o, 8 * B, cudaMemcpyDeviceToHost, s));
   if (terms) MTG_CUDA(h, cudaMemcpyAsync(terms, base + o_m, 24 * B, cudaMemcpyDeviceToHost, s));
+  if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_s, 4 * B, cudaMemcpyDeviceToHost, s));
+  MTG_CUDA(h, cudaStreamSynchronize(s));
+  return MTG_OK;
+}
+
+int mtg_scale_to_constraints_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                            const double* seg_times, const double* coeffs, double v_max, double a_max,
+                                            double* seg_times_out, double* coeffs_out, int32_t* within_range,
+                                            double* maxima, int32_t* status) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid_scale_args(N, K, D, B, v_max, a_max) ||
+      (B > 0 && (!seg_times || !coeffs || !seg_times_out || !coeffs_out))) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (B == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  // the stretch runs in place on the device copy; every copy in is queued before any copy out, so the host buffers
+  // may alias too
+  const size_t b_t = size_t(K) * 8 * B, b_c = size_t(K) * D * N * 8 * B;
+  const size_t o_c = align_up(b_t), o_w = align_up(o_c + b_c), o_m = align_up(o_w + 4 * size_t(B)),
+               o_s = align_up(o_m + 16 * size_t(B));
+  MTG_TRY(ensure_pipe(h, 0, o_s + 4 * size_t(B)));
+  cudaStream_t s = h->streams[0];
+  char* base = static_cast<char*>(h->dev_buf[0]);
+  PipeSyncGuard sync_on_exit{h};
+  double* d_t = reinterpret_cast<double*>(base);
+  double* d_c = reinterpret_cast<double*>(base + o_c);
+  MTG_CUDA(h, cudaMemcpyAsync(d_t, seg_times, b_t, cudaMemcpyHostToDevice, s));
+  MTG_CUDA(h, cudaMemcpyAsync(d_c, coeffs, b_c, cudaMemcpyHostToDevice, s));
+  MTG_TRY(mtg_scale_to_constraints_batch_f64(h, N, K, D, B, d_t, d_c, v_max, a_max, d_t, d_c,
+                                             within_range ? reinterpret_cast<int32_t*>(base + o_w) : nullptr,
+                                             maxima ? reinterpret_cast<double*>(base + o_m) : nullptr,
+                                             status ? reinterpret_cast<int32_t*>(base + o_s) : nullptr, s));
+  MTG_CUDA(h, cudaMemcpyAsync(seg_times_out, d_t, b_t, cudaMemcpyDeviceToHost, s));
+  MTG_CUDA(h, cudaMemcpyAsync(coeffs_out, d_c, b_c, cudaMemcpyDeviceToHost, s));
+  if (within_range) MTG_CUDA(h, cudaMemcpyAsync(within_range, base + o_w, 4 * size_t(B), cudaMemcpyDeviceToHost, s));
+  if (maxima) MTG_CUDA(h, cudaMemcpyAsync(maxima, base + o_m, 16 * size_t(B), cudaMemcpyDeviceToHost, s));
+  if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_s, 4 * size_t(B), cudaMemcpyDeviceToHost, s));
+  MTG_CUDA(h, cudaStreamSynchronize(s));
+  return MTG_OK;
+}
+
+int mtg_scale_times_with_violation_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
+                                                  const double* seg_times, const double* d_fixed, double v_max,
+                                                  double a_max, double* coeffs, double* seg_times_out,
+                                                  int32_t* within_range, double* maxima, int32_t* status) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid_problem(p) || !valid_scale_args(p->N, p->K, p->D, B, v_max, a_max) ||
+      (B > 0 && (!seg_times || !d_fixed || !coeffs || !seg_times_out))) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (B == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  CachedTopology* topo = get_topology(h, p);
+  if (!topo) return MTG_ERR_CUDA;
+  const size_t K = p->K, D = p->D, N = p->N, nf = topo->layout.n_fixed;
+  const size_t b_t = K * 8 * B, b_f = D * nf * 8 * B, b_c = K * D * N * 8 * B;
+  const size_t o_f = align_up(b_t), o_c = align_up(o_f + b_f), o_w = align_up(o_c + b_c), o_m = align_up(o_w + 4 * B),
+               o_s = align_up(o_m + 16 * B);
+  MTG_TRY(ensure_pipe(h, 0, o_s + 4 * B));
+  cudaStream_t s = h->streams[0];
+  char* base = static_cast<char*>(h->dev_buf[0]);
+  PipeSyncGuard sync_on_exit{h};
+  double* d_t = reinterpret_cast<double*>(base);
+  MTG_CUDA(h, cudaMemcpyAsync(d_t, seg_times, b_t, cudaMemcpyHostToDevice, s));
+  MTG_CUDA(h, cudaMemcpyAsync(base + o_f, d_fixed, b_f, cudaMemcpyHostToDevice, s));
+  MTG_TRY(mtg_scale_times_with_violation_batch_f64(h, p, B, d_t, reinterpret_cast<double*>(base + o_f), v_max, a_max,
+                                                   reinterpret_cast<double*>(base + o_c), d_t,
+                                                   within_range ? reinterpret_cast<int32_t*>(base + o_w) : nullptr,
+                                                   maxima ? reinterpret_cast<double*>(base + o_m) : nullptr,
+                                                   status ? reinterpret_cast<int32_t*>(base + o_s) : nullptr, s));
+  MTG_CUDA(h, cudaMemcpyAsync(coeffs, base + o_c, b_c, cudaMemcpyDeviceToHost, s));
+  MTG_CUDA(h, cudaMemcpyAsync(seg_times_out, d_t, b_t, cudaMemcpyDeviceToHost, s));
+  if (within_range) MTG_CUDA(h, cudaMemcpyAsync(within_range, base + o_w, 4 * B, cudaMemcpyDeviceToHost, s));
+  if (maxima) MTG_CUDA(h, cudaMemcpyAsync(maxima, base + o_m, 16 * B, cudaMemcpyDeviceToHost, s));
   if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_s, 4 * B, cudaMemcpyDeviceToHost, s));
   MTG_CUDA(h, cudaStreamSynchronize(s));
   return MTG_OK;

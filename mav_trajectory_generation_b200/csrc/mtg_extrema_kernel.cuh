@@ -166,12 +166,59 @@ __device__ __forceinline__ double extrema_magnitude(const double* __restrict__ c
   return sqrt(sq);
 }
 
+// The largest |p^(k)| of one segment (coefficients c [D][N], time T > 0 and finite) and where it is: the candidates
+// 0, T and the critical points, in the reference's order (0, T, then the critical points, here increasing).  best_v
+// and best_t start at 0: a candidate replaces them only when strictly larger.
+template <int N>
+__device__ __forceinline__ void extrema_segment_max(const double* __restrict__ c, double T, int D, int k,
+                                                    double& best_v, double& best_t) {
+  constexpr int M = N >= 2 ? 2 * N - 2 : 1;  // coefficients of the critical polynomial (degree 2N - 3)
+  // G(tau) = sum_d A_d(tau) A_d'(tau), A_d(tau) = p_d^(k)(tau T) (D = 1: A'(tau)); nominal degree 2N - 3
+  double g[M];
+#pragma unroll
+  for (int j = 0; j < M; ++j) g[j] = 0.0;
+  for (int d = 0; d < D; ++d) {
+    double a[N];
+#pragma unroll
+    for (int j = 0; j < N; ++j) a[j] = c[d * N + j];
+    for (int s = 0; s < k; ++s) {
+#pragma unroll
+      for (int j = 0; j < N - 1; ++j) a[j] = double(j + 1) * a[j + 1];
+      a[N - 1] = 0.0;
+    }
+    double tp = T;
+#pragma unroll
+    for (int j = 1; j < N; ++j) {
+      a[j] *= tp;
+      tp *= T;
+    }
+    if (D == 1) {
+#pragma unroll
+      for (int j = 0; j < N - 1; ++j) g[j] = double(j + 1) * a[j + 1];
+    } else {
+#pragma unroll
+      for (int i = 0; i < N; ++i)
+#pragma unroll
+        for (int j = 0; j < N - 1; ++j) g[i + j] = fma(a[i], double(j + 1) * a[j + 1], g[i + j]);
+    }
+  }
+  auto take = [&](double t) {
+    const double v = extrema_magnitude<N>(c, D, k, t);
+    if (best_v < v) {
+      best_v = v;
+      best_t = t;
+    }
+  };
+  take(0.0);
+  take(T);
+  extrema_candidates(g, [&](double tau) { take(tau * T); });
+}
+
 // Work item = (trajectory, segment): its best candidate per requested derivative goes to shared memory; one thread per
 // (trajectory, derivative) then reduces the segments in order (strict <, so the first maximum wins).
 // dynamic shared memory: [tpb * K * n_derivs] values, then as many times
 template <int N>
 __global__ void __launch_bounds__(kExtremaThreads, 1) max_magnitude_kernel(const ExtremaParams prm, const int tpb) {
-  constexpr int M = N >= 2 ? 2 * N - 2 : 1;  // coefficients of the critical polynomial (degree 2N - 3)
   extern __shared__ double extrema_sm[];
   const int K = prm.K, D = prm.D, ND = prm.n_derivs;
   double* pv = extrema_sm;
@@ -190,48 +237,7 @@ __global__ void __launch_bounds__(kExtremaThreads, 1) max_magnitude_kernel(const
         for (int j = 0; j < kExtremaMaxDerivs; ++j)
           if (j == q) k = prm.derivs[j];
         double best_v = 0.0, best_t = 0.0;
-        if (!bad) {
-          // G(tau) = sum_d A_d(tau) A_d'(tau), A_d(tau) = p_d^(k)(tau T) (D = 1: A'(tau)); nominal degree 2N - 3
-          double g[M];
-#pragma unroll
-          for (int j = 0; j < M; ++j) g[j] = 0.0;
-          for (int d = 0; d < D; ++d) {
-            double a[N];
-#pragma unroll
-            for (int j = 0; j < N; ++j) a[j] = c[d * N + j];
-            for (int s = 0; s < k; ++s) {
-#pragma unroll
-              for (int j = 0; j < N - 1; ++j) a[j] = double(j + 1) * a[j + 1];
-              a[N - 1] = 0.0;
-            }
-            double tp = T;
-#pragma unroll
-            for (int j = 1; j < N; ++j) {
-              a[j] *= tp;
-              tp *= T;
-            }
-            if (D == 1) {
-#pragma unroll
-              for (int j = 0; j < N - 1; ++j) g[j] = double(j + 1) * a[j + 1];
-            } else {
-#pragma unroll
-              for (int i = 0; i < N; ++i)
-#pragma unroll
-                for (int j = 0; j < N - 1; ++j) g[i + j] = fma(a[i], double(j + 1) * a[j + 1], g[i + j]);
-            }
-          }
-          // candidates in the reference's order: 0, T, then the critical points (here increasing)
-          auto take = [&](double t) {
-            const double v = extrema_magnitude<N>(c, D, k, t);
-            if (best_v < v) {
-              best_v = v;
-              best_t = t;
-            }
-          };
-          take(0.0);
-          take(T);
-          extrema_candidates(g, [&](double tau) { take(tau * T); });
-        }
+        if (!bad) extrema_segment_max<N>(c, T, D, k, best_v, best_t);
         pv[size_t(it) * ND + q] = bad ? __longlong_as_double(0x7ff8000000000000LL) : best_v;
         pt[size_t(it) * ND + q] = best_t;
       }
@@ -261,6 +267,157 @@ __global__ void __launch_bounds__(kExtremaThreads, 1) max_magnitude_kernel(const
     }
     __syncthreads();
   }
+}
+
+// Trajectory::scaleSegmentTimesToMeetConstraints (reference src/trajectory.cpp:382-429, Liu et al., RA-L 2017) for B
+// trajectories: up to 20 rounds of (max |v|, max |a|) -> stop when both are within 1e-3 of the limits, else stretch
+// every segment by max(1, v / v_max, sqrt(a / a_max)) and rescale its coefficients (Polynomial::scalePolynomialInTime,
+// src/polynomial.cpp:199-205).
+struct ScaleParams {
+  int K, D;
+  long long B;
+  double v_max, a_max;            // > 0; +inf = no limit on that order
+  const double* times;            // [B][K]
+  const double* coeffs;           // [B][K][D][N]
+  double* times_out;              // [B][K], may equal times
+  double* coeffs_out;             // [B][K][D][N], may equal coeffs
+  const int* __restrict__ skip;   // [B] or null: rows with a non-zero entry are passed through, and it is ORed into status
+  int* __restrict__ within;       // [B] or null
+  double* __restrict__ maxima;    // [B][2] or null
+  int* __restrict__ status;       // [B] or null
+};
+
+constexpr int kScaleMaxRounds = 20;  // kMaxCounter, trajectory.cpp:385
+
+// One CTA owns tpb trajectories at a time (tpb = max(1, 128 / K), as max_magnitude_kernel) and runs the whole loop on
+// them: phase A, one thread per (trajectory, segment) of every still-active trajectory, puts the segment's max |p'|
+// and max |p''| into shared memory; phase B, one thread per trajectory, reduces over segments in order and decides;
+// phase C, the threads of phase A with the same item -> thread mapping, stretch the active trajectories into the
+// output buffers.  A trajectory is active in round r only if it was stretched in every earlier round, so round 0 reads
+// the inputs and every later round reads what the same thread wrote in the round before: the buffers may alias.
+// dynamic shared memory: [tpb * K][2] segment maxima, [tpb] stretch factors, [tpb] stretch counts
+template <int N>
+__global__ void __launch_bounds__(kExtremaThreads, 1) scale_to_constraints_kernel(const ScaleParams prm, const int tpb) {
+  extern __shared__ double extrema_sm[];
+  const int K = prm.K, D = prm.D;
+  double* pv = extrema_sm;                                          // [tpb * K][2]
+  double* scale = extrema_sm + size_t(2) * tpb * K;                 // [tpb]; 0 = not stretched this round
+  int* stretched = reinterpret_cast<int*>(scale + tpb);             // [tpb]
+  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  const double limit = 1.0 + 1e-3;  // 1.0 + kTolerance, trajectory.cpp:386
+  for (long long t0 = (long long)blockIdx.x * tpb; t0 < prm.B; t0 += (long long)gridDim.x * tpb) {
+    const int ntraj = int(prm.B - t0 < tpb ? prm.B - t0 : tpb);
+    const int items = ntraj * K;
+    for (int lt = threadIdx.x; lt < ntraj; lt += blockDim.x) {
+      stretched[lt] = 0;
+      scale[lt] = 1.0;  // every row takes part in the first check
+    }
+    __syncthreads();
+    for (int round = 0; round < kScaleMaxRounds; ++round) {
+      const double* __restrict__ src_t = round == 0 ? prm.times : prm.times_out;
+      const double* __restrict__ src_c = round == 0 ? prm.coeffs : prm.coeffs_out;
+      // phase A: computeMaxVelocityAndAcceleration of the active rows, per segment
+      for (int it = threadIdx.x; it < items; it += blockDim.x) {
+        const int lt = it / K;
+        if (scale[lt] == 0.0) continue;
+        const long long item = t0 * K + it;
+        const double T = src_t[item];
+        const double* __restrict__ c = src_c + item * D * N;
+        const bool bad = !(T > 0.0) || !isfinite(T);
+        // one copy of the root isolation for both orders (two inlined copies run measurably slower)
+#pragma unroll 1
+        for (int k = 1; k <= 2; ++k) {
+          double best_v = 0.0, best_t = 0.0;
+          if (!bad) extrema_segment_max<N>(c, T, D, k, best_v, best_t);
+          pv[size_t(it) * 2 + (k - 1)] = bad ? nan : best_v;
+        }
+      }
+      __syncthreads();
+      // phase B: the reference's decision, one thread per active row
+      int any = 0;
+      for (int lt = threadIdx.x; lt < ntraj; lt += blockDim.x) {
+        if (scale[lt] == 0.0) continue;
+        const long long traj = t0 + lt;
+        const int pre = prm.skip ? prm.skip[traj] : 0;
+        double bv = 0.0, ba = 0.0;
+        bool bad = false;
+        for (int i = 0; i < K; ++i) {
+          const double T = src_t[traj * K + i];
+          if (!(T > 0.0) || !isfinite(T)) bad = true;
+          const double v = pv[(size_t(lt) * K + i) * 2 + 0], a = pv[(size_t(lt) * K + i) * 2 + 1];
+          if (bv < v) bv = v;
+          if (ba < a) ba = a;
+        }
+        double s = 0.0;
+        bool within = false;
+        if (bad || pre) {
+          bv = ba = nan;
+        } else {
+          const double vv = __ddiv_rn(bv, prm.v_max), av = __ddiv_rn(ba, prm.a_max);
+          within = vv <= limit && av <= limit;
+          if (!within) {
+            const double sa = __dsqrt_rn(av);
+            const double m = (vv < sa) ? sa : vv;  // std::max(vv, sqrt(av)): a NaN first argument is kept
+            s = (1.0 < m) ? m : 1.0;               // std::max(1.0, m): NaN gives 1
+          }
+        }
+        // the values of this check are the last ones if the row stops here or this is the last round (the reference
+        // stretches after its 20th check and returns that check's within_range).  A bad row stops: it is never
+        // stretched, so its inputs are passed through.
+        if (s == 0.0 || round == kScaleMaxRounds - 1) {
+          if (prm.within) prm.within[traj] = within ? 1 : 0;
+          if (prm.maxima) {
+            prm.maxima[traj * 2 + 0] = bv;
+            prm.maxima[traj * 2 + 1] = ba;
+          }
+          if (prm.status) prm.status[traj] = pre | (bad ? 1 : 0);  // MTG_STATUS_BAD_TIME
+        }
+        scale[lt] = s;
+        if (s != 0.0) {
+          stretched[lt] += 1;
+          any = 1;
+        }
+      }
+      // phase C: stretch the rows that did not meet the limits (scaleSegmentTimes' arithmetic)
+      if (!__syncthreads_or(any)) break;
+      for (int it = threadIdx.x; it < items; it += blockDim.x) {
+        const int lt = it / K;
+        const double s = scale[lt];
+        if (s == 0.0) continue;
+        const double inv = __ddiv_rn(1.0, s);
+        const long long item = t0 * K + it;
+        const double* c = src_c + item * D * N;
+        double* o = prm.coeffs_out + item * D * N;
+        const double T = src_t[item];
+        for (int d = 0; d < D; ++d) {
+          double f = 1.0;
+#pragma unroll
+          for (int n = 0; n < N; ++n) {
+            o[d * N + n] = __dmul_rn(c[d * N + n], f);
+            f = __dmul_rn(f, inv);
+          }
+        }
+        prm.times_out[item] = __dmul_rn(T, s);
+      }
+      __syncthreads();
+    }
+    // rows never stretched: pass the inputs through
+    if (prm.times_out != prm.times || prm.coeffs_out != prm.coeffs) {
+      for (int it = threadIdx.x; it < items; it += blockDim.x) {
+        if (stretched[it / K]) continue;
+        const long long item = t0 * K + it;
+        prm.times_out[item] = prm.times[item];
+        for (int j = 0; j < D * N; ++j) prm.coeffs_out[item * D * N + j] = prm.coeffs[item * D * N + j];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// b[i] |= a[i]
+__global__ void __launch_bounds__(128) or_status_kernel(long long n, const int* __restrict__ a, int* __restrict__ b) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    b[i] |= a[i];
 }
 
 // The time objective from the pieces the other kernels computed (one thread per trajectory):

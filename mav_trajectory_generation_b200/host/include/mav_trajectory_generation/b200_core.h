@@ -114,6 +114,12 @@ class BatchCore {
   // the solved coefficients replace coeffs_ (objective: [B], terms: [B][3] or nullptr)
   bool timeObjective(const TimeObjectiveParameters& params, const double* d_free, std::vector<double>* objective,
                      std::vector<double>* terms);
+  // Trajectory::scaleSegmentTimesToMeetConstraints on every trajectory: times_ and coeffs_ are stretched in place
+  // (within_range: [B] or nullptr)
+  bool scaleSegmentTimesToMeetConstraints(double v_max, double a_max, std::vector<uint8_t>* within_range);
+  // PolynomialOptimizationNonLinear::scaleSegmentTimesWithViolation: solve at times_, stretch times_, re-solve into
+  // coeffs_ with d_fixed_; status_ receives the OR of the three steps' status bits
+  bool scaleSegmentTimesWithViolation(double v_max, double a_max, std::vector<uint8_t>* within_range);
   void getSegments(size_t b, Segment::Vector* segments) const;
 
   int N_;

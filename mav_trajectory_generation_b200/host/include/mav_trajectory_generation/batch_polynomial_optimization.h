@@ -92,6 +92,19 @@ class BatchPolynomialOptimization {
                      std::vector<double>* terms = nullptr) {
     return core_.timeObjective(params, d_free, objective, terms);
   }
+  // Trajectory::scaleSegmentTimesToMeetConstraints (reference src/trajectory.cpp:382-429) of every trajectory:
+  // segmentTimes() and coefficients() are stretched in place until max |v| <= v_max and max |a| <= a_max (each within
+  // 1e-3 relative; at most 20 stretches).  within_range[b] is the reference's return value.  v_max or a_max = +inf:
+  // no limit on that order.
+  bool scaleSegmentTimesToMeetConstraints(double v_max, double a_max, std::vector<uint8_t>* within_range = nullptr) {
+    return core_.scaleSegmentTimesToMeetConstraints(v_max, a_max, within_range);
+  }
+  // PolynomialOptimizationNonLinear::scaleSegmentTimesWithViolation (reference
+  // impl/polynomial_optimization_nonlinear_impl.h:366-406): solve at segmentTimes(), stretch them as above, and solve
+  // again at the stretched times with the batch's own fixed constraints.  status()[b] is the OR of the three steps.
+  bool scaleSegmentTimesWithViolation(double v_max, double a_max, std::vector<uint8_t>* within_range = nullptr) {
+    return core_.scaleSegmentTimesWithViolation(v_max, a_max, within_range);
+  }
 
  private:
   b200::BatchCore core_;

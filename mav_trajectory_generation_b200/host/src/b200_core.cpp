@@ -605,6 +605,42 @@ bool BatchCore::timeObjective(const TimeObjectiveParameters& params, const doubl
   return true;
 }
 
+static void copyWithinRange(const std::vector<int32_t>& within, std::vector<uint8_t>* out) {
+  if (out) out->assign(within.begin(), within.end());
+}
+
+bool BatchCore::scaleSegmentTimesToMeetConstraints(double v_max, double a_max, std::vector<uint8_t>* within_range) {
+  CHECK_GT(B_, 0u) << "setup first";
+  std::vector<int32_t> within(B_, 0);
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_scale_to_constraints_batch_host_f64(h, N_, topo_.K, topo_.D, static_cast<int64_t>(B_), times_,
+                                                         coeffs_, v_max, a_max, times_, coeffs_, within.data(),
+                                                         nullptr, nullptr);
+  if (rc != MTG_OK) {
+    LOG(ERROR) << "mtg_scale_to_constraints_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+    return false;
+  }
+  copyWithinRange(within, within_range);
+  return true;
+}
+
+bool BatchCore::scaleSegmentTimesWithViolation(double v_max, double a_max, std::vector<uint8_t>* within_range) {
+  CHECK_GT(B_, 0u) << "setup first";
+  std::vector<int32_t> within(B_, 0);
+  mtg_problem p = {N_, topo_.r, topo_.K, topo_.D, topo_.mask.data()};
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_scale_times_with_violation_batch_host_f64(h, &p, static_cast<int64_t>(B_), times_, d_fixed_, v_max,
+                                                               a_max, coeffs_, times_, within.data(), nullptr, status_);
+  if (rc != MTG_OK) {
+    LOG(ERROR) << "mtg_scale_times_with_violation_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+    return false;
+  }
+  copyWithinRange(within, within_range);
+  return true;
+}
+
 void BatchCore::getSegments(size_t b, Segment::Vector* segments) const {
   CHECK_LT(b, B_);
   unpackSegments(topo_, coeffs_ + b * size_t(topo_.K) * topo_.D * N_, times_ + b * topo_.K, segments);
