@@ -169,7 +169,9 @@ int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
 /* SURVEY.md 8f-3 ("next" row): batched Trajectory::evaluate on a uniform grid t_s = t_start + s*dt,
  * s < n_samples (reference src/trajectory.cpp:48-79 conventions per sample: a time on a vertex belongs to the
  * segment on its right, t == total time is the end of the last segment, beyond the end yields zeros;
- * Horner form of Polynomial::evaluate, polynomial.h:134-149).  coeffs [B][K][D][N] -> out [B][n_samples][D]. */
+ * Horner form of Polynomial::evaluate, polynomial.h:134-149).  coeffs [B][K][D][N] -> out [B][n_samples][D].
+ * t_s is rounded twice, fl(t_start + fl(s*dt)) (never a fused multiply-add), so a sample lands on a vertex exactly
+ * when the same expression computed by the caller does. */
 int mtg_evaluate_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                            const double* coeffs, int32_t derivative, double t_start, double dt, int32_t n_samples,
                            double* out, void* stream);

@@ -121,6 +121,10 @@ def load():
     L.mtg_evaluate_range_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, C.c_double, C.c_double,
                                                C.c_double, C.c_int32, C.POINTER(C.c_int32), C.c_int32, dp, dp, dp, vp]
     L.mtg_cost_gradient_mellinger_batch_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dp, dp, vp]
+    L.mtg_cost_gradient_mellinger_batch_host_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dp, dp]
+    L.mtg_evaluate_range_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, C.c_double,
+                                                    C.c_double, C.c_double, C.c_int32, C.POINTER(C.c_int32),
+                                                    C.c_int32, dp, dp, dp]
     L.mtg_solve_waypoints_nfabian_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, i64, dp,
                                                              C.c_double, C.c_double, C.c_double, dp, dp, dp]
     L.mtg_solve_waypoints_nfabian_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, i64, dp,
@@ -268,11 +272,13 @@ class Solver:
         self._check(rc, "mtg_solve_waypoints_nfabian_batch_f64")
         return coeffs
 
-    def evaluate(self, seg_times, coeffs, derivative, t_start, dt, n_samples, stream=None):
+    def evaluate(self, seg_times, coeffs, derivative, t_start, dt, n_samples, stream=None, out=None):
         """coeffs [B][K][D][N] -> samples [B][n_samples][D] of the given derivative (Trajectory::evaluate)."""
         import torch
         B, K, D, N = coeffs.shape
-        out = torch.empty((B, n_samples, D), dtype=torch.float64, device=coeffs.device)
+        if out is None:
+            out = torch.empty((B, n_samples, D), dtype=torch.float64, device=coeffs.device)
+        assert out.is_contiguous() and tuple(out.shape) == (B, n_samples, D)
         s = stream if stream is not None else torch.cuda.current_stream(coeffs.device).cuda_stream
         rc = self.lib.mtg_evaluate_batch_f64(self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(),
                                              int(derivative), float(t_start), float(dt), int(n_samples),
@@ -457,6 +463,26 @@ class Solver:
                                                       self._hptr(coeffs), self._hptr(cost))
         self._check(rc, "mtg_compute_cost_batch_host_f64")
         return cost
+
+    def cost_gradient_mellinger_host(self, prob, seg_times, d_fixed, cost, grad):
+        """cost [B] (or None) and grad [B][K] host buffers -- batched getCostAndGradientMellinger."""
+        B = seg_times.shape[0]
+        rc = self.lib.mtg_cost_gradient_mellinger_batch_host_f64(
+            self.h, C.byref(prob.c), B, self._hptr(seg_times), self._hptr(d_fixed), self._hptr(cost), self._hptr(grad))
+        self._check(rc, "mtg_cost_gradient_mellinger_batch_host_f64")
+        return grad
+
+    def evaluate_range_host(self, seg_times, coeffs, t_start, t_end, dt, derivs, out, n_samples, sampling_times=None):
+        """Batched Trajectory::evaluateRange into host buffers: out [B][max_samples][len(derivs)][D], n_samples [B]
+        int32, sampling_times [B][max_samples] or None (max_samples is out.shape[1])."""
+        B, K, D, N = coeffs.shape
+        derivs = [int(x) for x in derivs]
+        arr = (C.c_int32 * len(derivs))(*derivs)
+        rc = self.lib.mtg_evaluate_range_batch_host_f64(
+            self.h, N, K, D, B, self._hptr(seg_times), self._hptr(coeffs), float(t_start), float(t_end), float(dt),
+            len(derivs), arr, int(out.shape[1]), self._hptr(out), self._hptr(n_samples), self._hptr(sampling_times))
+        self._check(rc, "mtg_evaluate_range_batch_host_f64")
+        return n_samples
 
     def max_magnitude_host(self, seg_times, coeffs, derivs, value, time=None, segment=None, status=None):
         B, K, D, N = coeffs.shape

@@ -1723,6 +1723,7 @@ int mtg_compute_cost_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t
   MTG_TRY(ensure_pipe(h, 0, o_cost + 8 * B));
   cudaStream_t s = h->streams[0];
   char* base = static_cast<char*>(h->dev_buf[0]);
+  PipeSyncGuard sync_on_exit{h};  // a refused launch (K * D too large) returns with the input copies enqueued
   MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, K * 8 * B, cudaMemcpyHostToDevice, s));
   MTG_CUDA(h, cudaMemcpyAsync(base + o_coef, coeffs, K * D * N * 8 * B, cudaMemcpyHostToDevice, s));
   MTG_TRY(mtg_compute_cost_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_coef),

@@ -353,7 +353,9 @@ __global__ void __launch_bounds__(256) evaluate_kernel(const EvalParams prm) {
     if (idx < total) {
       const long long b = idx / S;
       const int sidx = int(idx - b * S);
-      const double t = prm.t_start + sidx * prm.dt;
+      // t_start + s * dt rounded twice, as the header and every host-side caller compute it: a contracted fma would
+      // land an ulp away on some grids and take a sample on a vertex from the other segment
+      const double t = __dadd_rn(prm.t_start, __dmul_rn(double(sidx), prm.dt));
       const double* __restrict__ tt = prm.times + b * K;
       double start = 0.0;
       int i = 0;
