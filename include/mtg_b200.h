@@ -259,9 +259,11 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
                                              int32_t* status, void* stream);
 
 /* ---- the hot path, HOST pointers (what PolynomialOptimization<N>::solveLinear() calls) ---- */
-/* Same contract with host buffers; H2D, kernels and D2H are pipelined over internal streams and
- * the call returns when the results are in the host buffers.  Pinned buffers (mtg_host_alloc)
- * make the copies asynchronous; pageable buffers work but serialise. */
+/* Same contract with host buffers: each call refuses what its device entry refuses, before any copy, and
+ * returns when the results are in the host buffers.  Pinned buffers (mtg_host_alloc) make the copies
+ * asynchronous; pageable buffers work but serialise.  The three below are pipelined: up to 4096
+ * trajectories run as one chunk, larger batches in chunks of ceil(B / 3) (at most 32768) whose H2D, kernels
+ * and D2H overlap on three internal streams. */
 int mtg_solve_linear_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                     const double* d_fixed, double* coeffs, double* d_free,
                                     int32_t* status);
@@ -271,10 +273,11 @@ int mtg_solve_waypoints_nfabian_batch_host_f64(mtg_handle* h, int32_t N, int32_t
 int mtg_coeffs_from_constraints_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
                                                const double* seg_times, const double* d_fixed,
                                                const double* d_free, double* coeffs);
+
+/* The other host-pointer entry points run the whole batch as one copy in, launch and copy out on one
+ * internal stream. */
 int mtg_compute_cost_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                     const double* coeffs, double* cost);
-
-/* host-pointer variants of the two widened entry points (single stream: copy in, kernels, copy out) */
 int mtg_cost_gradient_mellinger_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                                const double* d_fixed, double* cost, double* grad);
 int mtg_evaluate_range_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,

@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -809,10 +810,6 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
                  cudaStream_t stream, bool backsub_only, const FusedInput* fused = nullptr,
                  int slot = mtg_handle::kPipe) {
   const Layout& L = topo->layout;
-  if (B == 0) return MTG_OK;
-  // clear a stale (non-sticky) error another library of the process may have left behind: the
-  // cudaGetLastError() after our launches must report OUR launch only
-  (void)cudaGetLastError();
   int kind = backsub_only ? MTG_KERNEL_NOFREE : route(p, L);
   // Every specialised kernel stores coefficients in 16-byte units (TMA tensor stores / double2): an output that
   // is only 8-byte aligned (e.g. a tensor slice) takes the banded generic kernel, which stores scalar doubles.
@@ -864,10 +861,6 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
   const int64_t max_blocks = int64_t(h->sm_count) * 8;
   if (blocks > max_blocks) blocks = max_blocks;
   if (kind == MTG_KERNEL_NOFREE) {
-    if (L.n_free > 0 && dfree_in == nullptr) {
-      h->error = "d_free is required for back-substitution of a problem with free constraints";
-      return MTG_ERR_BAD_ARG;
-    }
     mtg::backsub_kernel<<<(unsigned)blocks, threads, 0, stream>>>(prm);
   } else {
     const size_t per_thread = size_t(L.n_free) * (L.bw + 1 + p->D);
@@ -904,6 +897,120 @@ size_t align_up(size_t x) { return (x + 255) & ~size_t(255); }
 // element counts of sub-buffers carved out of one allocation: keep every sub-buffer 256-byte aligned
 // (the TMA tensor map of the coefficient buffer needs >= 16 bytes)
 size_t align_doubles(size_t n) { return (n + 31) & ~size_t(31); }
+
+// B >= 0, and every array that a batch of B > 0 rows needs is given
+bool valid_rows(int64_t B, std::initializer_list<const void*> required) {
+  if (B < 0) return false;
+  if (B > 0)
+    for (const void* q : required)
+      if (!q) return false;
+  return true;
+}
+
+// The opening of every compute entry point: a null handle, the entry's argument check (`valid`), an empty batch
+// (`rows` == 0); then `body` runs with the handle's device current.
+template <class Body>
+int run_entry(mtg_handle* h, bool valid, int64_t rows, Body&& body) {
+  if (!h) return MTG_ERR_BAD_ARG;
+  if (!valid) {
+    h->error = "bad argument";
+    return MTG_ERR_BAD_ARG;
+  }
+  if (rows == 0) return MTG_OK;
+  DeviceGuard g(h->device);
+  // Clear a stale (non-sticky) error that an earlier failed runtime call left behind: the cudaGetLastError() after
+  // our launches must report OUR launch only.  The CUDA runtime is linked in statically and keeps its own last
+  // error, so such a call is one of this library's (e.g. an mtg_device_alloc that could not be satisfied).
+  (void)cudaGetLastError();
+  return body();
+}
+
+// run_entry for an entry of one constraint problem: `body` gets the problem's cached layout
+template <class Body>
+int run_problem_entry(mtg_handle* h, bool valid, const mtg_problem* p, int64_t B, Body&& body) {
+  return run_entry(h, valid, B, [&]() -> int {
+    CachedTopology* topo = get_topology(h, p);
+    return topo ? body(topo) : MTG_ERR_CUDA;
+  });
+}
+
+// ---- host-pointer entry points: copy in, launch, copy out ---------------------------------------------------
+// One host buffer of a host-pointer entry, rows of `row_bytes`: `in` is copied to the device before the launch, the
+// device copy to `out` after it.  Either may be null, and both may be the same buffer.
+struct HostBuf {
+  const void* in;
+  void* out;
+  size_t row_bytes;
+};
+
+// The device copy of a HostBuf (null when both its host pointers are); converts to the launcher's pointer type.
+struct DevBuf {
+  void* p;
+  template <class T>
+  operator T*() const {
+    return static_cast<T*>(p);
+  }
+};
+
+// Every exit of a host-pointer entry point -- error returns included -- waits for all pipeline streams:
+// copies into caller-owned (possibly pinned) buffers must not be in flight when the caller gets control back.
+struct PipeSyncGuard {
+  mtg_handle* h;
+  ~PipeSyncGuard() {
+    for (int i = 0; i < mtg_handle::kPipe; ++i)
+      if (h->streams[i]) cudaStreamSynchronize(h->streams[i]);
+  }
+};
+
+// OneChunk: the whole batch on streams[0], launched with the caller-stream arenas (slot kPipe).  Pipelined: one chunk
+// up to 4096 rows; beyond, chunks of ceil(B / kPipe) rows (at most 32768, so that the pipeline has work for every
+// stream but stays in a few tens of MB) round-robin over the kPipe streams, each launched with its slot's arenas.
+enum class Staging { OneChunk, Pipelined };
+
+// Runs `launch(dev, rows, stream, slot)` on device copies of `bufs` (dev[i] is the copy of bufs[i]), chunk by chunk.
+// The sub-buffers of a chunk are 256-byte aligned in its slot's dev_buf.  Every copy in of a chunk is queued before
+// any of its copies out, so aliased host buffers stay correct; zero-byte copies are skipped.
+template <size_t NB, class Launch>
+int stage_host(mtg_handle* h, int64_t B, Staging staging, const HostBuf (&bufs)[NB], Launch&& launch) {
+  constexpr int kPipe = mtg_handle::kPipe;
+  const bool pipelined = staging == Staging::Pipelined;
+  const int64_t chunk =
+      pipelined && B > 4096 ? std::max<int64_t>(1, std::min<int64_t>((B + kPipe - 1) / kPipe, 32768)) : B;
+  PipeSyncGuard sync_on_exit{h};
+  int slot = 0;
+  for (int64_t b0 = 0; b0 < B; b0 += chunk, slot = (slot + 1) % kPipe) {
+    const int64_t nb = std::min<int64_t>(chunk, B - b0);
+    size_t off[NB], total = 0;
+    for (size_t i = 0; i < NB; ++i) {
+      off[i] = total;
+      if (bufs[i].in || bufs[i].out) total = align_up(total + bufs[i].row_bytes * nb);
+    }
+    MTG_TRY(ensure_pipe(h, slot, total));
+    const cudaStream_t s = h->streams[slot];
+    char* base = static_cast<char*>(h->dev_buf[slot]);
+    DevBuf dev[NB];
+    for (size_t i = 0; i < NB; ++i) {
+      const HostBuf& b = bufs[i];
+      dev[i].p = b.in || b.out ? base + off[i] : nullptr;
+      if (b.in && b.row_bytes)
+        MTG_CUDA(h, cudaMemcpyAsync(dev[i].p, static_cast<const char*>(b.in) + b0 * b.row_bytes, b.row_bytes * nb,
+                                    cudaMemcpyHostToDevice, s));
+    }
+    MTG_TRY(launch(dev, nb, s, pipelined ? slot : kPipe));
+    for (size_t i = 0; i < NB; ++i) {
+      const HostBuf& b = bufs[i];
+      if (b.out && b.row_bytes)
+        MTG_CUDA(h, cudaMemcpyAsync(static_cast<char*>(b.out) + b0 * b.row_bytes, dev[i].p, b.row_bytes * nb,
+                                    cudaMemcpyDeviceToHost, s));
+    }
+    // the buffer of this slot is reused kPipe chunks later: wait for it then
+    const int next = (slot + 1) % kPipe;
+    if (b0 + chunk < B && h->streams[next]) MTG_CUDA(h, cudaStreamSynchronize(h->streams[next]));
+  }
+  for (int i = 0; i < kPipe; ++i)
+    if (h->streams[i]) MTG_CUDA(h, cudaStreamSynchronize(h->streams[i]));
+  return MTG_OK;
+}
 
 }  // namespace
 
@@ -1034,50 +1141,65 @@ int mtg_problem_layout(const mtg_problem* p, mtg_layout* out, int32_t* slot_col)
   return MTG_OK;
 }
 
+// ---- the compute entry points ------------------------------------------------------------------------------------
+// Each kind has one argument check, shared by its device entry and its host twin, and one launcher, which takes
+// checked arguments and launches on `s` (with the arenas of pipeline slot `slot` where it uses any).  A device entry
+// is run_entry() around its launcher; a host entry is run_entry() around stage_host() around the same launcher.
+
+// the entries of one constraint problem with three arrays that every row needs (solve, setFreeConstraints,
+// computeCost, the Mellinger gradient)
+static bool valid_problem_args(const mtg_problem* p, int64_t B, const double* a, const double* b, const double* c) {
+  return valid_problem(p) && valid_rows(B, {a, b, c});
+}
+
+// setFreeConstraints needs d_free whenever the problem has free constraints
+static int check_d_free(mtg_handle* h, const Layout& L, const double* d_free) {
+  if (L.n_free == 0 || d_free) return MTG_OK;
+  h->error = "d_free is required for back-substitution of a problem with free constraints";
+  return MTG_ERR_BAD_ARG;
+}
+
+// solveLinear (backsub_only = false) and setFreeConstraints (backsub_only = true)
+static int solve_device(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times, const double* d_fixed,
+                        const double* d_free_in, double* coeffs, double* d_free, int32_t* status, void* stream,
+                        bool backsub_only) {
+  return run_problem_entry(h, valid_problem_args(p, B, seg_times, d_fixed, coeffs), p, B, [&](CachedTopology* topo) {
+    if (backsub_only) MTG_TRY(check_d_free(h, topo->layout, d_free_in));
+    return launch_solve(h, p, topo, B, seg_times, d_fixed, d_free_in, coeffs, d_free, status, (cudaStream_t)stream,
+                        backsub_only);
+  });
+}
+
 int mtg_solve_linear_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                const double* d_fixed, double* coeffs, double* d_free, int32_t* status,
                                void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || (B > 0 && (!seg_times || !d_fixed || !coeffs))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
-  return launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, d_free, status, (cudaStream_t)stream,
-                      false);
+  return solve_device(h, p, B, seg_times, d_fixed, nullptr, coeffs, d_free, status, stream, false);
 }
 
-static int nfabian_device(mtg_handle* h, int32_t N, int32_t r, int32_t K, int32_t D, int64_t B,
-                          const double* positions, double v_max, double a_max, double magic, double* coeffs,
-                          double* seg_times_out, int32_t* status, cudaStream_t s, int slot) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  mtg_problem p = {N, r, K, D, nullptr};
-  if (!valid_problem(&p) || B < 0 || !(v_max > 0.0) || !(a_max > 0.0) || (B > 0 && (!positions || !coeffs))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, &p);
-  if (!topo) return MTG_ERR_CUDA;
+static bool valid_nfabian(const mtg_problem* p, int64_t B, const double* positions, double v_max, double a_max,
+                          const double* coeffs) {
+  return valid_problem(p) && v_max > 0.0 && a_max > 0.0 && valid_rows(B, {positions, coeffs});
+}
+
+static int launch_nfabian(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B, const double* positions,
+                          double v_max, double a_max, double magic, double* coeffs, double* seg_times_out,
+                          int32_t* status, cudaStream_t s, int slot) {
   const Layout& L = topo->layout;
-  if (route(&p, L) == MTG_KERNEL_WAYPOINT) {
+  if (route(p, L) == MTG_KERNEL_WAYPOINT) {
     FusedInput f = {positions, v_max, a_max, magic, seg_times_out};
-    const int rc = launch_solve(h, &p, topo, B, nullptr, nullptr, nullptr, coeffs, nullptr, status, s, false, &f, slot);
+    const int rc = launch_solve(h, p, topo, B, nullptr, nullptr, nullptr, coeffs, nullptr, status, s, false, &f, slot);
     if (rc != MTG_ERR_ALLOC) return rc;
   }
   // no fused specialisation: pack (times, d_fixed) with a small kernel, then the regular path
-  const size_t n_t = align_doubles(size_t(B) * K), n_f = size_t(B) * D * L.n_fixed;
+  const size_t n_t = align_doubles(size_t(B) * p->K), n_f = size_t(B) * p->D * L.n_fixed;
   mtg_handle::Arena& ar = h->pack[slot];
   MTG_TRY(arena_acquire(h, ar, (n_t + n_f) * 8, s));
   double* t_buf = seg_times_out ? seg_times_out : ar.p;
   double* f_buf = ar.p + n_t;
   mtg::PackParams pk;
-  pk.N = N;
-  pk.K = K;
-  pk.D = D;
+  pk.N = p->N;
+  pk.K = p->K;
+  pk.D = p->D;
   pk.n_fixed = L.n_fixed;
   pk.B = B;
   pk.positions = positions;
@@ -1091,41 +1213,28 @@ static int nfabian_device(mtg_handle* h, int32_t N, int32_t r, int32_t K, int32_
   mtg::nfabian_pack_kernel<<<(unsigned)blocks, threads, 0, s>>>(pk);
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
-  MTG_TRY(launch_solve(h, &p, topo, B, t_buf, f_buf, nullptr, coeffs, nullptr, status, s, false, nullptr, slot));
+  MTG_TRY(launch_solve(h, p, topo, B, t_buf, f_buf, nullptr, coeffs, nullptr, status, s, false, nullptr, slot));
   return arena_release(h, ar, s);  // the solve was the last reader of the packed inputs
 }
 
 int mtg_solve_waypoints_nfabian_batch_f64(mtg_handle* h, int32_t N, int32_t r, int32_t K, int32_t D, int64_t B,
                                           const double* positions, double v_max, double a_max, double magic,
                                           double* coeffs, double* seg_times_out, int32_t* status, void* stream) {
-  return nfabian_device(h, N, r, K, D, B, positions, v_max, a_max, magic, coeffs, seg_times_out, status,
-                        (cudaStream_t)stream, mtg_handle::kPipe);
+  const mtg_problem p = {N, r, K, D, nullptr};
+  return run_problem_entry(h, valid_nfabian(&p, B, positions, v_max, a_max, coeffs), &p, B, [&](CachedTopology* topo) {
+    return launch_nfabian(h, &p, topo, B, positions, v_max, a_max, magic, coeffs, seg_times_out, status,
+                          (cudaStream_t)stream, mtg_handle::kPipe);
+  });
 }
 
 int mtg_coeffs_from_constraints_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
                                           const double* seg_times, const double* d_fixed,
                                           const double* d_free, double* coeffs, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || (B > 0 && (!seg_times || !d_fixed || !coeffs))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
-  return launch_solve(h, p, topo, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, (cudaStream_t)stream,
-                      true);
+  return solve_device(h, p, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, stream, true);
 }
 
-int mtg_compute_cost_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
-                               const double* coeffs, double* cost, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || (B > 0 && (!seg_times || !coeffs || !cost))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
+static int launch_cost(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times, const double* coeffs,
+                       double* cost, cudaStream_t s) {
   mtg::CostParams prm;
   prm.N = p->N;
   prm.r = p->r;
@@ -1157,76 +1266,76 @@ int mtg_compute_cost_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, c
     if (e.N == p->N && e.r == p->r) fn = e.fn;
   MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
   int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
-  fn<<<(unsigned)blocks, threads, smem, (cudaStream_t)stream>>>(prm, tpb);
+  fn<<<(unsigned)blocks, threads, smem, s>>>(prm, tpb);
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
   return MTG_OK;
+}
+
+int mtg_compute_cost_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                               const double* coeffs, double* cost, void* stream) {
+  return run_entry(h, valid_problem_args(p, B, seg_times, coeffs, cost), B,
+                   [&] { return launch_cost(h, p, B, seg_times, coeffs, cost, (cudaStream_t)stream); });
 }
 
 int mtg_evaluate_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                            const double* coeffs, int32_t derivative, double t_start, double dt, int32_t n_samples,
                            double* out, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (N < 1 || N > MTG_MAX_N || K < 1 || D < 1 || B < 0 || derivative < 0 || n_samples < 0 ||
-      (B > 0 && n_samples > 0 && (!seg_times || !coeffs || !out))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0 || n_samples == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  mtg::EvalParams ep;
-  ep.N = N;
-  ep.K = K;
-  ep.D = D;
-  ep.derivative = derivative;
-  ep.n_samples = n_samples;
-  ep.B = B;
-  ep.t_start = t_start;
-  ep.dt = dt;
-  ep.times = seg_times;
-  ep.coeffs = coeffs;
-  ep.out = out;
-  if (size_t(32) * D * 8 > size_t(160) * 1024) {
-    h->error = "mtg_evaluate_batch_f64: D too large for the output tile";
-    return MTG_ERR_BAD_ARG;
-  }
-  const int threads = std::max(32, std::min(256, int((40 * 1024) / (D * 8)) / 32 * 32));
-  const size_t smem = size_t(threads) * D * sizeof(double);
-  typedef void (*EvalFn)(const mtg::EvalParams);
-  static const EvalFn kEval[MTG_MAX_N] = {
-      mtg::evaluate_kernel<1>, mtg::evaluate_kernel<2>,  mtg::evaluate_kernel<3>,  mtg::evaluate_kernel<4>,
-      mtg::evaluate_kernel<5>, mtg::evaluate_kernel<6>,  mtg::evaluate_kernel<7>,  mtg::evaluate_kernel<8>,
-      mtg::evaluate_kernel<9>, mtg::evaluate_kernel<10>, mtg::evaluate_kernel<11>, mtg::evaluate_kernel<12>};
-  const EvalFn fn = kEval[N - 1];
-  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
-  const int64_t total = B * int64_t(n_samples);
-  const int64_t blocks = std::min<int64_t>((total + threads - 1) / threads, int64_t(h->sm_count) * 32);
-  fn<<<(unsigned)blocks, threads, smem, (cudaStream_t)stream>>>(ep);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
-}
-
-int mtg_evaluate_range_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
-                                 const double* coeffs, double t_start, double t_end, double dt, int32_t n_derivs,
-                                 const int32_t* derivs, int32_t max_samples, double* out, int32_t* n_samples,
-                                 double* sampling_times, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (N < 1 || N > MTG_MAX_N || K < 1 || D < 1 || B < 0 || n_derivs < 1 || n_derivs > 8 || !derivs || max_samples < 0 ||
-      !(dt > 0.0) || (B > 0 && (!seg_times || !coeffs || !n_samples || (max_samples > 0 && !out)))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  for (int q = 0; q < n_derivs; ++q)
-    if (derivs[q] < 0) {
-      h->error = "bad argument";
+  const bool valid = N >= 1 && N <= MTG_MAX_N && K >= 1 && D >= 1 && B >= 0 && derivative >= 0 && n_samples >= 0 &&
+                     (n_samples == 0 || valid_rows(B, {seg_times, coeffs, out}));
+  return run_entry(h, valid, n_samples > 0 ? B : 0, [&]() -> int {
+    mtg::EvalParams ep;
+    ep.N = N;
+    ep.K = K;
+    ep.D = D;
+    ep.derivative = derivative;
+    ep.n_samples = n_samples;
+    ep.B = B;
+    ep.t_start = t_start;
+    ep.dt = dt;
+    ep.times = seg_times;
+    ep.coeffs = coeffs;
+    ep.out = out;
+    if (size_t(32) * D * 8 > size_t(160) * 1024) {
+      h->error = "mtg_evaluate_batch_f64: D too large for the output tile";
       return MTG_ERR_BAD_ARG;
     }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  cudaStream_t s = (cudaStream_t)stream;
+    const int threads = std::max(32, std::min(256, int((40 * 1024) / (D * 8)) / 32 * 32));
+    const size_t smem = size_t(threads) * D * sizeof(double);
+    typedef void (*EvalFn)(const mtg::EvalParams);
+    static const EvalFn kEval[MTG_MAX_N] = {
+        mtg::evaluate_kernel<1>, mtg::evaluate_kernel<2>,  mtg::evaluate_kernel<3>,  mtg::evaluate_kernel<4>,
+        mtg::evaluate_kernel<5>, mtg::evaluate_kernel<6>,  mtg::evaluate_kernel<7>,  mtg::evaluate_kernel<8>,
+        mtg::evaluate_kernel<9>, mtg::evaluate_kernel<10>, mtg::evaluate_kernel<11>, mtg::evaluate_kernel<12>};
+    const EvalFn fn = kEval[N - 1];
+    MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
+    const int64_t total = B * int64_t(n_samples);
+    const int64_t blocks = std::min<int64_t>((total + threads - 1) / threads, int64_t(h->sm_count) * 32);
+    fn<<<(unsigned)blocks, threads, smem, (cudaStream_t)stream>>>(ep);
+    MTG_CUDA(h, cudaGetLastError());
+    h->launches++;
+    return MTG_OK;
+  });
+}
+
+// evaluateRange: 1..8 derivative orders, each >= 0, dt > 0; out may be null while max_samples is 0
+static bool valid_range(int32_t N, int32_t K, int32_t D, int64_t B, double dt, int32_t n_derivs, const int32_t* derivs,
+                        int32_t max_samples, const double* seg_times, const double* coeffs, const double* out,
+                        const int32_t* n_samples) {
+  if (N < 1 || N > MTG_MAX_N || K < 1 || D < 1 || n_derivs < 1 || n_derivs > 8 || !derivs || max_samples < 0 ||
+      !(dt > 0.0))
+    return false;
+  for (int q = 0; q < n_derivs; ++q)
+    if (derivs[q] < 0) return false;
+  return valid_rows(B, {seg_times, coeffs, n_samples}) && (B == 0 || max_samples == 0 || out);
+}
+
+static int launch_range(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                        const double* coeffs, double t_start, double t_end, double dt, int32_t n_derivs,
+                        const int32_t* derivs, int32_t max_samples, double* out, int32_t* n_samples,
+                        double* sampling_times, cudaStream_t s, int slot) {
   const size_t ns = size_t(B) * size_t(std::max(max_samples, 1));
-  mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
+  mtg_handle::Arena& ar = h->pack[slot];
   const size_t o_idx = align_doubles(ns);  // t_local first (doubles), then seg_idx (int32)
   MTG_TRY(arena_acquire(h, ar, (o_idx + align_doubles((ns + 1) / 2)) * 8, s));
   mtg::RangeParams rp;
@@ -1280,33 +1389,36 @@ int mtg_evaluate_range_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D,
   return arena_release(h, ar, s);
 }
 
-int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
-                                          const double* d_fixed, double* cost, double* grad, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || (B > 0 && (!seg_times || !d_fixed || !grad))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
+int mtg_evaluate_range_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                 const double* coeffs, double t_start, double t_end, double dt, int32_t n_derivs,
+                                 const int32_t* derivs, int32_t max_samples, double* out, int32_t* n_samples,
+                                 double* sampling_times, void* stream) {
+  return run_entry(h, valid_range(N, K, D, B, dt, n_derivs, derivs, max_samples, seg_times, coeffs, out, n_samples), B,
+                   [&] {
+                     return launch_range(h, N, K, D, B, seg_times, coeffs, t_start, t_end, dt, n_derivs, derivs,
+                                         max_samples, out, n_samples, sampling_times, (cudaStream_t)stream,
+                                         mtg_handle::kPipe);
+                   });
+}
+
+static int launch_mellinger(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B,
+                            const double* seg_times, const double* d_fixed, double* cost, double* grad, cudaStream_t s,
+                            int slot) {
   const Layout& L = topo->layout;
-  cudaStream_t s = (cudaStream_t)stream;
   const size_t K = p->K, D = p->D, N = p->N, nf = L.n_fixed;
+  mtg_handle::Arena& ar = h->pack[slot];
   if (p->K > 1 && h->mellinger_unfused == 0) {
     // fused path: one cost-only launch over the B*(K+1) expanded problems (expansion generated in the kernel, no
     // perturbed inputs or coefficients ever written), then the finite differences
-    mtg_handle::Arena& arf = h->pack[mtg_handle::kPipe];
-    MTG_TRY(arena_acquire(h, arf, size_t(B) * (K + 1) * 8, s));
-    const int rc = launch_cost_fused(h, p, topo, B * int64_t(K + 1), seg_times, d_fixed, arf.p, int(K + 1), 0.1, 0.1, s);
+    MTG_TRY(arena_acquire(h, ar, size_t(B) * (K + 1) * 8, s));
+    const int rc = launch_cost_fused(h, p, topo, B * int64_t(K + 1), seg_times, d_fixed, ar.p, int(K + 1), 0.1, 0.1, s);
     if (rc == MTG_OK) {
       const int threads = 128;
       const int64_t gb = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
-      mtg::mellinger_gradient_kernel<<<(unsigned)gb, threads, 0, s>>>(B, p->K, arf.p, cost, grad, 0.1);
+      mtg::mellinger_gradient_kernel<<<(unsigned)gb, threads, 0, s>>>(B, p->K, ar.p, cost, grad, 0.1);
       MTG_CUDA(h, cudaGetLastError());
       h->launches++;
-      return arena_release(h, arf, s);
+      return arena_release(h, ar, s);
     }
     if (rc != MTG_ERR_ALLOC) return rc;
   }
@@ -1316,10 +1428,7 @@ int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
   const size_t nx_max = size_t(chunk) * (K + 1);
   const size_t o_f = align_doubles(nx_max * K), o_c = o_f + align_doubles(nx_max * D * nf),
                o_j = o_c + align_doubles(nx_max * K * D * N), need = (o_j + align_doubles(nx_max)) * 8;
-  mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
-  {
-    MTG_TRY(arena_acquire(h, ar, need, s));
-  }
+  MTG_TRY(arena_acquire(h, ar, need, s));
   for (int64_t b0 = 0; b0 < B; b0 += chunk) {
     const int64_t nb = std::min<int64_t>(chunk, B - b0), nx = nb * int64_t(K + 1);
     double* t_x = ar.p;
@@ -1342,8 +1451,8 @@ int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
     mtg::mellinger_expand_kernel<<<(unsigned)blocks, threads, 0, s>>>(mp);
     MTG_CUDA(h, cudaGetLastError());
     h->launches++;
-    MTG_TRY(launch_solve(h, p, topo, nx, t_x, f_x, nullptr, c_x, nullptr, nullptr, s, false));
-    MTG_TRY(mtg_compute_cost_batch_f64(h, p, nx, t_x, c_x, j_x, s));
+    MTG_TRY(launch_solve(h, p, topo, nx, t_x, f_x, nullptr, c_x, nullptr, nullptr, s, false, nullptr, slot));
+    MTG_TRY(launch_cost(h, p, nx, t_x, c_x, j_x, s));
     const int64_t gb = std::min<int64_t>((nb + threads - 1) / threads, int64_t(h->sm_count) * 16);
     mtg::mellinger_gradient_kernel<<<(unsigned)gb, threads, 0, s>>>(nb, p->K, j_x, cost ? cost + b0 : nullptr,
                                                                   grad + b0 * K, mp.increment);
@@ -1353,14 +1462,22 @@ int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
   return arena_release(h, ar, s);
 }
 
+int mtg_cost_gradient_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                          const double* d_fixed, double* cost, double* grad, void* stream) {
+  return run_problem_entry(h, valid_problem_args(p, B, seg_times, d_fixed, grad), p, B, [&](CachedTopology* topo) {
+    return launch_mellinger(h, p, topo, B, seg_times, d_fixed, cost, grad, (cudaStream_t)stream, mtg_handle::kPipe);
+  });
+}
+
 // computeMaximumOfMagnitude: N even in [2, 12], 1..8 derivative orders, each in [0, N-2] (linear_impl.h:401 CHECKs
 // N - k - 1 > 0)
-static bool valid_extrema_args(int32_t N, int32_t K, int32_t D, int64_t B, int32_t n_derivs, const int32_t* derivs) {
-  if (N < 2 || N > MTG_MAX_N || (N & 1) || K < 1 || D < 1 || B < 0) return false;
+static bool valid_extrema_args(int32_t N, int32_t K, int32_t D, int64_t B, int32_t n_derivs, const int32_t* derivs,
+                               const double* seg_times, const double* coeffs, const double* value) {
+  if (N < 2 || N > MTG_MAX_N || (N & 1) || K < 1 || D < 1) return false;
   if (n_derivs < 1 || n_derivs > mtg::kExtremaMaxDerivs || !derivs) return false;
   for (int q = 0; q < n_derivs; ++q)
     if (derivs[q] < 0 || derivs[q] > N - 2) return false;
-  return true;
+  return valid_rows(B, {seg_times, coeffs, value});
 }
 
 static int launch_max_magnitude(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
@@ -1400,20 +1517,15 @@ static int launch_max_magnitude(mtg_handle* h, int32_t N, int32_t K, int32_t D, 
 int mtg_max_magnitude_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                                 const double* coeffs, int32_t n_derivs, const int32_t* derivs, double* value,
                                 double* time, int32_t* segment, int32_t* status, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_extrema_args(N, K, D, B, n_derivs, derivs) || (B > 0 && (!seg_times || !coeffs || !value))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  (void)cudaGetLastError();
-  return launch_max_magnitude(h, N, K, D, B, seg_times, coeffs, n_derivs, derivs, value, time, segment, status,
-                              (cudaStream_t)stream);
+  return run_entry(h, valid_extrema_args(N, K, D, B, n_derivs, derivs, seg_times, coeffs, value), B, [&] {
+    return launch_max_magnitude(h, N, K, D, B, seg_times, coeffs, n_derivs, derivs, value, time, segment, status,
+                                (cudaStream_t)stream);
+  });
 }
 
-static bool valid_objective(const mtg_problem* p, const mtg_time_objective* obj) {
-  if (!obj || (obj->time_cost != 0 && obj->time_cost != 1)) return false;
+static bool valid_objective(const mtg_problem* p, int64_t B, const mtg_time_objective* obj, const double* seg_times,
+                            const double* d_fixed, const double* coeffs, const double* objective) {
+  if (!valid_problem(p) || !obj || (obj->time_cost != 0 && obj->time_cost != 1)) return false;
   if (obj->n_constraints < 0 || obj->n_constraints > mtg::kExtremaMaxDerivs) return false;
   if (obj->n_constraints > 0 && !obj->constraints) return false;
   for (int q = 0; q < obj->n_constraints; ++q) {
@@ -1421,28 +1533,18 @@ static bool valid_objective(const mtg_problem* p, const mtg_time_objective* obj)
     // max_value == 0 would divide by zero in the reference (nonlinear_impl.h:785)
     if (c.derivative < 0 || c.derivative > p->N - 2 || !(c.max_value > 0.0) || !std::isfinite(c.max_value)) return false;
   }
-  return true;
+  return valid_rows(B, {seg_times, d_fixed, coeffs, objective});
 }
 
-int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
-                                 const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
-                                 double* coeffs, double* objective, double* terms, int32_t* status, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || !valid_objective(p, obj) ||
-      (B > 0 && (!seg_times || !d_fixed || !coeffs || !objective))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
-  cudaStream_t s = (cudaStream_t)stream;
+static int launch_time_objective(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B,
+                                 const double* seg_times, const double* d_fixed, const double* d_free,
+                                 const mtg_time_objective* obj, double* coeffs, double* objective, double* terms,
+                                 int32_t* status, cudaStream_t s, int slot) {
   const int nc = obj->n_constraints;
   // scratch: computeCost [B], maxima [B][nc], solve status [B]
   const size_t o_max = align_doubles(size_t(B)), o_st = o_max + align_doubles(size_t(B) * nc),
                need = (o_st + align_doubles((size_t(B) + 1) / 2)) * 8;
-  mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
+  mtg_handle::Arena& ar = h->pack[slot];
   MTG_TRY(arena_acquire(h, ar, need, s));
   double* cost = ar.p;
   double* maxima = ar.p + o_max;
@@ -1450,10 +1552,11 @@ int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
   MTG_CUDA(h, cudaMemsetAsync(solve_status, 0, sizeof(int32_t) * size_t(B), s));
   // the same launches as mtg_solve_linear_batch_f64 / mtg_coeffs_from_constraints_batch_f64
   if (!d_free)
-    MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, solve_status, s, false));
+    MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, solve_status, s, false, nullptr,
+                         slot));
   else
-    MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, s, true));
-  MTG_TRY(mtg_compute_cost_batch_f64(h, p, B, seg_times, coeffs, cost, s));
+    MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, s, true, nullptr, slot));
+  MTG_TRY(launch_cost(h, p, B, seg_times, coeffs, cost, s));
   mtg::ObjectiveParams op;
   op.K = p->K;
   op.n_constraints = nc;
@@ -1486,9 +1589,25 @@ int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
   return arena_release(h, ar, s);
 }
 
+int mtg_time_objective_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                 const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
+                                 double* coeffs, double* objective, double* terms, int32_t* status, void* stream) {
+  return run_problem_entry(h, valid_objective(p, B, obj, seg_times, d_fixed, coeffs, objective), p, B,
+                           [&](CachedTopology* topo) {
+                             return launch_time_objective(h, p, topo, B, seg_times, d_fixed, d_free, obj, coeffs,
+                                                          objective, terms, status, (cudaStream_t)stream,
+                                                          mtg_handle::kPipe);
+                           });
+}
+
 // scaleSegmentTimesToMeetConstraints: N even in [4, 12] (N = 2 has no acceleration), limits > 0 (+inf = no limit)
 static bool valid_scale_args(int32_t N, int32_t K, int32_t D, int64_t B, double v_max, double a_max) {
   return N >= 4 && N <= MTG_MAX_N && !(N & 1) && K >= 1 && D >= 1 && B >= 0 && v_max > 0.0 && a_max > 0.0;
+}
+
+static bool valid_scale(int32_t N, int32_t K, int32_t D, int64_t B, double v_max, double a_max, const double* seg_times,
+                        const double* coeffs, const double* seg_times_out, const double* coeffs_out) {
+  return valid_scale_args(N, K, D, B, v_max, a_max) && valid_rows(B, {seg_times, coeffs, seg_times_out, coeffs_out});
 }
 
 static int launch_scale_to_constraints(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
@@ -1532,37 +1651,25 @@ int mtg_scale_to_constraints_batch_f64(mtg_handle* h, int32_t N, int32_t K, int3
                                        const double* seg_times, const double* coeffs, double v_max, double a_max,
                                        double* seg_times_out, double* coeffs_out, int32_t* within_range,
                                        double* maxima, int32_t* status, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_scale_args(N, K, D, B, v_max, a_max) ||
-      (B > 0 && (!seg_times || !coeffs || !seg_times_out || !coeffs_out))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  (void)cudaGetLastError();
-  return launch_scale_to_constraints(h, N, K, D, B, seg_times, coeffs, v_max, a_max, seg_times_out, coeffs_out,
-                                     nullptr, within_range, maxima, status, (cudaStream_t)stream);
+  return run_entry(h, valid_scale(N, K, D, B, v_max, a_max, seg_times, coeffs, seg_times_out, coeffs_out), B, [&] {
+    return launch_scale_to_constraints(h, N, K, D, B, seg_times, coeffs, v_max, a_max, seg_times_out, coeffs_out,
+                                       nullptr, within_range, maxima, status, (cudaStream_t)stream);
+  });
 }
 
-int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
-                                             const double* d_fixed, double v_max, double a_max, double* coeffs,
-                                             double* seg_times_out, int32_t* within_range, double* maxima,
-                                             int32_t* status, void* stream) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || !valid_scale_args(p->N, p->K, p->D, B, v_max, a_max) ||
-      (B > 0 && (!seg_times || !d_fixed || !coeffs || !seg_times_out))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
-  cudaStream_t s = (cudaStream_t)stream;
+static bool valid_violation(const mtg_problem* p, int64_t B, double v_max, double a_max, const double* seg_times,
+                            const double* d_fixed, const double* coeffs, const double* seg_times_out) {
+  return valid_problem(p) && valid_scale_args(p->N, p->K, p->D, B, v_max, a_max) &&
+         valid_rows(B, {seg_times, d_fixed, coeffs, seg_times_out});
+}
+
+static int launch_scale_with_violation(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B,
+                                       const double* seg_times, const double* d_fixed, double v_max, double a_max,
+                                       double* coeffs, double* seg_times_out, int32_t* within_range, double* maxima,
+                                       int32_t* status, cudaStream_t s, int slot) {
   // scratch: status of the first solve [B], of the scaling [B], of the re-solve [B]
   const size_t o_sc = align_doubles((size_t(B) + 1) / 2), o_re = 2 * o_sc;
-  mtg_handle::Arena& ar = h->pack[mtg_handle::kPipe];
+  mtg_handle::Arena& ar = h->pack[slot];
   MTG_TRY(arena_acquire(h, ar, 3 * o_sc * 8, s));
   int32_t* st_solve = reinterpret_cast<int32_t*>(ar.p);
   int32_t* st_scale = reinterpret_cast<int32_t*>(ar.p + o_sc);
@@ -1571,10 +1678,11 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
   MTG_CUDA(h, cudaMemsetAsync(st_resolve, 0, sizeof(int32_t) * size_t(B), s));
   // nonlinear_impl.h:366-406: the solve at the given times (trajectory_.scaleSegmentTimesToMeetConstraints acts on
   // the solved trajectory), the stretch in place on coeffs, then solveLinear() at the stretched times
-  MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, st_solve, s, false));
+  MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, st_solve, s, false, nullptr, slot));
   MTG_TRY(launch_scale_to_constraints(h, p->N, p->K, p->D, B, seg_times, coeffs, v_max, a_max, seg_times_out, coeffs,
                                       st_solve, within_range, maxima, st_scale, s));
-  MTG_TRY(launch_solve(h, p, topo, B, seg_times_out, d_fixed, nullptr, coeffs, nullptr, st_resolve, s, false));
+  MTG_TRY(launch_solve(h, p, topo, B, seg_times_out, d_fixed, nullptr, coeffs, nullptr, st_resolve, s, false, nullptr,
+                       slot));
   if (status) {
     MTG_CUDA(h, cudaMemcpyAsync(status, st_scale, sizeof(int32_t) * size_t(B), cudaMemcpyDeviceToDevice, s));
     const int threads = 128;
@@ -1586,358 +1694,171 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
   return arena_release(h, ar, s);
 }
 
-// ---- host-pointer variants: chunked H2D -> kernel -> D2H over kPipe streams ---------------
-// Every exit of a host-pointer entry point -- error returns included -- waits for all pipeline streams:
-// copies into caller-owned (possibly pinned) buffers must not be in flight when the caller gets control back.
-struct PipeSyncGuard {
-  mtg_handle* h;
-  ~PipeSyncGuard() {
-    for (int i = 0; i < mtg_handle::kPipe; ++i)
-      if (h->streams[i]) cudaStreamSynchronize(h->streams[i]);
-  }
-};
+int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                             const double* d_fixed, double v_max, double a_max, double* coeffs,
+                                             double* seg_times_out, int32_t* within_range, double* maxima,
+                                             int32_t* status, void* stream) {
+  return run_problem_entry(
+      h, valid_violation(p, B, v_max, a_max, seg_times, d_fixed, coeffs, seg_times_out), p, B, [&](CachedTopology* topo) {
+        return launch_scale_with_violation(h, p, topo, B, seg_times, d_fixed, v_max, a_max, coeffs, seg_times_out,
+                                           within_range, maxima, status, (cudaStream_t)stream, mtg_handle::kPipe);
+      });
+}
 
-static int host_pipeline(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
-                         const double* d_fixed, const double* d_free_in, double* coeffs, double* d_free_out,
-                         int32_t* status, bool backsub_only) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || (B > 0 && (!seg_times || !d_fixed || !coeffs))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
-  const Layout& L = topo->layout;
-  const size_t K = p->K, D = p->D, N = p->N;
-  const size_t b_times = K * 8, b_fix = D * L.n_fixed * 8, b_free = D * size_t(L.n_free) * 8,
-               b_coef = K * D * N * 8;
-  const bool need_free_in = backsub_only && L.n_free > 0;
-  if (need_free_in && !d_free_in) {
-    h->error = "d_free is required";
-    return MTG_ERR_BAD_ARG;
-  }
-  // chunk so that the pipeline has work for every stream but stays in a few tens of MB
-  int64_t chunk = std::max<int64_t>(1, std::min<int64_t>((B + mtg_handle::kPipe - 1) / mtg_handle::kPipe, 32768));
-  if (B <= 4096) chunk = B;
-  int slot = 0;
-  PipeSyncGuard sync_on_exit{h};
-  for (int64_t b0 = 0; b0 < B; b0 += chunk, slot = (slot + 1) % mtg_handle::kPipe) {
-    const int64_t nb = std::min<int64_t>(chunk, B - b0);
-    const size_t o_times = 0;
-    const size_t o_fix = align_up(o_times + b_times * nb);
-    const size_t o_freein = align_up(o_fix + b_fix * nb);
-    const size_t o_coef = align_up(o_freein + (need_free_in ? b_free * nb : 0));
-    const size_t o_free = align_up(o_coef + b_coef * nb);
-    const size_t o_stat = align_up(o_free + (d_free_out ? b_free * nb : 0));
-    const size_t total = align_up(o_stat + (status ? 4 * nb : 0));
-    MTG_TRY(ensure_pipe(h, slot, total));
-    cudaStream_t s = h->streams[slot];
-    char* base = static_cast<char*>(h->dev_buf[slot]);
-    MTG_CUDA(h, cudaMemcpyAsync(base + o_times, seg_times + b0 * K, b_times * nb, cudaMemcpyHostToDevice, s));
-    MTG_CUDA(h, cudaMemcpyAsync(base + o_fix, d_fixed + b0 * D * L.n_fixed, b_fix * nb, cudaMemcpyHostToDevice, s));
-    if (need_free_in)
-      MTG_CUDA(h, cudaMemcpyAsync(base + o_freein, d_free_in + b0 * D * L.n_free, b_free * nb,
-                                  cudaMemcpyHostToDevice, s));
-    MTG_TRY(launch_solve(h, p, topo, nb, reinterpret_cast<double*>(base + o_times),
-                         reinterpret_cast<double*>(base + o_fix),
-                         need_free_in ? reinterpret_cast<double*>(base + o_freein) : nullptr,
-                         reinterpret_cast<double*>(base + o_coef),
-                         d_free_out ? reinterpret_cast<double*>(base + o_free) : nullptr,
-                         status ? reinterpret_cast<int32_t*>(base + o_stat) : nullptr, s, backsub_only, nullptr, slot));
-    MTG_CUDA(h, cudaMemcpyAsync(coeffs + b0 * K * D * N, base + o_coef, b_coef * nb, cudaMemcpyDeviceToHost, s));
-    if (d_free_out && L.n_free > 0)
-      MTG_CUDA(h, cudaMemcpyAsync(d_free_out + b0 * D * L.n_free, base + o_free, b_free * nb,
-                                  cudaMemcpyDeviceToHost, s));
-    if (status) MTG_CUDA(h, cudaMemcpyAsync(status + b0, base + o_stat, 4 * nb, cudaMemcpyDeviceToHost, s));
-    // the buffer of this slot is reused kPipe chunks later: wait for it then
-    const int next = (slot + 1) % mtg_handle::kPipe;
-    if (b0 + chunk < B && h->streams[next]) MTG_CUDA(h, cudaStreamSynchronize(h->streams[next]));
-  }
-  for (int i = 0; i < mtg_handle::kPipe; ++i)
-    if (h->streams[i]) MTG_CUDA(h, cudaStreamSynchronize(h->streams[i]));
-  return MTG_OK;
+// ---- host-pointer entry points: the device entry's check and launcher, around stage_host() ------------------------
+
+static int solve_host(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times, const double* d_fixed,
+                      const double* d_free_in, double* coeffs, double* d_free, int32_t* status, bool backsub_only) {
+  return run_problem_entry(h, valid_problem_args(p, B, seg_times, d_fixed, coeffs), p, B, [&](CachedTopology* topo) {
+    const Layout& L = topo->layout;
+    if (backsub_only) MTG_TRY(check_d_free(h, L, d_free_in));
+    const size_t K = p->K, D = p->D, N = p->N;
+    const HostBuf bufs[] = {{seg_times, nullptr, K * 8},           {d_fixed, nullptr, D * L.n_fixed * 8},
+                            {d_free_in, nullptr, D * L.n_free * 8}, {nullptr, coeffs, K * D * N * 8},
+                            {nullptr, d_free, D * L.n_free * 8},    {nullptr, status, 4}};
+    return stage_host(h, B, Staging::Pipelined, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+      return launch_solve(h, p, topo, nb, d[0], d[1], d[2], d[3], d[4], d[5], s, backsub_only, nullptr, slot);
+    });
+  });
 }
 
 int mtg_solve_linear_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                     const double* d_fixed, double* coeffs, double* d_free, int32_t* status) {
-  return host_pipeline(h, p, B, seg_times, d_fixed, nullptr, coeffs, d_free, status, false);
+  return solve_host(h, p, B, seg_times, d_fixed, nullptr, coeffs, d_free, status, false);
 }
 
 int mtg_solve_waypoints_nfabian_batch_host_f64(mtg_handle* h, int32_t N, int32_t r, int32_t K, int32_t D, int64_t B,
                                                const double* positions, double v_max, double a_max, double magic,
                                                double* coeffs, double* seg_times_out, int32_t* status) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  mtg_problem p = {N, r, K, D, nullptr};
-  if (!valid_problem(&p) || B < 0 || (B > 0 && (!positions || !coeffs))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  const size_t b_pos = size_t(K + 1) * D * 8, b_coef = size_t(K) * D * N * 8, b_t = size_t(K) * 8;
-  int64_t chunk = std::max<int64_t>(1, std::min<int64_t>((B + mtg_handle::kPipe - 1) / mtg_handle::kPipe, 32768));
-  if (B <= 4096) chunk = B;
-  int slot = 0;
-  PipeSyncGuard sync_on_exit{h};
-  for (int64_t b0 = 0; b0 < B; b0 += chunk, slot = (slot + 1) % mtg_handle::kPipe) {
-    const int64_t nb = std::min<int64_t>(chunk, B - b0);
-    const size_t o_coef = align_up(b_pos * nb), o_t = align_up(o_coef + b_coef * nb), o_stat = align_up(o_t + b_t * nb);
-    MTG_TRY(ensure_pipe(h, slot, align_up(o_stat + 4 * nb)));
-    cudaStream_t s = h->streams[slot];
-    char* base = static_cast<char*>(h->dev_buf[slot]);
-    MTG_CUDA(h, cudaMemcpyAsync(base, positions + b0 * (K + 1) * D, b_pos * nb, cudaMemcpyHostToDevice, s));
-    MTG_TRY(nfabian_device(h, N, r, K, D, nb, reinterpret_cast<double*>(base), v_max, a_max, magic,
-                           reinterpret_cast<double*>(base + o_coef), reinterpret_cast<double*>(base + o_t),
-                           reinterpret_cast<int32_t*>(base + o_stat), s, slot));
-    MTG_CUDA(h, cudaMemcpyAsync(coeffs + b0 * K * D * N, base + o_coef, b_coef * nb, cudaMemcpyDeviceToHost, s));
-    if (seg_times_out)
-      MTG_CUDA(h, cudaMemcpyAsync(seg_times_out + b0 * K, base + o_t, b_t * nb, cudaMemcpyDeviceToHost, s));
-    if (status) MTG_CUDA(h, cudaMemcpyAsync(status + b0, base + o_stat, 4 * nb, cudaMemcpyDeviceToHost, s));
-    const int next = (slot + 1) % mtg_handle::kPipe;
-    if (b0 + chunk < B && h->streams[next]) MTG_CUDA(h, cudaStreamSynchronize(h->streams[next]));
-  }
-  for (int i = 0; i < mtg_handle::kPipe; ++i)
-    if (h->streams[i]) MTG_CUDA(h, cudaStreamSynchronize(h->streams[i]));
-  return MTG_OK;
+  const mtg_problem p = {N, r, K, D, nullptr};
+  return run_problem_entry(h, valid_nfabian(&p, B, positions, v_max, a_max, coeffs), &p, B, [&](CachedTopology* topo) {
+    const HostBuf bufs[] = {{positions, nullptr, size_t(K + 1) * D * 8},
+                            {nullptr, coeffs, size_t(K) * D * N * 8},
+                            {nullptr, seg_times_out, size_t(K) * 8},
+                            {nullptr, status, 4}};
+    return stage_host(h, B, Staging::Pipelined, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+      return launch_nfabian(h, &p, topo, nb, d[0], v_max, a_max, magic, d[1], d[2], d[3], s, slot);
+    });
+  });
 }
 
 int mtg_coeffs_from_constraints_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
                                                const double* seg_times, const double* d_fixed,
                                                const double* d_free, double* coeffs) {
-  return host_pipeline(h, p, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, true);
+  return solve_host(h, p, B, seg_times, d_fixed, d_free, coeffs, nullptr, nullptr, true);
 }
 
 int mtg_compute_cost_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                     const double* coeffs, double* cost) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || (B > 0 && (!seg_times || !coeffs || !cost))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  const size_t K = p->K, D = p->D, N = p->N;
-  const size_t o_coef = align_up(K * 8 * B), o_cost = align_up(o_coef + K * D * N * 8 * B);
-  MTG_TRY(ensure_pipe(h, 0, o_cost + 8 * B));
-  cudaStream_t s = h->streams[0];
-  char* base = static_cast<char*>(h->dev_buf[0]);
-  PipeSyncGuard sync_on_exit{h};  // a refused launch (K * D too large) returns with the input copies enqueued
-  MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, K * 8 * B, cudaMemcpyHostToDevice, s));
-  MTG_CUDA(h, cudaMemcpyAsync(base + o_coef, coeffs, K * D * N * 8 * B, cudaMemcpyHostToDevice, s));
-  MTG_TRY(mtg_compute_cost_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_coef),
-                                     reinterpret_cast<double*>(base + o_cost), s));
-  MTG_CUDA(h, cudaMemcpyAsync(cost, base + o_cost, 8 * B, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaStreamSynchronize(s));
-  return MTG_OK;
+  return run_entry(h, valid_problem_args(p, B, seg_times, coeffs, cost), B, [&] {
+    const size_t K = p->K, D = p->D, N = p->N;
+    const HostBuf bufs[] = {{seg_times, nullptr, K * 8}, {coeffs, nullptr, K * D * N * 8}, {nullptr, cost, 8}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
+      return launch_cost(h, p, nb, d[0], d[1], d[2], s);
+    });
+  });
 }
 
 int mtg_cost_gradient_mellinger_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                                const double* d_fixed, double* cost, double* grad) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || (B > 0 && (!seg_times || !d_fixed || !grad))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
-  const size_t K = p->K, D = p->D, nf = topo->layout.n_fixed;
-  const size_t o_f = align_up(K * 8 * B), o_c = align_up(o_f + D * nf * 8 * B), o_g = align_up(o_c + 8 * B);
-  MTG_TRY(ensure_pipe(h, 0, o_g + K * 8 * B));
-  cudaStream_t s = h->streams[0];
-  char* base = static_cast<char*>(h->dev_buf[0]);
-  PipeSyncGuard sync_on_exit{h};
-  MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, K * 8 * B, cudaMemcpyHostToDevice, s));
-  MTG_CUDA(h, cudaMemcpyAsync(base + o_f, d_fixed, D * nf * 8 * B, cudaMemcpyHostToDevice, s));
-  MTG_TRY(mtg_cost_gradient_mellinger_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_f),
-                                                reinterpret_cast<double*>(base + o_c), reinterpret_cast<double*>(base + o_g), s));
-  if (cost) MTG_CUDA(h, cudaMemcpyAsync(cost, base + o_c, 8 * B, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaMemcpyAsync(grad, base + o_g, K * 8 * B, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaStreamSynchronize(s));
-  return MTG_OK;
+  return run_problem_entry(h, valid_problem_args(p, B, seg_times, d_fixed, grad), p, B, [&](CachedTopology* topo) {
+    const size_t K = p->K, D = p->D;
+    const HostBuf bufs[] = {{seg_times, nullptr, K * 8},
+                            {d_fixed, nullptr, D * topo->layout.n_fixed * 8},
+                            {nullptr, cost, 8},
+                            {nullptr, grad, K * 8}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+      return launch_mellinger(h, p, topo, nb, d[0], d[1], d[2], d[3], s, slot);
+    });
+  });
 }
 
 int mtg_evaluate_range_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                                       const double* coeffs, double t_start, double t_end, double dt, int32_t n_derivs,
                                       const int32_t* derivs, int32_t max_samples, double* out, int32_t* n_samples,
                                       double* sampling_times) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (N < 1 || N > MTG_MAX_N || K < 1 || D < 1 || B < 0 || n_derivs < 1 || n_derivs > 8 || max_samples < 0 ||
-      (B > 0 && (!seg_times || !coeffs || !n_samples || (max_samples > 0 && !out)))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  const size_t b_t = size_t(K) * 8 * B, b_c = size_t(K) * D * N * 8 * B, b_o = size_t(max_samples) * n_derivs * D * 8 * B,
-               b_n = 4 * size_t(B), b_s = size_t(max_samples) * 8 * B;
-  const size_t o_c = align_up(b_t), o_o = align_up(o_c + b_c), o_n = align_up(o_o + b_o), o_s = align_up(o_n + b_n);
-  MTG_TRY(ensure_pipe(h, 0, o_s + b_s));
-  cudaStream_t s = h->streams[0];
-  char* base = static_cast<char*>(h->dev_buf[0]);
-  PipeSyncGuard sync_on_exit{h};
-  MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, b_t, cudaMemcpyHostToDevice, s));
-  MTG_CUDA(h, cudaMemcpyAsync(base + o_c, coeffs, b_c, cudaMemcpyHostToDevice, s));
-  MTG_TRY(mtg_evaluate_range_batch_f64(h, N, K, D, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_c),
-                                       t_start, t_end, dt, n_derivs, derivs, max_samples, reinterpret_cast<double*>(base + o_o),
-                                       reinterpret_cast<int32_t*>(base + o_n),
-                                       sampling_times ? reinterpret_cast<double*>(base + o_s) : nullptr, s));
-  if (max_samples > 0) MTG_CUDA(h, cudaMemcpyAsync(out, base + o_o, b_o, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaMemcpyAsync(n_samples, base + o_n, b_n, cudaMemcpyDeviceToHost, s));
-  if (sampling_times && max_samples > 0)
-    MTG_CUDA(h, cudaMemcpyAsync(sampling_times, base + o_s, b_s, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaStreamSynchronize(s));
-  return MTG_OK;
+  return run_entry(h, valid_range(N, K, D, B, dt, n_derivs, derivs, max_samples, seg_times, coeffs, out, n_samples), B,
+                   [&] {
+                     const HostBuf bufs[] = {{seg_times, nullptr, size_t(K) * 8},
+                                             {coeffs, nullptr, size_t(K) * D * N * 8},
+                                             {nullptr, out, size_t(max_samples) * n_derivs * D * 8},
+                                             {nullptr, n_samples, 4},
+                                             {nullptr, sampling_times, size_t(max_samples) * 8}};
+                     return stage_host(h, B, Staging::OneChunk, bufs,
+                                       [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+                                         return launch_range(h, N, K, D, nb, d[0], d[1], t_start, t_end, dt, n_derivs,
+                                                             derivs, max_samples, d[2], d[3], d[4], s, slot);
+                                       });
+                   });
 }
 
 int mtg_max_magnitude_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                                      const double* coeffs, int32_t n_derivs, const int32_t* derivs, double* value,
                                      double* time, int32_t* segment, int32_t* status) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_extrema_args(N, K, D, B, n_derivs, derivs) || (B > 0 && (!seg_times || !coeffs || !value))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  const size_t b_t = size_t(K) * 8 * B, b_c = size_t(K) * D * N * 8 * B, b_v = size_t(n_derivs) * 8 * B,
-               b_s = size_t(n_derivs) * 4 * B;
-  const size_t o_c = align_up(b_t), o_v = align_up(o_c + b_c), o_t = align_up(o_v + b_v), o_s = align_up(o_t + b_v),
-               o_st = align_up(o_s + b_s);
-  MTG_TRY(ensure_pipe(h, 0, o_st + 4 * size_t(B)));
-  cudaStream_t s = h->streams[0];
-  char* base = static_cast<char*>(h->dev_buf[0]);
-  PipeSyncGuard sync_on_exit{h};
-  MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, b_t, cudaMemcpyHostToDevice, s));
-  MTG_CUDA(h, cudaMemcpyAsync(base + o_c, coeffs, b_c, cudaMemcpyHostToDevice, s));
-  MTG_TRY(mtg_max_magnitude_batch_f64(h, N, K, D, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_c),
-                                      n_derivs, derivs, reinterpret_cast<double*>(base + o_v),
-                                      time ? reinterpret_cast<double*>(base + o_t) : nullptr,
-                                      segment ? reinterpret_cast<int32_t*>(base + o_s) : nullptr,
-                                      status ? reinterpret_cast<int32_t*>(base + o_st) : nullptr, s));
-  MTG_CUDA(h, cudaMemcpyAsync(value, base + o_v, b_v, cudaMemcpyDeviceToHost, s));
-  if (time) MTG_CUDA(h, cudaMemcpyAsync(time, base + o_t, b_v, cudaMemcpyDeviceToHost, s));
-  if (segment) MTG_CUDA(h, cudaMemcpyAsync(segment, base + o_s, b_s, cudaMemcpyDeviceToHost, s));
-  if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_st, 4 * size_t(B), cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaStreamSynchronize(s));
-  return MTG_OK;
+  return run_entry(h, valid_extrema_args(N, K, D, B, n_derivs, derivs, seg_times, coeffs, value), B, [&] {
+    const HostBuf bufs[] = {{seg_times, nullptr, size_t(K) * 8},       {coeffs, nullptr, size_t(K) * D * N * 8},
+                            {nullptr, value, size_t(n_derivs) * 8},    {nullptr, time, size_t(n_derivs) * 8},
+                            {nullptr, segment, size_t(n_derivs) * 4},  {nullptr, status, 4}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
+      return launch_max_magnitude(h, N, K, D, nb, d[0], d[1], n_derivs, derivs, d[2], d[3], d[4], d[5], s);
+    });
+  });
 }
 
 int mtg_time_objective_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
                                       const double* d_fixed, const double* d_free, const mtg_time_objective* obj,
                                       double* coeffs, double* objective, double* terms, int32_t* status) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || B < 0 || !valid_objective(p, obj) ||
-      (B > 0 && (!seg_times || !d_fixed || !coeffs || !objective))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
-  const size_t K = p->K, D = p->D, N = p->N, nf = topo->layout.n_fixed, np = topo->layout.n_free;
-  const size_t b_t = K * 8 * B, b_f = D * nf * 8 * B, b_p = d_free ? D * np * 8 * B : 0, b_c = K * D * N * 8 * B;
-  const size_t o_f = align_up(b_t), o_p = align_up(o_f + b_f), o_c = align_up(o_p + b_p), o_o = align_up(o_c + b_c),
-               o_m = align_up(o_o + 8 * B), o_s = align_up(o_m + (terms ? 24 * B : 0));
-  MTG_TRY(ensure_pipe(h, 0, o_s + 4 * B));
-  cudaStream_t s = h->streams[0];
-  char* base = static_cast<char*>(h->dev_buf[0]);
-  PipeSyncGuard sync_on_exit{h};
-  MTG_CUDA(h, cudaMemcpyAsync(base, seg_times, b_t, cudaMemcpyHostToDevice, s));
-  MTG_CUDA(h, cudaMemcpyAsync(base + o_f, d_fixed, b_f, cudaMemcpyHostToDevice, s));
-  if (d_free && b_p) MTG_CUDA(h, cudaMemcpyAsync(base + o_p, d_free, b_p, cudaMemcpyHostToDevice, s));
-  MTG_TRY(mtg_time_objective_batch_f64(h, p, B, reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + o_f),
-                                       d_free ? reinterpret_cast<double*>(base + o_p) : nullptr, obj,
-                                       reinterpret_cast<double*>(base + o_c), reinterpret_cast<double*>(base + o_o),
-                                       terms ? reinterpret_cast<double*>(base + o_m) : nullptr,
-                                       status ? reinterpret_cast<int32_t*>(base + o_s) : nullptr, s));
-  MTG_CUDA(h, cudaMemcpyAsync(coeffs, base + o_c, b_c, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaMemcpyAsync(objective, base + o_o, 8 * B, cudaMemcpyDeviceToHost, s));
-  if (terms) MTG_CUDA(h, cudaMemcpyAsync(terms, base + o_m, 24 * B, cudaMemcpyDeviceToHost, s));
-  if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_s, 4 * B, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaStreamSynchronize(s));
-  return MTG_OK;
+  return run_problem_entry(
+      h, valid_objective(p, B, obj, seg_times, d_fixed, coeffs, objective), p, B, [&](CachedTopology* topo) {
+        const Layout& L = topo->layout;
+        const size_t K = p->K, D = p->D, N = p->N;
+        const HostBuf bufs[] = {{seg_times, nullptr, K * 8},      {d_fixed, nullptr, D * L.n_fixed * 8},
+                                {d_free, nullptr, D * L.n_free * 8}, {nullptr, coeffs, K * D * N * 8},
+                                {nullptr, objective, 8},          {nullptr, terms, 24},
+                                {nullptr, status, 4}};
+        return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+          return launch_time_objective(h, p, topo, nb, d[0], d[1], d[2], obj, d[3], d[4], d[5], d[6], s, slot);
+        });
+      });
 }
 
 int mtg_scale_to_constraints_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
                                             const double* seg_times, const double* coeffs, double v_max, double a_max,
                                             double* seg_times_out, double* coeffs_out, int32_t* within_range,
                                             double* maxima, int32_t* status) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_scale_args(N, K, D, B, v_max, a_max) ||
-      (B > 0 && (!seg_times || !coeffs || !seg_times_out || !coeffs_out))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  // the stretch runs in place on the device copy; every copy in is queued before any copy out, so the host buffers
-  // may alias too
-  const size_t b_t = size_t(K) * 8 * B, b_c = size_t(K) * D * N * 8 * B;
-  const size_t o_c = align_up(b_t), o_w = align_up(o_c + b_c), o_m = align_up(o_w + 4 * size_t(B)),
-               o_s = align_up(o_m + 16 * size_t(B));
-  MTG_TRY(ensure_pipe(h, 0, o_s + 4 * size_t(B)));
-  cudaStream_t s = h->streams[0];
-  char* base = static_cast<char*>(h->dev_buf[0]);
-  PipeSyncGuard sync_on_exit{h};
-  double* d_t = reinterpret_cast<double*>(base);
-  double* d_c = reinterpret_cast<double*>(base + o_c);
-  MTG_CUDA(h, cudaMemcpyAsync(d_t, seg_times, b_t, cudaMemcpyHostToDevice, s));
-  MTG_CUDA(h, cudaMemcpyAsync(d_c, coeffs, b_c, cudaMemcpyHostToDevice, s));
-  MTG_TRY(mtg_scale_to_constraints_batch_f64(h, N, K, D, B, d_t, d_c, v_max, a_max, d_t, d_c,
-                                             within_range ? reinterpret_cast<int32_t*>(base + o_w) : nullptr,
-                                             maxima ? reinterpret_cast<double*>(base + o_m) : nullptr,
-                                             status ? reinterpret_cast<int32_t*>(base + o_s) : nullptr, s));
-  MTG_CUDA(h, cudaMemcpyAsync(seg_times_out, d_t, b_t, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaMemcpyAsync(coeffs_out, d_c, b_c, cudaMemcpyDeviceToHost, s));
-  if (within_range) MTG_CUDA(h, cudaMemcpyAsync(within_range, base + o_w, 4 * size_t(B), cudaMemcpyDeviceToHost, s));
-  if (maxima) MTG_CUDA(h, cudaMemcpyAsync(maxima, base + o_m, 16 * size_t(B), cudaMemcpyDeviceToHost, s));
-  if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_s, 4 * size_t(B), cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaStreamSynchronize(s));
-  return MTG_OK;
+  return run_entry(h, valid_scale(N, K, D, B, v_max, a_max, seg_times, coeffs, seg_times_out, coeffs_out), B, [&] {
+    // the stretch runs in place on the device copies of the times and coefficients
+    const HostBuf bufs[] = {{seg_times, seg_times_out, size_t(K) * 8},
+                            {coeffs, coeffs_out, size_t(K) * D * N * 8},
+                            {nullptr, within_range, 4},
+                            {nullptr, maxima, 16},
+                            {nullptr, status, 4}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
+      return launch_scale_to_constraints(h, N, K, D, nb, d[0], d[1], v_max, a_max, d[0], d[1], nullptr, d[2], d[3],
+                                         d[4], s);
+    });
+  });
 }
 
 int mtg_scale_times_with_violation_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B,
                                                   const double* seg_times, const double* d_fixed, double v_max,
                                                   double a_max, double* coeffs, double* seg_times_out,
                                                   int32_t* within_range, double* maxima, int32_t* status) {
-  if (!h) return MTG_ERR_BAD_ARG;
-  if (!valid_problem(p) || !valid_scale_args(p->N, p->K, p->D, B, v_max, a_max) ||
-      (B > 0 && (!seg_times || !d_fixed || !coeffs || !seg_times_out))) {
-    h->error = "bad argument";
-    return MTG_ERR_BAD_ARG;
-  }
-  if (B == 0) return MTG_OK;
-  DeviceGuard g(h->device);
-  CachedTopology* topo = get_topology(h, p);
-  if (!topo) return MTG_ERR_CUDA;
-  const size_t K = p->K, D = p->D, N = p->N, nf = topo->layout.n_fixed;
-  const size_t b_t = K * 8 * B, b_f = D * nf * 8 * B, b_c = K * D * N * 8 * B;
-  const size_t o_f = align_up(b_t), o_c = align_up(o_f + b_f), o_w = align_up(o_c + b_c), o_m = align_up(o_w + 4 * B),
-               o_s = align_up(o_m + 16 * B);
-  MTG_TRY(ensure_pipe(h, 0, o_s + 4 * B));
-  cudaStream_t s = h->streams[0];
-  char* base = static_cast<char*>(h->dev_buf[0]);
-  PipeSyncGuard sync_on_exit{h};
-  double* d_t = reinterpret_cast<double*>(base);
-  MTG_CUDA(h, cudaMemcpyAsync(d_t, seg_times, b_t, cudaMemcpyHostToDevice, s));
-  MTG_CUDA(h, cudaMemcpyAsync(base + o_f, d_fixed, b_f, cudaMemcpyHostToDevice, s));
-  MTG_TRY(mtg_scale_times_with_violation_batch_f64(h, p, B, d_t, reinterpret_cast<double*>(base + o_f), v_max, a_max,
-                                                   reinterpret_cast<double*>(base + o_c), d_t,
-                                                   within_range ? reinterpret_cast<int32_t*>(base + o_w) : nullptr,
-                                                   maxima ? reinterpret_cast<double*>(base + o_m) : nullptr,
-                                                   status ? reinterpret_cast<int32_t*>(base + o_s) : nullptr, s));
-  MTG_CUDA(h, cudaMemcpyAsync(coeffs, base + o_c, b_c, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaMemcpyAsync(seg_times_out, d_t, b_t, cudaMemcpyDeviceToHost, s));
-  if (within_range) MTG_CUDA(h, cudaMemcpyAsync(within_range, base + o_w, 4 * B, cudaMemcpyDeviceToHost, s));
-  if (maxima) MTG_CUDA(h, cudaMemcpyAsync(maxima, base + o_m, 16 * B, cudaMemcpyDeviceToHost, s));
-  if (status) MTG_CUDA(h, cudaMemcpyAsync(status, base + o_s, 4 * B, cudaMemcpyDeviceToHost, s));
-  MTG_CUDA(h, cudaStreamSynchronize(s));
-  return MTG_OK;
+  return run_problem_entry(
+      h, valid_violation(p, B, v_max, a_max, seg_times, d_fixed, coeffs, seg_times_out), p, B, [&](CachedTopology* topo) {
+        const size_t K = p->K, D = p->D, N = p->N;
+        // the times go in from seg_times and come back, stretched in place, into seg_times_out
+        const HostBuf bufs[] = {{seg_times, seg_times_out, K * 8},
+                                {d_fixed, nullptr, D * topo->layout.n_fixed * 8},
+                                {nullptr, coeffs, K * D * N * 8},
+                                {nullptr, within_range, 4},
+                                {nullptr, maxima, 16},
+                                {nullptr, status, 4}};
+        return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+          return launch_scale_with_violation(h, p, topo, nb, d[0], d[1], v_max, a_max, d[2], d[0], d[3], d[4], d[5], s,
+                                             slot);
+        });
+      });
 }
 
 void* mtg_host_alloc(mtg_handle* h, uint64_t bytes) {
