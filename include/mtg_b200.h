@@ -56,6 +56,8 @@ extern "C" {
 /* per-trajectory status bits (status[b] == 0 means solved) */
 #define MTG_STATUS_BAD_TIME 1     /* some segment time <= 0, NaN or +inf (reference: CHECK_GT, linear_impl.h:297) */
 #define MTG_STATUS_NOT_SPD 2      /* non-positive / NaN / infinite pivot in the R_pp factorisation */
+#define MTG_STATUS_FEAS_CAPACITY 4 /* input feasibility: a candidate list (48 entries) or the roll/pitch walk (64 levels)
+                                      ran out of room; the segment is reported Indeterminable */
 
 /* which kernel family a problem is routed to (introspection for tests / profiles) */
 #define MTG_KERNEL_WAYPOINT 1     /* specialised block-tridiagonal Cholesky kernels, waypoint topology */
@@ -258,6 +260,55 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
                                              double* seg_times_out, int32_t* within_range, double* maxima,
                                              int32_t* status, void* stream);
 
+/* FeasibilityAnalytic::checkInputFeasibility per segment and checkInputFeasibilityTrajectory per trajectory (reference
+ * mav_trajectory_generation_ros/src/feasibility_analytic.cpp, feasibility_base.cpp).  result[b] is an MTG_FEAS_* code
+ * (InputFeasibilityResult): the first segment that is not Feasible decides, in the reference's order of checks --
+ * thrust in [f_min, f_max] (ThrustLow before ThrustHigh; run when f_min, f_max or omega_xy_max is present), speed over
+ * dims 0..2, yaw rate and yaw acceleration (D = 4 only), then the recursive roll/pitch bound sqrt(j_max / f_min) over
+ * halved sections down to min_section_time.  The roll/pitch step returns only Feasible or Indeterminable (a section
+ * shorter than min_section_time, the whole segment included, is Indeterminable); MTG_FEAS_ROLL_PITCH_RATES is never
+ * returned.  Candidates are 0, T and the exact real roots of each critical polynomial in [0, T] (the reference's
+ * Jenkins-Traub |imag| > eps filter is not reproduced); their values use the reference's arithmetic.
+ *   segment[b]: index of the deciding segment, -1 when the row is Feasible or has a bad time.  segment, status nullable.
+ *   D not 3 or 4: every row Indeterminable at segment 0, as the reference.
+ *   A segment time <= 0 or non-finite: status MTG_STATUS_BAD_TIME, result Indeterminable, segment -1.
+ *   status MTG_STATUS_FEAS_CAPACITY: see above (not met by trajectories with distinct roots and T / min_section_time
+ *   below 2^60).
+ * N even in [4, 12].  The limits are final values: InputConstraints::addConstraint's abs() and f_min / f_max
+ * corrections belong to the caller (the host mirror's InputConstraints applies them).  Refused (MTG_ERR_BAD_ARG, no
+ * launch): a present limit that is NaN or negative, unknown `present` bits, a non-finite gravity, min_section_time <= 0
+ * or non-finite.  An absent limit's value is ignored; +inf never fails. */
+#define MTG_FEAS_FEASIBLE 0
+#define MTG_FEAS_INDETERMINABLE 1
+#define MTG_FEAS_THRUST_HIGH 2
+#define MTG_FEAS_THRUST_LOW 3
+#define MTG_FEAS_VELOCITY 4
+#define MTG_FEAS_ROLL_PITCH_RATES 5
+#define MTG_FEAS_YAW_RATES 6
+#define MTG_FEAS_YAW_ACC 7
+/* mtg_input_constraints::present bits (InputConstraintType order) */
+#define MTG_INPUT_F_MIN (1u << 0)
+#define MTG_INPUT_F_MAX (1u << 1)
+#define MTG_INPUT_V_MAX (1u << 2)
+#define MTG_INPUT_OMEGA_XY_MAX (1u << 3)
+#define MTG_INPUT_OMEGA_Z_MAX (1u << 4)
+#define MTG_INPUT_OMEGA_Z_DOT_MAX (1u << 5)
+#define MTG_INPUT_ALL 0x3fu
+typedef struct mtg_input_constraints {
+  uint32_t present;        /* MTG_INPUT_* bits: which limits apply */
+  double f_min;            /* normalized thrust [m/s^2] */
+  double f_max;
+  double v_max;            /* [m/s] */
+  double omega_xy_max;     /* roll/pitch rate [rad/s] */
+  double omega_z_max;      /* yaw rate [rad/s] */
+  double omega_z_dot_max;  /* yaw acceleration [rad/s^2] */
+  double gravity;          /* added to the z acceleration for the thrust (mav_msgs::kGravity in the reference) */
+  double min_section_time; /* FeasibilityAnalytic::Settings, reference default 0.05 s */
+} mtg_input_constraints;
+int mtg_input_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                    const double* coeffs, const mtg_input_constraints* constraints, int32_t* result,
+                                    int32_t* segment, int32_t* status, void* stream);
+
 /* ---- the hot path, HOST pointers (what PolynomialOptimization<N>::solveLinear() calls) ---- */
 /* Same contract with host buffers: each call refuses what its device entry refuses, before any copy, and
  * returns when the results are in the host buffers.  Pinned buffers (mtg_host_alloc) make the copies
@@ -298,6 +349,11 @@ int mtg_scale_times_with_violation_batch_host_f64(mtg_handle* h, const mtg_probl
                                                   const double* seg_times, const double* d_fixed, double v_max,
                                                   double a_max, double* coeffs, double* seg_times_out,
                                                   int32_t* within_range, double* maxima, int32_t* status);
+
+int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                         const double* seg_times, const double* coeffs,
+                                         const mtg_input_constraints* constraints, int32_t* result, int32_t* segment,
+                                         int32_t* status);
 
 /* ---- memory helpers (so host code above the ABI needs no CUDA headers) -------------------- */
 void* mtg_host_alloc(mtg_handle* h, uint64_t bytes);   /* pinned */

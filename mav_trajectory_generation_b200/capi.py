@@ -37,9 +37,21 @@ EXPORTED_SYMBOLS = [
     "mtg_max_magnitude_batch_f64", "mtg_time_objective_batch_f64", "mtg_max_magnitude_batch_host_f64",
     "mtg_time_objective_batch_host_f64", "mtg_scale_to_constraints_batch_f64",
     "mtg_scale_times_with_violation_batch_f64", "mtg_scale_to_constraints_batch_host_f64",
-    "mtg_scale_times_with_violation_batch_host_f64",
+    "mtg_scale_times_with_violation_batch_host_f64", "mtg_input_feasibility_batch_f64",
+    "mtg_input_feasibility_batch_host_f64",
 ]
 TIME_COST_SQUARED, TIME_COST_RICHTER = 0, 1
+STATUS_FEAS_CAPACITY = 4
+# InputFeasibilityResult
+(FEAS_FEASIBLE, FEAS_INDETERMINABLE, FEAS_THRUST_HIGH, FEAS_THRUST_LOW, FEAS_VELOCITY, FEAS_ROLL_PITCH_RATES,
+ FEAS_YAW_RATES, FEAS_YAW_ACC) = range(8)
+FEAS_NAMES = ("Feasible", "Indeterminable", "InfeasibleThrustHigh", "InfeasibleThrustLow", "InfeasibleVelocity",
+              "InfeasibleRollPitchRates", "InfeasibleYawRates", "InfeasibleYawAcc")
+# InputConstraintType order: the bit of mtg_input_constraints::present
+INPUT_LIMITS = ("f_min", "f_max", "v_max", "omega_xy_max", "omega_z_max", "omega_z_dot_max")
+# Gravity of the host mirror's InputConstraints / FeasibilityAnalytic default (the reference uses mav_msgs::kGravity;
+# mav_comm is not part of this project, so this value was not checked against it).
+GRAVITY = 9.81
 
 
 class MtgProblem(C.Structure):
@@ -59,6 +71,33 @@ class MtgTimeObjective(C.Structure):
     _fields_ = [("time_cost", C.c_int32), ("time_penalty", C.c_double), ("soft_constraint_weight", C.c_double),
                 ("maximum_cost", C.c_double), ("n_constraints", C.c_int32),
                 ("constraints", C.POINTER(MtgSoftConstraint))]
+
+
+class MtgInputConstraints(C.Structure):
+    _fields_ = [("present", C.c_uint32)] + [(n, C.c_double) for n in INPUT_LIMITS] + \
+               [("gravity", C.c_double), ("min_section_time", C.c_double)]
+
+
+def default_input_limits(gravity=GRAVITY):
+    """InputConstraints::setDefaultValues(): every limit present."""
+    return dict(f_min=0.5 * gravity, f_max=1.5 * gravity, v_max=3.0, omega_xy_max=np.pi / 2, omega_z_max=np.pi / 2,
+                omega_z_dot_max=2.0 * np.pi)
+
+
+def input_constraints(limits, min_section_time=0.05, gravity=GRAVITY):
+    """mtg_input_constraints from {name: value} (names of INPUT_LIMITS; a missing name is an absent limit).  The values
+    are passed as given: they are the final limits."""
+    unknown = set(limits) - set(INPUT_LIMITS)
+    if unknown:
+        raise ValueError(f"unknown input constraints {sorted(unknown)}")
+    c = MtgInputConstraints()
+    for q, n in enumerate(INPUT_LIMITS):
+        if n in limits:
+            c.present |= 1 << q
+            setattr(c, n, float(limits[n]))
+    c.gravity = float(gravity)
+    c.min_section_time = float(min_section_time)
+    return c
 
 
 def time_objective_params(time_cost=TIME_COST_SQUARED, time_penalty=500.0, soft_constraint_weight=100.0,
@@ -147,6 +186,10 @@ def load():
                                                            dp, dp, dp, vp]
     L.mtg_scale_times_with_violation_batch_host_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, dbl, dbl, dp,
                                                                 dp, dp, dp, dp]
+    L.mtg_input_feasibility_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
+                                                  C.POINTER(MtgInputConstraints), dp, dp, dp, vp]
+    L.mtg_input_feasibility_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
+                                                       C.POINTER(MtgInputConstraints), dp, dp, dp]
     for name in EXPORTED_SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export what the header declares
     _lib = L
@@ -397,6 +440,24 @@ class Solver:
         self._check(rc, "mtg_scale_times_with_violation_batch_f64")
         return coeffs, seg_times_out, within, maxima, status
 
+    def check_input_feasibility(self, seg_times, coeffs, limits, min_section_time=0.05, gravity=GRAVITY, stream=None):
+        """Batched FeasibilityAnalytic::checkInputFeasibilityTrajectory: (result [B], segment [B], status [B]), int32.
+        limits: {name: value} over INPUT_LIMITS (absent name = no limit; default_input_limits() gives the reference's
+        defaults) or an MtgInputConstraints."""
+        import torch
+        B, K, D, N = coeffs.shape
+        dev = coeffs.device
+        ic = limits if isinstance(limits, MtgInputConstraints) else input_constraints(limits, min_section_time, gravity)
+        result = torch.empty((B,), dtype=torch.int32, device=dev)
+        segment = torch.empty((B,), dtype=torch.int32, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.mtg_input_feasibility_batch_f64(self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(),
+                                                      C.byref(ic), result.data_ptr(), segment.data_ptr(),
+                                                      status.data_ptr(), s)
+        self._check(rc, "mtg_input_feasibility_batch_f64")
+        return result, segment, status
+
     def coeffs_from_constraints(self, prob, seg_times, d_fixed, d_free, coeffs=None, stream=None):
         import torch
         B = seg_times.shape[0]
@@ -522,3 +583,14 @@ class Solver:
             self._hptr(status))
         self._check(rc, "mtg_scale_times_with_violation_batch_host_f64")
         return coeffs
+
+    def check_input_feasibility_host(self, seg_times, coeffs, limits, result, segment=None, status=None,
+                                     min_section_time=0.05, gravity=GRAVITY):
+        """check_input_feasibility into host buffers: result [B], segment [B] or None, status [B] or None (int32)."""
+        B, K, D, N = coeffs.shape
+        ic = limits if isinstance(limits, MtgInputConstraints) else input_constraints(limits, min_section_time, gravity)
+        rc = self.lib.mtg_input_feasibility_batch_host_f64(self.h, N, K, D, B, self._hptr(seg_times),
+                                                           self._hptr(coeffs), C.byref(ic), self._hptr(result),
+                                                           self._hptr(segment), self._hptr(status))
+        self._check(rc, "mtg_input_feasibility_batch_host_f64")
+        return result

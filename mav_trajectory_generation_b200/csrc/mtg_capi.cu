@@ -14,6 +14,7 @@
 
 #include "../../include/mtg_b200.h"
 #include "mtg_extrema_kernel.cuh"
+#include "mtg_feasibility_kernel.cuh"
 #include "mtg_generic_kernel.cuh"
 #include "mtg_twisted_kernel.cuh"
 #include "mtg_twisted_tmem_kernel.cuh"
@@ -1705,6 +1706,70 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
       });
 }
 
+// FeasibilityAnalytic: N even in [4, 12]; the limits are final values (the host mirror's InputConstraints applies
+// addConstraint's corrections), each present one not NaN and >= 0 (+inf never fails); gravity finite; min_section_time
+// > 0 and finite.  Any D: rows with D not 3 or 4 are Indeterminable, as in the reference.
+static bool valid_feasibility(int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                              const double* coeffs, const mtg_input_constraints* ic, const int32_t* result) {
+  if (N < 4 || N > MTG_MAX_N || (N & 1) || K < 1 || D < 1 || !ic) return false;
+  if (ic->present & ~uint32_t(MTG_INPUT_ALL)) return false;
+  const double limits[6] = {ic->f_min, ic->f_max, ic->v_max, ic->omega_xy_max, ic->omega_z_max, ic->omega_z_dot_max};
+  for (int q = 0; q < 6; ++q)
+    if ((ic->present >> q & 1u) && !(limits[q] >= 0.0)) return false;
+  if (!std::isfinite(ic->gravity) || !(ic->min_section_time > 0.0) || !std::isfinite(ic->min_section_time))
+    return false;
+  return valid_rows(B, {seg_times, coeffs, result});
+}
+
+static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                    const double* coeffs, const mtg_input_constraints* ic, int32_t* result,
+                                    int32_t* segment, int32_t* status, cudaStream_t s) {
+  mtg::FeasParams fp;
+  fp.K = K;
+  fp.D = D;
+  fp.present = ic->present;
+  fp.f_min = ic->f_min;
+  fp.f_max = ic->f_max;
+  fp.v_max = ic->v_max;
+  fp.omega_xy = ic->omega_xy_max;
+  fp.omega_z = ic->omega_z_max;
+  fp.omega_z_dot = ic->omega_z_dot_max;
+  fp.gravity = ic->gravity;
+  fp.min_section_time = ic->min_section_time;
+  fp.B = B;
+  fp.times = seg_times;
+  fp.coeffs = coeffs;
+  fp.result = result;
+  fp.segment = segment;
+  fp.status = status;
+  const int tpb = std::max(1, mtg::kExtremaThreads / K);
+  const size_t smem = size_t(tpb) * K * sizeof(int);
+  if (smem > h->smem_optin) {
+    h->error = "mtg_input_feasibility_batch_f64: K too large";
+    return MTG_ERR_BAD_ARG;
+  }
+  typedef void (*FeasFn)(const mtg::FeasParams, const int);
+  static const FeasFn kFeas[MTG_MAX_N / 2 - 1] = {
+      mtg::input_feasibility_kernel<4>, mtg::input_feasibility_kernel<6>, mtg::input_feasibility_kernel<8>,
+      mtg::input_feasibility_kernel<10>, mtg::input_feasibility_kernel<12>};
+  const FeasFn fn = kFeas[N / 2 - 2];
+  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
+  const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
+  fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(fp, tpb);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  return MTG_OK;
+}
+
+int mtg_input_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                    const double* coeffs, const mtg_input_constraints* constraints, int32_t* result,
+                                    int32_t* segment, int32_t* status, void* stream) {
+  return run_entry(h, valid_feasibility(N, K, D, B, seg_times, coeffs, constraints, result), B, [&] {
+    return launch_input_feasibility(h, N, K, D, B, seg_times, coeffs, constraints, result, segment, status,
+                                    (cudaStream_t)stream);
+  });
+}
+
 // ---- host-pointer entry points: the device entry's check and launcher, around stage_host() ------------------------
 
 static int solve_host(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times, const double* d_fixed,
@@ -1859,6 +1924,22 @@ int mtg_scale_times_with_violation_batch_host_f64(mtg_handle* h, const mtg_probl
                                              slot);
         });
       });
+}
+
+int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                         const double* seg_times, const double* coeffs,
+                                         const mtg_input_constraints* constraints, int32_t* result, int32_t* segment,
+                                         int32_t* status) {
+  return run_entry(h, valid_feasibility(N, K, D, B, seg_times, coeffs, constraints, result), B, [&] {
+    const HostBuf bufs[] = {{seg_times, nullptr, size_t(K) * 8},
+                            {coeffs, nullptr, size_t(K) * D * N * 8},
+                            {nullptr, result, 4},
+                            {nullptr, segment, 4},
+                            {nullptr, status, 4}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
+      return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s);
+    });
+  });
 }
 
 void* mtg_host_alloc(mtg_handle* h, uint64_t bytes) {

@@ -106,14 +106,17 @@ __device__ double extrema_refine(const double (&g)[M], double lo, double hi) {
   return x;
 }
 
-// Calls visit(tau) for every candidate tau in (0, 1) of the critical polynomial g, in increasing order.
+// Calls visit(tau, root) for every candidate tau in (0, 1) of the critical polynomial g, in increasing order.  root is
+// true for a refined root and for the midpoint of an interval still unresolved at the depth cap or node budget, false
+// for the extra safety samples (halving points, the ends of an unresolved interval): a whole-segment extremum may use
+// every candidate, a check confined to a sub-interval only the first kind (the reference's candidate set).
 template <int M, typename Visit>
 __device__ void extrema_candidates(const double (&g)[M], Visit&& visit) {
   int level = 0, nodes = 0;
   unsigned idx = 0;
   while (true) {
     const double h = ldexp(1.0, -level), a = double(idx) * h;
-    if (idx & 1u) visit(a);  // a halving point
+    if (idx & 1u) visit(a, false);  // a halving point
     double b[M];
     extrema_bernstein(g, a, h, b);
     ++nodes;
@@ -128,14 +131,14 @@ __device__ void extrema_candidates(const double (&g)[M], Visit&& visit) {
     }
     bool descend = false;
     if (changes == 1 && b[0] != 0.0 && b[M - 1] != 0.0) {
-      visit(extrema_refine(g, a, a + h));
+      visit(extrema_refine(g, a, a + h), true);
     } else if (changes >= 1) {
       if (level < kExtremaMaxDepth && nodes < kExtremaNodeBudget) {
         descend = true;
       } else {
-        visit(a);
-        visit(a + 0.5 * h);
-        visit(a + h);
+        visit(a, false);
+        visit(a + 0.5 * h, true);
+        visit(a + h, false);
       }
     }
     if (descend) {
@@ -166,15 +169,12 @@ __device__ __forceinline__ double extrema_magnitude(const double* __restrict__ c
   return sqrt(sq);
 }
 
-// The largest |p^(k)| of one segment (coefficients c [D][N], time T > 0 and finite) and where it is: the candidates
-// 0, T and the critical points, in the reference's order (0, T, then the critical points, here increasing).  best_v
-// and best_t start at 0: a candidate replaces them only when strictly larger.
-template <int N>
-__device__ __forceinline__ void extrema_segment_max(const double* __restrict__ c, double T, int D, int k,
-                                                    double& best_v, double& best_t) {
-  constexpr int M = N >= 2 ? 2 * N - 2 : 1;  // coefficients of the critical polynomial (degree 2N - 3)
-  // G(tau) = sum_d A_d(tau) A_d'(tau), A_d(tau) = p_d^(k)(tau T) (D = 1: A'(tau)); nominal degree 2N - 3
-  double g[M];
+// The critical polynomial of |p^(k)| on one segment (coefficients c [D][N], time T), in tau = t / T over [0, 1]:
+// G(tau) = sum_d A_d(tau) A_d'(tau), A_d(tau) = p_d^(k)(tau T) (D = 1: A'(tau)); nominal degree 2N - 3.  lift is
+// added to the constant term of p_2^(k) first (gravity on z: the thrust polynomial of the feasibility check).
+template <int N, int M = (N >= 2 ? 2 * N - 2 : 1)>
+__device__ __forceinline__ void extrema_critical(const double* __restrict__ c, double T, int D, int k, double lift,
+                                                 double (&g)[M]) {
 #pragma unroll
   for (int j = 0; j < M; ++j) g[j] = 0.0;
   for (int d = 0; d < D; ++d) {
@@ -186,6 +186,7 @@ __device__ __forceinline__ void extrema_segment_max(const double* __restrict__ c
       for (int j = 0; j < N - 1; ++j) a[j] = double(j + 1) * a[j + 1];
       a[N - 1] = 0.0;
     }
+    if (lift != 0.0 && d == 2) a[0] += lift;
     double tp = T;
 #pragma unroll
     for (int j = 1; j < N; ++j) {
@@ -202,6 +203,17 @@ __device__ __forceinline__ void extrema_segment_max(const double* __restrict__ c
         for (int j = 0; j < N - 1; ++j) g[i + j] = fma(a[i], double(j + 1) * a[j + 1], g[i + j]);
     }
   }
+}
+
+// The largest |p^(k)| of one segment (coefficients c [D][N], time T > 0 and finite) and where it is: the candidates
+// 0, T and the critical points, in the reference's order (0, T, then the critical points, here increasing).  best_v
+// and best_t start at 0: a candidate replaces them only when strictly larger.
+template <int N>
+__device__ __forceinline__ void extrema_segment_max(const double* __restrict__ c, double T, int D, int k,
+                                                    double& best_v, double& best_t) {
+  constexpr int M = N >= 2 ? 2 * N - 2 : 1;  // coefficients of the critical polynomial (degree 2N - 3)
+  double g[M];
+  extrema_critical<N>(c, T, D, k, 0.0, g);
   auto take = [&](double t) {
     const double v = extrema_magnitude<N>(c, D, k, t);
     if (best_v < v) {
@@ -211,7 +223,7 @@ __device__ __forceinline__ void extrema_segment_max(const double* __restrict__ c
   };
   take(0.0);
   take(T);
-  extrema_candidates(g, [&](double tau) { take(tau * T); });
+  extrema_candidates(g, [&](double tau, bool) { take(tau * T); });
 }
 
 // Work item = (trajectory, segment): its best candidate per requested derivative goes to shared memory; one thread per

@@ -15,6 +15,7 @@
 #include "mav_trajectory_generation/segment.h"
 #include "mav_trajectory_generation/trajectory.h"
 #include "mav_trajectory_generation/vertex.h"
+#include "mav_trajectory_generation_ros/feasibility_base.h"
 
 struct mtg_handle;
 
@@ -120,6 +121,10 @@ class BatchCore {
   // PolynomialOptimizationNonLinear::scaleSegmentTimesWithViolation: solve at times_, stretch times_, re-solve into
   // coeffs_ with d_fixed_; status_ receives the OR of the three steps' status bits
   bool scaleSegmentTimesWithViolation(double v_max, double a_max, std::vector<uint8_t>* within_range);
+  // FeasibilityAnalytic::checkInputFeasibilityTrajectory of the current coefficients (result, segment: [B]; segment
+  // nullable, -1 where the row is feasible or has a bad segment time)
+  bool checkInputFeasibility(const InputConstraints& constraints, double min_section_time, double gravity,
+                             std::vector<InputFeasibilityResult>* result, std::vector<int>* segment) const;
   void getSegments(size_t b, Segment::Vector* segments) const;
 
   int N_;

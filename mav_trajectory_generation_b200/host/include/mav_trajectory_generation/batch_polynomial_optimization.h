@@ -105,6 +105,15 @@ class BatchPolynomialOptimization {
   bool scaleSegmentTimesWithViolation(double v_max, double a_max, std::vector<uint8_t>* within_range = nullptr) {
     return core_.scaleSegmentTimesWithViolation(v_max, a_max, within_range);
   }
+  // FeasibilityAnalytic::checkInputFeasibilityTrajectory (reference mav_trajectory_generation_ros/src/
+  // feasibility_analytic.cpp, feasibility_base.cpp) of every trajectory at its current coefficients, on the GPU:
+  // result[b], and segment[b] = the first segment that is not feasible (-1 when the row is feasible or has a segment
+  // time <= 0 or non-finite; such a row is Indeterminable).  Candidates are exact real roots, not Jenkins-Traub's.
+  bool checkInputFeasibility(const InputConstraints& constraints, double min_section_time,
+                             std::vector<InputFeasibilityResult>* result, std::vector<int>* segment = nullptr,
+                             double gravity = kGravity) const {
+    return core_.checkInputFeasibility(constraints, min_section_time, gravity, result, segment);
+  }
 
  private:
   b200::BatchCore core_;

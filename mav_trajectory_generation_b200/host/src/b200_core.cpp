@@ -641,6 +641,31 @@ bool BatchCore::scaleSegmentTimesWithViolation(double v_max, double a_max, std::
   return true;
 }
 
+bool BatchCore::checkInputFeasibility(const InputConstraints& constraints, double min_section_time, double gravity,
+                                      std::vector<InputFeasibilityResult>* result, std::vector<int>* segment) const {
+  CHECK_GT(B_, 0u) << "setup first";
+  CHECK_NOTNULL(result);
+  mtg_input_constraints ic = {};
+  double* values[6] = {&ic.f_min, &ic.f_max, &ic.v_max, &ic.omega_xy_max, &ic.omega_z_max, &ic.omega_z_dot_max};
+  for (int q = 0; q < 6; ++q)
+    if (constraints.getConstraint(q, values[q])) ic.present |= 1u << q;  // InputConstraintType order
+  ic.gravity = gravity;
+  ic.min_section_time = std::abs(min_section_time);  // FeasibilityAnalytic::Settings::setMinSectionTimeS
+  std::vector<int32_t> res(B_, 0), seg(B_, -1);
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_input_feasibility_batch_host_f64(h, N_, topo_.K, topo_.D, static_cast<int64_t>(B_), times_,
+                                                      coeffs_, &ic, res.data(), seg.data(), nullptr);
+  if (rc != MTG_OK) {
+    LOG(ERROR) << "mtg_input_feasibility_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+    return false;
+  }
+  result->resize(B_);
+  for (size_t b = 0; b < B_; ++b) (*result)[b] = static_cast<InputFeasibilityResult>(res[b]);
+  if (segment) segment->assign(seg.begin(), seg.end());
+  return true;
+}
+
 void BatchCore::getSegments(size_t b, Segment::Vector* segments) const {
   CHECK_LT(b, B_);
   unpackSegments(topo_, coeffs_ + b * size_t(topo_.K) * topo_.D * N_, times_ + b * topo_.K, segments);
