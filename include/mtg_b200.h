@@ -309,6 +309,34 @@ int mtg_input_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t
                                     const double* coeffs, const mtg_input_constraints* constraints, int32_t* result,
                                     int32_t* segment, int32_t* status, void* stream);
 
+/* FeasibilityBase::checkHalfPlaneFeasibility per segment and per trajectory (reference
+ * mav_trajectory_generation_ros/src/feasibility_base.cpp:109-154): a segment passes plane (point q, normal n) when
+ * (p(t) - q) . n > 0 at 0, T and every real root in [0, T] of the derivative of the projection n . p(t); the first
+ * segment with a failing plane decides, and within it the first plane.  Values use the reference's arithmetic
+ * (Horner per dimension, the subtraction, the dot product in dimension order), so a NaN value passes, as there.
+ *   feasible[b]: 1 or 0.  segment[b], plane[b]: the first failing pair, -1 when none.  status[b]: 0 or
+ *   MTG_STATUS_BAD_TIME.  segment, plane and status are nullable.
+ *   planes: a HOST array of n_planes entries, read before the call returns (the caller may reuse it at once).  The
+ *   planes are used as given: the reference's HalfPlane constructor normalises the normal, and so do the host mirror's
+ *   HalfPlane and the Python helpers; a normal of another length scales every distance but changes no sign.
+ *   n_planes = 0: every row with D in {3, 4} is feasible.
+ *   D not 3 or 4: every row infeasible with segment 0 and plane -1, as the reference.
+ *   A segment time <= 0 or non-finite: status MTG_STATUS_BAD_TIME, feasible 0, segment and plane -1 (the reference
+ *   would pass it: its candidate list is empty when T < 0).
+ *   Candidates are exact real roots, not Jenkins-Traub's: a row whose smallest distance lies within rounding of 0 can
+ *   be decided differently from the reference.
+ * N even in [2, 12].  Refused (MTG_ERR_BAD_ARG, no launch): n_planes < 0 or > MTG_MAX_HALF_PLANES, a null planes with
+ * n_planes > 0, a non-finite point or normal component, an all-zero normal. */
+#define MTG_MAX_HALF_PLANES 64
+typedef struct mtg_half_plane {
+  double point[3];   /* a point on the plane */
+  double normal[3];  /* points into the allowed half-space */
+} mtg_half_plane;
+int mtg_half_plane_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                         const double* seg_times, const double* coeffs, int32_t n_planes,
+                                         const mtg_half_plane* planes, int32_t* feasible, int32_t* segment,
+                                         int32_t* plane, int32_t* status, void* stream);
+
 /* ---- the hot path, HOST pointers (what PolynomialOptimization<N>::solveLinear() calls) ---- */
 /* Same contract with host buffers: each call refuses what its device entry refuses, before any copy, and
  * returns when the results are in the host buffers.  Pinned buffers (mtg_host_alloc) make the copies
@@ -354,6 +382,10 @@ int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, in
                                          const double* seg_times, const double* coeffs,
                                          const mtg_input_constraints* constraints, int32_t* result, int32_t* segment,
                                          int32_t* status);
+int mtg_half_plane_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                              const double* seg_times, const double* coeffs, int32_t n_planes,
+                                              const mtg_half_plane* planes, int32_t* feasible, int32_t* segment,
+                                              int32_t* plane, int32_t* status);
 
 /* ---- memory helpers (so host code above the ABI needs no CUDA headers) -------------------- */
 void* mtg_host_alloc(mtg_handle* h, uint64_t bytes);   /* pinned */

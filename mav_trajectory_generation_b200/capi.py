@@ -38,7 +38,8 @@ EXPORTED_SYMBOLS = [
     "mtg_time_objective_batch_host_f64", "mtg_scale_to_constraints_batch_f64",
     "mtg_scale_times_with_violation_batch_f64", "mtg_scale_to_constraints_batch_host_f64",
     "mtg_scale_times_with_violation_batch_host_f64", "mtg_input_feasibility_batch_f64",
-    "mtg_input_feasibility_batch_host_f64",
+    "mtg_input_feasibility_batch_host_f64", "mtg_half_plane_feasibility_batch_f64",
+    "mtg_half_plane_feasibility_batch_host_f64",
 ]
 TIME_COST_SQUARED, TIME_COST_RICHTER = 0, 1
 STATUS_FEAS_CAPACITY = 4
@@ -98,6 +99,68 @@ def input_constraints(limits, min_section_time=0.05, gravity=GRAVITY):
     c.gravity = float(gravity)
     c.min_section_time = float(min_section_time)
     return c
+
+
+class MtgHalfPlane(C.Structure):
+    _fields_ = [("point", C.c_double * 3), ("normal", C.c_double * 3)]
+
+
+MAX_HALF_PLANES = 64
+
+
+def _normalized(v):
+    """Eigen's normalized() of a 3-vector: v / sqrt((v0 v0 + v1 v1) + v2 v2), each step rounded once."""
+    v = np.asarray(v, dtype=np.float64)
+    sq = np.float64(0.0)
+    for x in v:
+        sq = sq + x * x
+    if not sq > 0.0:
+        return v.copy()
+    return v / np.sqrt(sq)
+
+
+def half_plane(point, normal):
+    """HalfPlane(point, normal): [1][6] float64 (point, then the normal normalised as the reference does)."""
+    point = np.asarray(point, dtype=np.float64).reshape(3)
+    normal = np.asarray(normal, dtype=np.float64).reshape(3)
+    if not np.linalg.norm(normal) > 0.0:
+        raise ValueError("invalid normal")
+    return np.concatenate([point, _normalized(normal)])[None, :]
+
+
+def half_plane_from_points(a, b, c):
+    """HalfPlane(a, b, c): the plane through a, b and c with normal (b - a) x (c - a), normalised; [1][6] float64."""
+    a, b, c = (np.asarray(x, dtype=np.float64).reshape(3) for x in (a, b, c))
+    if np.array_equal(a, b) or np.array_equal(a, c):
+        raise ValueError("the three points must differ from the first")
+    u, v = b - a, c - a
+    n = np.array([u[1] * v[2] - u[2] * v[1], u[2] * v[0] - u[0] * v[2], u[0] * v[1] - u[1] * v[0]])
+    return np.concatenate([a, _normalized(n)])[None, :]
+
+
+def bounding_box(center, size):
+    """HalfPlane::createBoundingBox(center, size): for each axis, (center - size / 2, +e_axis) then
+    (center + size / 2, -e_axis); [6][6] float64."""
+    center = np.asarray(center, dtype=np.float64).reshape(3)
+    size = np.asarray(size, dtype=np.float64).reshape(3)
+    lo, hi = center - size / 2.0, center + size / 2.0
+    rows = []
+    for axis in range(3):
+        e = np.zeros(3)
+        e[axis] = 1.0
+        rows.append(half_plane(lo, e))
+        rows.append(half_plane(hi, -e))
+    return np.concatenate(rows)
+
+
+def half_plane_array(planes):
+    """An MtgHalfPlane array (and its length) from [P][6] float64 rows: point, normal."""
+    planes = np.asarray(planes, dtype=np.float64).reshape(-1, 6)
+    arr = (MtgHalfPlane * max(len(planes), 1))()
+    for i, row in enumerate(planes):
+        arr[i].point[:] = [float(x) for x in row[:3]]
+        arr[i].normal[:] = [float(x) for x in row[3:]]
+    return arr, len(planes)
 
 
 def time_objective_params(time_cost=TIME_COST_SQUARED, time_penalty=500.0, soft_constraint_weight=100.0,
@@ -190,6 +253,10 @@ def load():
                                                   C.POINTER(MtgInputConstraints), dp, dp, dp, vp]
     L.mtg_input_feasibility_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
                                                        C.POINTER(MtgInputConstraints), dp, dp, dp]
+    L.mtg_half_plane_feasibility_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, C.c_int32,
+                                                       C.POINTER(MtgHalfPlane), dp, dp, dp, dp, vp]
+    L.mtg_half_plane_feasibility_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
+                                                            C.c_int32, C.POINTER(MtgHalfPlane), dp, dp, dp, dp]
     for name in EXPORTED_SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export what the header declares
     _lib = L
@@ -458,6 +525,20 @@ class Solver:
         self._check(rc, "mtg_input_feasibility_batch_f64")
         return result, segment, status
 
+    def check_half_plane_feasibility(self, seg_times, coeffs, planes, stream=None):
+        """Batched FeasibilityBase::checkHalfPlaneFeasibility: (feasible, segment, plane, status), each [B] int32.
+        planes: [P][6] float64 rows (point, normal; see half_plane / bounding_box), used as given."""
+        import torch
+        B, K, D, N = coeffs.shape
+        dev = coeffs.device
+        arr, P = half_plane_array(planes)
+        out = [torch.empty((B,), dtype=torch.int32, device=dev) for _ in range(4)]
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.mtg_half_plane_feasibility_batch_f64(self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(),
+                                                           P, arr, *(o.data_ptr() for o in out), s)
+        self._check(rc, "mtg_half_plane_feasibility_batch_f64")
+        return tuple(out)
+
     def coeffs_from_constraints(self, prob, seg_times, d_fixed, d_free, coeffs=None, stream=None):
         import torch
         B = seg_times.shape[0]
@@ -594,3 +675,15 @@ class Solver:
                                                            self._hptr(segment), self._hptr(status))
         self._check(rc, "mtg_input_feasibility_batch_host_f64")
         return result
+
+    def check_half_plane_feasibility_host(self, seg_times, coeffs, planes, feasible, segment=None, plane=None,
+                                          status=None):
+        """check_half_plane_feasibility into host buffers: feasible [B]; segment, plane, status [B] or None (int32)."""
+        B, K, D, N = coeffs.shape
+        arr, P = half_plane_array(planes)
+        rc = self.lib.mtg_half_plane_feasibility_batch_host_f64(self.h, N, K, D, B, self._hptr(seg_times),
+                                                                self._hptr(coeffs), P, arr, self._hptr(feasible),
+                                                                self._hptr(segment), self._hptr(plane),
+                                                                self._hptr(status))
+        self._check(rc, "mtg_half_plane_feasibility_batch_host_f64")
+        return feasible

@@ -16,6 +16,7 @@
 #include "mtg_extrema_kernel.cuh"
 #include "mtg_feasibility_kernel.cuh"
 #include "mtg_generic_kernel.cuh"
+#include "mtg_half_plane_kernel.cuh"
 #include "mtg_twisted_kernel.cuh"
 #include "mtg_twisted_tmem_kernel.cuh"
 #include "mtg_twisted_tmem_v4_kernel.cuh"
@@ -1770,6 +1771,73 @@ int mtg_input_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t
   });
 }
 
+// checkHalfPlaneFeasibility: N even in [2, 12]; 0 <= n_planes <= MTG_MAX_HALF_PLANES, the planes (a host array)
+// finite with a non-zero normal.  Any D: rows with D not 3 or 4 are infeasible, as in the reference.
+static bool valid_half_plane(int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                             const double* coeffs, int32_t n_planes, const mtg_half_plane* planes,
+                             const int32_t* feasible) {
+  if (N < 2 || N > MTG_MAX_N || (N & 1) || K < 1 || D < 1) return false;
+  if (n_planes < 0 || n_planes > MTG_MAX_HALF_PLANES || (n_planes > 0 && !planes)) return false;
+  for (int p = 0; p < n_planes; ++p) {
+    bool zero = true;
+    for (int d = 0; d < 3; ++d) {
+      if (!std::isfinite(planes[p].point[d]) || !std::isfinite(planes[p].normal[d])) return false;
+      if (planes[p].normal[d] != 0.0) zero = false;
+    }
+    if (zero) return false;
+  }
+  return valid_rows(B, {seg_times, coeffs, feasible});
+}
+
+static int launch_half_plane(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                             const double* coeffs, int32_t n_planes, const mtg_half_plane* planes, int32_t* feasible,
+                             int32_t* segment, int32_t* plane, int32_t* status, cudaStream_t s) {
+  static_assert(mtg::kHalfPlaneMax == MTG_MAX_HALF_PLANES, "plane table size");
+  mtg::HalfPlaneParams hp;  // the planes travel by value in the kernel parameters
+  hp.K = K;
+  hp.D = D;
+  hp.n_planes = n_planes;
+  hp.B = B;
+  hp.times = seg_times;
+  hp.coeffs = coeffs;
+  hp.feasible = feasible;
+  hp.segment = segment;
+  hp.plane = plane;
+  hp.status = status;
+  for (int p = 0; p < mtg::kHalfPlaneMax; ++p)
+    for (int d = 0; d < 3; ++d) {
+      hp.planes[p][d] = p < n_planes ? planes[p].point[d] : 0.0;
+      hp.planes[p][3 + d] = p < n_planes ? planes[p].normal[d] : 0.0;
+    }
+  const int tpb = std::max(1, mtg::kExtremaThreads / K);
+  const size_t smem = size_t(tpb) * K * sizeof(int);
+  if (smem > h->smem_optin) {
+    h->error = "mtg_half_plane_feasibility_batch_f64: K too large";
+    return MTG_ERR_BAD_ARG;
+  }
+  typedef void (*HalfPlaneFn)(const mtg::HalfPlaneParams, const int);
+  static const HalfPlaneFn kHalfPlane[MTG_MAX_N / 2] = {mtg::half_plane_kernel<2>,  mtg::half_plane_kernel<4>,
+                                                        mtg::half_plane_kernel<6>,  mtg::half_plane_kernel<8>,
+                                                        mtg::half_plane_kernel<10>, mtg::half_plane_kernel<12>};
+  const HalfPlaneFn fn = kHalfPlane[N / 2 - 1];
+  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
+  const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
+  fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(hp, tpb);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  return MTG_OK;
+}
+
+int mtg_half_plane_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                         const double* seg_times, const double* coeffs, int32_t n_planes,
+                                         const mtg_half_plane* planes, int32_t* feasible, int32_t* segment,
+                                         int32_t* plane, int32_t* status, void* stream) {
+  return run_entry(h, valid_half_plane(N, K, D, B, seg_times, coeffs, n_planes, planes, feasible), B, [&] {
+    return launch_half_plane(h, N, K, D, B, seg_times, coeffs, n_planes, planes, feasible, segment, plane, status,
+                             (cudaStream_t)stream);
+  });
+}
+
 // ---- host-pointer entry points: the device entry's check and launcher, around stage_host() ------------------------
 
 static int solve_host(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times, const double* d_fixed,
@@ -1938,6 +2006,23 @@ int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, in
                             {nullptr, status, 4}};
     return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
       return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s);
+    });
+  });
+}
+
+int mtg_half_plane_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                              const double* seg_times, const double* coeffs, int32_t n_planes,
+                                              const mtg_half_plane* planes, int32_t* feasible, int32_t* segment,
+                                              int32_t* plane, int32_t* status) {
+  return run_entry(h, valid_half_plane(N, K, D, B, seg_times, coeffs, n_planes, planes, feasible), B, [&] {
+    const HostBuf bufs[] = {{seg_times, nullptr, size_t(K) * 8},
+                            {coeffs, nullptr, size_t(K) * D * N * 8},
+                            {nullptr, feasible, 4},
+                            {nullptr, segment, 4},
+                            {nullptr, plane, 4},
+                            {nullptr, status, 4}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
+      return launch_half_plane(h, N, K, D, nb, d[0], d[1], n_planes, planes, d[2], d[3], d[4], d[5], s);
     });
   });
 }

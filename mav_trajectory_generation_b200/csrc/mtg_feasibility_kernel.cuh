@@ -189,51 +189,68 @@ __device__ int feas_segment(const double* __restrict__ c, double T, const FeasPa
   }
 }
 
-// Work item = (trajectory, segment), as max_magnitude_kernel: each segment's code goes to shared memory, then one
-// thread per trajectory takes the first segment that is not Feasible.
+// The tile loop of the feasibility kernels.  Work item = (trajectory, segment), as max_magnitude_kernel: each
+// segment's code goes to shared memory, then one thread per trajectory takes the first segment whose code is not 0.
+// segment_code(item, T) checks one segment with a good time T (item = trajectory * K + segment) and returns 0 when it
+// passes; row(traj, bad, seg, code) writes one trajectory's outputs: bad when some segment time is <= 0 or non-finite
+// (seg = -1, code = 0 then), else the first failing segment and its code, or seg = -1 and code = 0.
 // dynamic shared memory: [tpb * K] codes
-template <int N>
-__global__ void __launch_bounds__(kExtremaThreads, 1) input_feasibility_kernel(const FeasParams prm, const int tpb) {
+template <typename SegmentCode, typename Row>
+__device__ __forceinline__ void first_failing_segment(long long B, int K, const double* __restrict__ times, int tpb,
+                                                      SegmentCode&& segment_code, Row&& row) {
   extern __shared__ int feas_sm[];
-  const int K = prm.K, D = prm.D;
-  for (long long t0 = (long long)blockIdx.x * tpb; t0 < prm.B; t0 += (long long)gridDim.x * tpb) {
-    const int ntraj = int(prm.B - t0 < tpb ? prm.B - t0 : tpb);
+  for (long long t0 = (long long)blockIdx.x * tpb; t0 < B; t0 += (long long)gridDim.x * tpb) {
+    const int ntraj = int(B - t0 < tpb ? B - t0 : tpb);
     const int items = ntraj * K;
     for (int it = threadIdx.x; it < items; it += blockDim.x) {
       const long long item = t0 * K + it;
-      const double T = prm.times[item];
+      const double T = times[item];
       const bool bad = !(T > 0.0) || !isfinite(T);
-      feas_sm[it] = bad ? kFeasIndeterminable : feas_segment<N>(prm.coeffs + item * D * N, T, prm);
+      feas_sm[it] = bad ? 0 : segment_code(item, T);
     }
     __syncthreads();
     for (int lt = threadIdx.x; lt < ntraj; lt += blockDim.x) {
       const long long traj = t0 + lt;
       bool bad = false;
       for (int i = 0; i < K; ++i) {
-        const double T = prm.times[traj * K + i];
+        const double T = times[traj * K + i];
         if (!(T > 0.0) || !isfinite(T)) bad = true;
       }
-      int res = kFeasFeasible, seg = -1, st = 0;
-      if (bad) {
-        res = kFeasIndeterminable;
-        st = 1;  // MTG_STATUS_BAD_TIME
-      } else {
+      int seg = -1, code = 0;
+      if (!bad) {
         for (int i = 0; i < K; ++i) {
-          const int code = feas_sm[lt * K + i];
-          if ((code & 0xff) != kFeasFeasible) {
-            res = code & 0xff;
+          const int c = feas_sm[lt * K + i];
+          if (c != 0) {
             seg = i;
-            if (code & kFeasCapacity) st = 4;  // MTG_STATUS_FEAS_CAPACITY
+            code = c;
             break;
           }
         }
       }
-      prm.result[traj] = res;
-      if (prm.segment) prm.segment[traj] = seg;
-      if (prm.status) prm.status[traj] = st;
+      row(traj, bad, seg, code);
     }
     __syncthreads();
   }
+}
+
+// One thread per (trajectory, segment) runs feas_segment; the first segment that is not Feasible decides.
+template <int N>
+__global__ void __launch_bounds__(kExtremaThreads, 1) input_feasibility_kernel(const FeasParams prm, const int tpb) {
+  first_failing_segment(
+      prm.B, prm.K, prm.times, tpb,
+      [&](long long item, double T) { return feas_segment<N>(prm.coeffs + item * prm.D * N, T, prm); },
+      [&](long long traj, bool bad, int seg, int code) {
+        int res = code & 0xff, st = 0;
+        if (bad) {
+          res = kFeasIndeterminable;
+          st = 1;  // MTG_STATUS_BAD_TIME
+        } else if (code & kFeasCapacity) {
+          st = 4;  // MTG_STATUS_FEAS_CAPACITY
+        }
+        prm.result[traj] = res;
+        if (prm.segment) prm.segment[traj] = seg;
+        if (prm.status) prm.status[traj] = st;
+      });
 }
 
 }  // namespace mtg

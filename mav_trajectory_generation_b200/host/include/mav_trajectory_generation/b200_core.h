@@ -125,6 +125,10 @@ class BatchCore {
   // nullable, -1 where the row is feasible or has a bad segment time)
   bool checkInputFeasibility(const InputConstraints& constraints, double min_section_time, double gravity,
                              std::vector<InputFeasibilityResult>* result, std::vector<int>* segment) const;
+  // FeasibilityBase::checkHalfPlaneFeasibility of the current coefficients (feasible, segment, plane: [B]; segment and
+  // plane nullable, -1 where the row is feasible or has a bad segment time)
+  bool checkHalfPlaneFeasibility(const HalfPlane::Vector& planes, std::vector<uint8_t>* feasible,
+                                 std::vector<int>* segment, std::vector<int>* plane) const;
   void getSegments(size_t b, Segment::Vector* segments) const;
 
   int N_;

@@ -114,6 +114,14 @@ class BatchPolynomialOptimization {
                              double gravity = kGravity) const {
     return core_.checkInputFeasibility(constraints, min_section_time, gravity, result, segment);
   }
+  // FeasibilityBase::checkHalfPlaneFeasibility (reference mav_trajectory_generation_ros/src/feasibility_base.cpp) of
+  // every trajectory at its current coefficients against one set of at most MTG_MAX_HALF_PLANES planes, on the GPU:
+  // feasible[b] (1 or 0), and segment[b], plane[b] = the first failing pair (-1 when the row is feasible or has a
+  // segment time <= 0 or non-finite; such a row is infeasible).  Candidates are exact real roots, not Jenkins-Traub's.
+  bool checkHalfPlaneFeasibility(const HalfPlane::Vector& planes, std::vector<uint8_t>* feasible,
+                                 std::vector<int>* segment = nullptr, std::vector<int>* plane = nullptr) const {
+    return core_.checkHalfPlaneFeasibility(planes, feasible, segment, plane);
+  }
 
  private:
   b200::BatchCore core_;

@@ -113,6 +113,34 @@ class Matrix {
     return s;
   }
   Scalar norm() const { return std::sqrt(squaredNorm()); }
+  // Eigen's dot, cross, normalize and normalized: sums in index order, cross products as (y z' - z y', ...), and
+  // normalisation by one division by sqrt(squaredNorm()) (a zero vector is left as it is)
+  template <int R2, int C2>
+  Scalar dot(const Matrix<Scalar, R2, C2>& o) const {
+    Scalar s = size() > 0 ? data_[0] * o.data()[0] : Scalar(0);
+    for (Index i = 1; i < size(); ++i) s += data_[size_t(i)] * o.data()[i];
+    return s;
+  }
+  template <int R2, int C2>
+  Matrix cross(const Matrix<Scalar, R2, C2>& o) const {
+    Matrix r(*this);
+    r[0] = data_[1] * o[2] - data_[2] * o[1];
+    r[1] = data_[2] * o[0] - data_[0] * o[2];
+    r[2] = data_[0] * o[1] - data_[1] * o[0];
+    return r;
+  }
+  void normalize() {
+    const Scalar z = squaredNorm();
+    if (z > Scalar(0)) {
+      const Scalar n = std::sqrt(z);
+      for (auto& v : data_) v /= n;
+    }
+  }
+  Matrix normalized() const {
+    Matrix r(*this);
+    r.normalize();
+    return r;
+  }
   Scalar sum() const {
     Scalar s(0);
     for (const auto& v : data_) s += v;

@@ -1,10 +1,11 @@
 // feasibility_base.h -- input feasibility results and the trajectory-level check (reference
-// mav_trajectory_generation_ros/include/mav_trajectory_generation_ros/feasibility_base.h, src/feasibility_base.cpp).
-// Half-plane feasibility is not mirrored.
+// mav_trajectory_generation_ros/include/mav_trajectory_generation_ros/feasibility_base.h, src/feasibility_base.cpp),
+// and the half-plane (workspace) check of single segments and trajectories.
 #ifndef MAV_TRAJECTORY_GENERATION_ROS_FEASIBILITY_BASE_H_
 #define MAV_TRAJECTORY_GENERATION_ROS_FEASIBILITY_BASE_H_
 
 #include <string>
+#include <vector>
 
 #include "mav_trajectory_generation/trajectory.h"
 #include "mav_trajectory_generation_ros/input_constraints.h"
@@ -25,6 +26,22 @@ enum InputFeasibilityResult {
 
 std::string getInputFeasibilityResultName(InputFeasibilityResult fr);
 
+// A half-space {x : (x - point) . normal > 0}.  The normal is normalised on construction, as in the reference.
+class HalfPlane {
+ public:
+  typedef std::vector<HalfPlane, Eigen::aligned_allocator<HalfPlane>> Vector;
+  // point on the plane and a normal pointing into the allowed side (CHECKs that the normal is not zero)
+  HalfPlane(const Eigen::Vector3d& point, const Eigen::Vector3d& normal);
+  // the plane through a, b and c, normal (b - a) x (c - a) (CHECKs b != a and c != a)
+  HalfPlane(const Eigen::Vector3d& a, const Eigen::Vector3d& b, const Eigen::Vector3d& c);
+  // six planes bounding the axis-aligned box of the given size around point: for each axis, the lower face (normal
+  // +e_axis) and then the upper face (normal -e_axis)
+  static HalfPlane::Vector createBoundingBox(const Eigen::Vector3d& point, const Eigen::Vector3d& bounding_box_size);
+
+  Eigen::Vector3d point;
+  Eigen::Vector3d normal;
+};
+
 class FeasibilityBase {
  public:
   FeasibilityBase() : gravity_(0.0, 0.0, kGravity) {}
@@ -41,7 +58,15 @@ class FeasibilityBase {
   }
   InputConstraints getInputConstraints() const { return input_constraints_; }
 
+  // true when every segment passes checkHalfPlaneFeasibility(segment)
+  bool checkHalfPlaneFeasibility(const Trajectory& trajectory) const;
+  // true when the segment's position stays strictly inside every half-space of half_plane_constraints_ at the extremum
+  // candidates of its projection on each normal (0, T and the real critical points in [0, T]); false for D not 3 or 4.
+  // Runs on the host; batches go through BatchPolynomialOptimization<N>::checkHalfPlaneFeasibility on the GPU.
+  bool checkHalfPlaneFeasibility(const Segment& segment) const;
+
   InputConstraints input_constraints_;
+  HalfPlane::Vector half_plane_constraints_;
   Eigen::Vector3d gravity_;
 };
 

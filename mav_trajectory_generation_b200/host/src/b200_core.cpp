@@ -666,6 +666,32 @@ bool BatchCore::checkInputFeasibility(const InputConstraints& constraints, doubl
   return true;
 }
 
+bool BatchCore::checkHalfPlaneFeasibility(const HalfPlane::Vector& planes, std::vector<uint8_t>* feasible,
+                                          std::vector<int>* segment, std::vector<int>* plane) const {
+  CHECK_GT(B_, 0u) << "setup first";
+  CHECK_NOTNULL(feasible);
+  std::vector<mtg_half_plane> table(planes.size());
+  for (size_t p = 0; p < planes.size(); ++p)
+    for (int d = 0; d < 3; ++d) {
+      table[p].point[d] = planes[p].point[d];
+      table[p].normal[d] = planes[p].normal[d];
+    }
+  std::vector<int32_t> ok(B_, 0), seg(B_, -1), pl(B_, -1);
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_half_plane_feasibility_batch_host_f64(h, N_, topo_.K, topo_.D, static_cast<int64_t>(B_), times_,
+                                                           coeffs_, static_cast<int32_t>(table.size()), table.data(),
+                                                           ok.data(), seg.data(), pl.data(), nullptr);
+  if (rc != MTG_OK) {
+    LOG(ERROR) << "mtg_half_plane_feasibility_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+    return false;
+  }
+  feasible->assign(ok.begin(), ok.end());
+  if (segment) segment->assign(seg.begin(), seg.end());
+  if (plane) plane->assign(pl.begin(), pl.end());
+  return true;
+}
+
 void BatchCore::getSegments(size_t b, Segment::Vector* segments) const {
   CHECK_LT(b, B_);
   unpackSegments(topo_, coeffs_ + b * size_t(topo_.K) * topo_.D * N_, times_ + b * topo_.K, segments);

@@ -81,6 +81,55 @@ InputFeasibilityResult FeasibilityBase::checkInputFeasibilityTrajectory(const Tr
   return result;
 }
 
+HalfPlane::HalfPlane(const Eigen::Vector3d& point, const Eigen::Vector3d& normal) : point(point), normal(normal) {
+  CHECK_GT(normal.norm(), 0.0) << "Invalid normal.";
+  this->normal.normalize();
+}
+
+HalfPlane::HalfPlane(const Eigen::Vector3d& a, const Eigen::Vector3d& b, const Eigen::Vector3d& c) {
+  CHECK(a != b);
+  CHECK(a != c);
+  point = a;
+  normal = (b - a).cross(c - a).normalized();
+}
+
+HalfPlane::Vector HalfPlane::createBoundingBox(const Eigen::Vector3d& point, const Eigen::Vector3d& bounding_box_size) {
+  const Eigen::Vector3d lower = point - bounding_box_size / 2.0, upper = point + bounding_box_size / 2.0;
+  HalfPlane::Vector box;
+  for (int axis = 0; axis < 3; ++axis) {
+    Eigen::Vector3d inward(0.0, 0.0, 0.0);
+    inward[axis] = 1.0;
+    box.emplace_back(lower, inward);
+    box.emplace_back(upper, -inward);
+  }
+  return box;
+}
+
+bool FeasibilityBase::checkHalfPlaneFeasibility(const Trajectory& trajectory) const {
+  for (const Segment& segment : trajectory.segments())
+    if (!checkHalfPlaneFeasibility(segment)) return false;
+  return true;
+}
+
+bool FeasibilityBase::checkHalfPlaneFeasibility(const Segment& segment) const {
+  if (segment.D() != 3 && segment.D() != 4) {
+    LOG(WARNING) << "Half-plane feasibility needs D = 3 or 4, got " << segment.D() << ".";
+    return false;
+  }
+  for (const HalfPlane& hp : half_plane_constraints_) {
+    // the position projected on the normal; its extrema are where the segment comes closest to the plane
+    Polynomial projection(segment.N());
+    for (int d = 0; d < 3; ++d) projection += segment[d] * hp.normal[d];
+    std::vector<double> times;
+    projection.computeMinMaxCandidates(0.0, segment.getTime(), derivative_order::POSITION, &times);
+    for (const double t : times) {
+      const Eigen::VectorXd p = segment.evaluate(t).head(3);
+      if ((p - Eigen::VectorXd(hp.point)).dot(hp.normal) <= 0.0) return false;
+    }
+  }
+  return true;
+}
+
 InputFeasibilityResult FeasibilityAnalytic::checkInputFeasibility(const Segment& segment) const {
   if (segment.D() != 3 && segment.D() != 4) return kInputIndeterminable;
   const InputConstraints& ic = input_constraints_;
