@@ -303,11 +303,38 @@ typedef struct mtg_input_constraints {
   double omega_z_max;      /* yaw rate [rad/s] */
   double omega_z_dot_max;  /* yaw acceleration [rad/s^2] */
   double gravity;          /* added to the z acceleration for the thrust (mav_msgs::kGravity in the reference) */
-  double min_section_time; /* FeasibilityAnalytic::Settings, reference default 0.05 s */
+  double min_section_time; /* FeasibilityAnalytic / FeasibilityRecursive::Settings, reference default 0.05 s */
 } mtg_input_constraints;
 int mtg_input_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                                     const double* coeffs, const mtg_input_constraints* constraints, int32_t* result,
                                     int32_t* segment, int32_t* status, void* stream);
+
+/* FeasibilityRecursive::checkInputFeasibility per segment and checkInputFeasibilityTrajectory per trajectory
+ * (reference mav_trajectory_generation_ros/src/feasibility_recursive.cpp).  Same arguments, outputs, refusals, bad-time
+ * rule and D rule as mtg_input_feasibility_batch_f64; min_section_time is FeasibilityRecursive::Settings'.  Per segment:
+ * the recursion over [0, T], then (D = 4, only when it gives Feasible) yaw rate and yaw acceleration over the whole
+ * segment.  Per section [t1, t2], depth first and left half first:
+ *   t2 - t1 < min_section_time: Indeterminable (also with no limit present, so a segment shorter than
+ *   min_section_time is always Indeterminable, unlike the analytic check);
+ *   thrust |p'' + (0, 0, g)| at t1 and t2 against f_min (ThrustLow) and f_max (ThrustHigh); speed |p'| over dims 0..2
+ *   at t1 and t2 (Velocity);
+ *   per axis, from t1, t2 and the roots in [t1, t2]: a single-axis speed above v_max (Velocity), a single-axis thrust
+ *   above f_max (ThrustHigh), and upper / lower bounds on speed, thrust and jerk summed over the axes;
+ *   thrust upper bound < f_min: ThrustLow; lower bound > f_max: ThrustHigh;
+ *   a bound beyond its limit (or the roll/pitch bound sqrt(j_max^2 / f_min^2), DBL_MAX when f_min^2 <= 1e-6, above
+ *   omega_xy_max) halves the section; otherwise the section is Feasible.
+ * Reachable results: Feasible, Indeterminable, ThrustLow, ThrustHigh, Velocity, YawRates, YawAcc; never
+ * MTG_FEAS_ROLL_PITCH_RATES.  The roots are the exact real roots of p_i'', p_i''' and p_i'''' in [0, T] (the
+ * reference's Jenkins-Traub roots with their |imag| > eps filter are not reproduced, and root finding never fails
+ * here); every value uses the reference's arithmetic (Polynomial::evaluate, then g added to z; std::pow(x, 2) as
+ * x * x, which is what an optimised x86 build of the reference computes).
+ *   status MTG_STATUS_FEAS_CAPACITY (result Indeterminable): the roots of one axis and order k (k = 1, 2, 3) needed
+ *   more than N - 2 - k + 2 entries (only clusters of roots unresolved at 2^-24 T add entries), or the bisection went
+ *   64 levels deep (a section with f_min^2 <= 1e-6 at a min_section_time below T / 2^64). */
+int mtg_input_feasibility_recursive_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                              const double* seg_times, const double* coeffs,
+                                              const mtg_input_constraints* constraints, int32_t* result,
+                                              int32_t* segment, int32_t* status, void* stream);
 
 /* FeasibilityBase::checkHalfPlaneFeasibility per segment and per trajectory (reference
  * mav_trajectory_generation_ros/src/feasibility_base.cpp:109-154): a segment passes plane (point q, normal n) when
@@ -382,6 +409,10 @@ int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, in
                                          const double* seg_times, const double* coeffs,
                                          const mtg_input_constraints* constraints, int32_t* result, int32_t* segment,
                                          int32_t* status);
+int mtg_input_feasibility_recursive_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                                   const double* seg_times, const double* coeffs,
+                                                   const mtg_input_constraints* constraints, int32_t* result,
+                                                   int32_t* segment, int32_t* status);
 int mtg_half_plane_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
                                               const double* seg_times, const double* coeffs, int32_t n_planes,
                                               const mtg_half_plane* planes, int32_t* feasible, int32_t* segment,

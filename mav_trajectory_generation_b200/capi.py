@@ -39,7 +39,8 @@ EXPORTED_SYMBOLS = [
     "mtg_scale_times_with_violation_batch_f64", "mtg_scale_to_constraints_batch_host_f64",
     "mtg_scale_times_with_violation_batch_host_f64", "mtg_input_feasibility_batch_f64",
     "mtg_input_feasibility_batch_host_f64", "mtg_half_plane_feasibility_batch_f64",
-    "mtg_half_plane_feasibility_batch_host_f64",
+    "mtg_half_plane_feasibility_batch_host_f64", "mtg_input_feasibility_recursive_batch_f64",
+    "mtg_input_feasibility_recursive_batch_host_f64",
 ]
 TIME_COST_SQUARED, TIME_COST_RICHTER = 0, 1
 STATUS_FEAS_CAPACITY = 4
@@ -253,6 +254,8 @@ def load():
                                                   C.POINTER(MtgInputConstraints), dp, dp, dp, vp]
     L.mtg_input_feasibility_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
                                                        C.POINTER(MtgInputConstraints), dp, dp, dp]
+    L.mtg_input_feasibility_recursive_batch_f64.argtypes = L.mtg_input_feasibility_batch_f64.argtypes
+    L.mtg_input_feasibility_recursive_batch_host_f64.argtypes = L.mtg_input_feasibility_batch_host_f64.argtypes
     L.mtg_half_plane_feasibility_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, C.c_int32,
                                                        C.POINTER(MtgHalfPlane), dp, dp, dp, dp, vp]
     L.mtg_half_plane_feasibility_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
@@ -511,6 +514,17 @@ class Solver:
         """Batched FeasibilityAnalytic::checkInputFeasibilityTrajectory: (result [B], segment [B], status [B]), int32.
         limits: {name: value} over INPUT_LIMITS (absent name = no limit; default_input_limits() gives the reference's
         defaults) or an MtgInputConstraints."""
+        return self._input_feasibility("mtg_input_feasibility_batch_f64", seg_times, coeffs, limits, min_section_time,
+                                       gravity, stream)
+
+    def check_input_feasibility_recursive(self, seg_times, coeffs, limits, min_section_time=0.05, gravity=GRAVITY,
+                                          stream=None):
+        """Batched FeasibilityRecursive::checkInputFeasibilityTrajectory: (result [B], segment [B], status [B]), int32,
+        with the arguments of check_input_feasibility."""
+        return self._input_feasibility("mtg_input_feasibility_recursive_batch_f64", seg_times, coeffs, limits,
+                                       min_section_time, gravity, stream)
+
+    def _input_feasibility(self, entry, seg_times, coeffs, limits, min_section_time, gravity, stream):
         import torch
         B, K, D, N = coeffs.shape
         dev = coeffs.device
@@ -519,10 +533,9 @@ class Solver:
         segment = torch.empty((B,), dtype=torch.int32, device=dev)
         status = torch.empty((B,), dtype=torch.int32, device=dev)
         s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
-        rc = self.lib.mtg_input_feasibility_batch_f64(self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(),
-                                                      C.byref(ic), result.data_ptr(), segment.data_ptr(),
-                                                      status.data_ptr(), s)
-        self._check(rc, "mtg_input_feasibility_batch_f64")
+        rc = getattr(self.lib, entry)(self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(), C.byref(ic),
+                                      result.data_ptr(), segment.data_ptr(), status.data_ptr(), s)
+        self._check(rc, entry)
         return result, segment, status
 
     def check_half_plane_feasibility(self, seg_times, coeffs, planes, stream=None):
@@ -668,12 +681,23 @@ class Solver:
     def check_input_feasibility_host(self, seg_times, coeffs, limits, result, segment=None, status=None,
                                      min_section_time=0.05, gravity=GRAVITY):
         """check_input_feasibility into host buffers: result [B], segment [B] or None, status [B] or None (int32)."""
+        return self._input_feasibility_host("mtg_input_feasibility_batch_host_f64", seg_times, coeffs, limits, result,
+                                            segment, status, min_section_time, gravity)
+
+    def check_input_feasibility_recursive_host(self, seg_times, coeffs, limits, result, segment=None, status=None,
+                                               min_section_time=0.05, gravity=GRAVITY):
+        """check_input_feasibility_recursive into host buffers: result [B], segment [B] or None, status [B] or None
+        (int32)."""
+        return self._input_feasibility_host("mtg_input_feasibility_recursive_batch_host_f64", seg_times, coeffs,
+                                            limits, result, segment, status, min_section_time, gravity)
+
+    def _input_feasibility_host(self, entry, seg_times, coeffs, limits, result, segment, status, min_section_time,
+                                gravity):
         B, K, D, N = coeffs.shape
         ic = limits if isinstance(limits, MtgInputConstraints) else input_constraints(limits, min_section_time, gravity)
-        rc = self.lib.mtg_input_feasibility_batch_host_f64(self.h, N, K, D, B, self._hptr(seg_times),
-                                                           self._hptr(coeffs), C.byref(ic), self._hptr(result),
-                                                           self._hptr(segment), self._hptr(status))
-        self._check(rc, "mtg_input_feasibility_batch_host_f64")
+        rc = getattr(self.lib, entry)(self.h, N, K, D, B, self._hptr(seg_times), self._hptr(coeffs), C.byref(ic),
+                                      self._hptr(result), self._hptr(segment), self._hptr(status))
+        self._check(rc, entry)
         return result
 
     def check_half_plane_feasibility_host(self, seg_times, coeffs, planes, feasible, segment=None, plane=None,

@@ -1722,9 +1722,10 @@ static bool valid_feasibility(int32_t N, int32_t K, int32_t D, int64_t B, const 
   return valid_rows(B, {seg_times, coeffs, result});
 }
 
+// recursive: FeasibilityRecursive (input_feasibility_recursive_kernel), else FeasibilityAnalytic
 static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                                     const double* coeffs, const mtg_input_constraints* ic, int32_t* result,
-                                    int32_t* segment, int32_t* status, cudaStream_t s) {
+                                    int32_t* segment, int32_t* status, cudaStream_t s, bool recursive = false) {
   mtg::FeasParams fp;
   fp.K = K;
   fp.D = D;
@@ -1746,14 +1747,19 @@ static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t
   const int tpb = std::max(1, mtg::kExtremaThreads / K);
   const size_t smem = size_t(tpb) * K * sizeof(int);
   if (smem > h->smem_optin) {
-    h->error = "mtg_input_feasibility_batch_f64: K too large";
+    h->error = recursive ? "mtg_input_feasibility_recursive_batch_f64: K too large"
+                         : "mtg_input_feasibility_batch_f64: K too large";
     return MTG_ERR_BAD_ARG;
   }
   typedef void (*FeasFn)(const mtg::FeasParams, const int);
   static const FeasFn kFeas[MTG_MAX_N / 2 - 1] = {
       mtg::input_feasibility_kernel<4>, mtg::input_feasibility_kernel<6>, mtg::input_feasibility_kernel<8>,
       mtg::input_feasibility_kernel<10>, mtg::input_feasibility_kernel<12>};
-  const FeasFn fn = kFeas[N / 2 - 2];
+  static const FeasFn kFeasRec[MTG_MAX_N / 2 - 1] = {
+      mtg::input_feasibility_recursive_kernel<4>, mtg::input_feasibility_recursive_kernel<6>,
+      mtg::input_feasibility_recursive_kernel<8>, mtg::input_feasibility_recursive_kernel<10>,
+      mtg::input_feasibility_recursive_kernel<12>};
+  const FeasFn fn = (recursive ? kFeasRec : kFeas)[N / 2 - 2];
   MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
   const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
   fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(fp, tpb);
@@ -1768,6 +1774,17 @@ int mtg_input_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t
   return run_entry(h, valid_feasibility(N, K, D, B, seg_times, coeffs, constraints, result), B, [&] {
     return launch_input_feasibility(h, N, K, D, B, seg_times, coeffs, constraints, result, segment, status,
                                     (cudaStream_t)stream);
+  });
+}
+
+// FeasibilityRecursive: the same arguments, refused by the same check
+int mtg_input_feasibility_recursive_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                              const double* seg_times, const double* coeffs,
+                                              const mtg_input_constraints* constraints, int32_t* result,
+                                              int32_t* segment, int32_t* status, void* stream) {
+  return run_entry(h, valid_feasibility(N, K, D, B, seg_times, coeffs, constraints, result), B, [&] {
+    return launch_input_feasibility(h, N, K, D, B, seg_times, coeffs, constraints, result, segment, status,
+                                    (cudaStream_t)stream, true);
   });
 }
 
@@ -2006,6 +2023,22 @@ int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, in
                             {nullptr, status, 4}};
     return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
       return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s);
+    });
+  });
+}
+
+int mtg_input_feasibility_recursive_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                                   const double* seg_times, const double* coeffs,
+                                                   const mtg_input_constraints* constraints, int32_t* result,
+                                                   int32_t* segment, int32_t* status) {
+  return run_entry(h, valid_feasibility(N, K, D, B, seg_times, coeffs, constraints, result), B, [&] {
+    const HostBuf bufs[] = {{seg_times, nullptr, size_t(K) * 8},
+                            {coeffs, nullptr, size_t(K) * D * N * 8},
+                            {nullptr, result, 4},
+                            {nullptr, segment, 4},
+                            {nullptr, status, 4}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
+      return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s, true);
     });
   });
 }

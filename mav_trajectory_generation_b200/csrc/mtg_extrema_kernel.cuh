@@ -18,6 +18,8 @@
 // one would be a wrong answer.
 #pragma once
 
+#include <cfloat>
+
 #include "mtg_generic_kernel.cuh"
 
 namespace mtg {
@@ -110,13 +112,28 @@ __device__ double extrema_refine(const double (&g)[M], double lo, double hi) {
 // true for a refined root and for the midpoint of an interval still unresolved at the depth cap or node budget, false
 // for the extra safety samples (halving points, the ends of an unresolved interval): a whole-segment extremum may use
 // every candidate, a check confined to a sub-interval only the first kind (the reference's candidate set).
-template <int M, typename Visit>
+// kZeroHalvingRoots: a halving point where g is 0 to within the rounding of its evaluation is also flagged as a root.
+// A root on a halving point (a symmetric polynomial's, at 1/2) shows its sign change in neither half, since each half
+// rounds g there on its own, so it would otherwise be only a safety sample.
+template <int M, bool kZeroHalvingRoots = false, typename Visit>
 __device__ void extrema_candidates(const double (&g)[M], Visit&& visit) {
   int level = 0, nodes = 0;
   unsigned idx = 0;
   while (true) {
     const double h = ldexp(1.0, -level), a = double(idx) * h;
-    if (idx & 1u) visit(a, false);  // a halving point
+    if (idx & 1u) {  // a halving point
+      bool root = false;
+      if (kZeroHalvingRoots) {
+        double v = g[M - 1], s = fabs(g[M - 1]);
+#pragma unroll
+        for (int j = M - 2; j >= 0; --j) {
+          v = fma(v, a, g[j]);
+          s = fma(s, a, fabs(g[j]));
+        }
+        root = fabs(v) <= 4.0 * M * DBL_EPSILON * s;
+      }
+      visit(a, root);
+    }
     double b[M];
     extrema_bernstein(g, a, h, b);
     ++nodes;
@@ -171,7 +188,8 @@ __device__ __forceinline__ double extrema_magnitude(const double* __restrict__ c
 
 // The critical polynomial of |p^(k)| on one segment (coefficients c [D][N], time T), in tau = t / T over [0, 1]:
 // G(tau) = sum_d A_d(tau) A_d'(tau), A_d(tau) = p_d^(k)(tau T) (D = 1: A'(tau)); nominal degree 2N - 3.  lift is
-// added to the constant term of p_2^(k) first (gravity on z: the thrust polynomial of the feasibility check).
+// added to the constant term of p_2^(k) first (gravity on z: the thrust polynomial of the feasibility check).  A D = 1
+// caller may pass M = N - 1 (the degree of A') to keep its root isolation at that degree.
 template <int N, int M = (N >= 2 ? 2 * N - 2 : 1)>
 __device__ __forceinline__ void extrema_critical(const double* __restrict__ c, double T, int D, int k, double lift,
                                                  double (&g)[M]) {
@@ -196,7 +214,7 @@ __device__ __forceinline__ void extrema_critical(const double* __restrict__ c, d
     if (D == 1) {
 #pragma unroll
       for (int j = 0; j < N - 1; ++j) g[j] = double(j + 1) * a[j + 1];
-    } else {
+    } else if constexpr (M >= 2 * N - 2) {
 #pragma unroll
       for (int i = 0; i < N; ++i)
 #pragma unroll

@@ -81,6 +81,44 @@ __device__ __forceinline__ double feas_thrust(const double* __restrict__ c, doub
   return sqrt(sq);
 }
 
+constexpr int kFeasSplit = -1;  // a walk node's "halve this section"
+
+// The reference's recursive bisection of [0, T] (recursiveRollPitchFeasibility / recursiveFeasibility), depth first,
+// left half first, without a stack: the current node is a level and a path of left/right bits (bit l is 1 when the
+// node at level l + 1 is the right half of its parent), and its bounds are recomputed from [0, T] with the reference's
+// (t1 + t2) / 2.  A section shorter than min_section_time is Indeterminable; otherwise node(t1, t2) returns kFeasSplit
+// or the section's FeasResult.  A split node's result is its left half's when that is not Feasible, else its right
+// half's, so the first leaf that is not Feasible decides.  Splitting below level kFeasMaxLevel gives Indeterminable |
+// kFeasCapacity.
+template <typename Node>
+__device__ __forceinline__ int feas_walk(double T, double min_section_time, Node&& node) {
+  unsigned long long path = 0;
+  int level = 0;
+  while (true) {
+    double t1 = 0.0, t2 = T;
+    for (int l = 0; l < level; ++l) {
+      const double th = __dmul_rn(__dadd_rn(t1, t2), 0.5);  // (t1 + t2) / 2
+      if ((path >> l) & 1ull) t1 = th;
+      else t2 = th;
+    }
+    if (__dsub_rn(t2, t1) < min_section_time) return kFeasIndeterminable;
+    const int r = node(t1, t2);
+    if (r == kFeasSplit) {
+      if (level == kFeasMaxLevel) return kFeasIndeterminable | kFeasCapacity;
+      ++level;  // the left half (its path bit is 0)
+      continue;
+    }
+    if (r != kFeasFeasible) return r;
+    // this node is feasible: a right half completes its parent
+    while (level > 0 && ((path >> (level - 1)) & 1ull)) {
+      --level;
+      path &= ~(1ull << level);
+    }
+    if (level == 0) return kFeasFeasible;
+    path |= 1ull << (level - 1);  // the right half of the same parent
+  }
+}
+
 // The check of one segment (time T > 0 and finite): a FeasResult, or-ed with kFeasCapacity when a candidate list or
 // the roll/pitch walk ran out of room (the segment is then reported Indeterminable).
 template <int N>
@@ -153,20 +191,9 @@ __device__ int feas_segment(const double* __restrict__ c, double T, const FeasPa
     }
   }
   if (!(pr & kFeasOmegaXY)) return kFeasFeasible;
-  // recursiveRollPitchFeasibility, depth first, left half first.  A node's result is Feasible or Indeterminable, and
-  // the first Indeterminable node decides the segment.  Bit l of `path` is 1 when the node at level l + 1 is the
-  // right half of its parent.
-  const double limit = prm.omega_xy, mst = prm.min_section_time;
-  unsigned long long path = 0;
-  int level = 0;
-  while (true) {
-    double t1 = 0.0, t2 = T;
-    for (int l = 0; l < level; ++l) {
-      const double th = __dmul_rn(__dadd_rn(t1, t2), 0.5);  // (t1 + t2) / 2
-      if ((path >> l) & 1ull) t1 = th;
-      else t2 = th;
-    }
-    if (__dsub_rn(t2, t1) < mst) return kFeasIndeterminable;
+  // recursiveRollPitchFeasibility: a node whose bound sqrt(j_max / f_min) exceeds omega_xy_max is halved
+  const double limit = prm.omega_xy;
+  return feas_walk(T, prm.min_section_time, [&](double t1, double t2) {
     double f_min = DBL_MAX, j_max = -DBL_MAX;  // selectMinMaxMagnitudeFromCandidates: closed interval, no end points
     for (int i = 0; i < n_th; ++i)
       if (!(th_t[i] < t1 || th_t[i] > t2) && th_v[i] < f_min) f_min = th_v[i];
@@ -174,19 +201,8 @@ __device__ int feas_segment(const double* __restrict__ c, double T, const FeasPa
       if (!(jk_t[i] < t1 || jk_t[i] > t2) && j_max < jk_v[i]) j_max = jk_v[i];
     // no jerk candidate: sqrt of a negative number is NaN, and NaN > limit is false
     const double bound = f_min > 1.0e-6 ? __dsqrt_rn(__ddiv_rn(j_max, f_min)) : DBL_MAX;
-    if (bound > limit) {
-      if (level == kFeasMaxLevel) return kFeasIndeterminable | kFeasCapacity;
-      ++level;  // the left half (its path bit is 0)
-      continue;
-    }
-    // this node is feasible: a right half completes its parent
-    while (level > 0 && ((path >> (level - 1)) & 1ull)) {
-      --level;
-      path &= ~(1ull << level);
-    }
-    if (level == 0) return kFeasFeasible;
-    path |= 1ull << (level - 1);  // the right half of the same parent
-  }
+    return bound > limit ? kFeasSplit : int(kFeasFeasible);
+  });
 }
 
 // The tile loop of the feasibility kernels.  Work item = (trajectory, segment), as max_magnitude_kernel: each
@@ -233,24 +249,189 @@ __device__ __forceinline__ void first_failing_segment(long long B, int K, const 
   }
 }
 
+// One trajectory's outputs from first_failing_segment: a bad time gives Indeterminable and MTG_STATUS_BAD_TIME, a
+// segment code with kFeasCapacity gives MTG_STATUS_FEAS_CAPACITY.
+__device__ __forceinline__ void feas_row(const FeasParams& prm, long long traj, bool bad, int seg, int code) {
+  int res = code & 0xff, st = 0;
+  if (bad) {
+    res = kFeasIndeterminable;
+    st = 1;  // MTG_STATUS_BAD_TIME
+  } else if (code & kFeasCapacity) {
+    st = 4;  // MTG_STATUS_FEAS_CAPACITY
+  }
+  prm.result[traj] = res;
+  if (prm.segment) prm.segment[traj] = seg;
+  if (prm.status) prm.status[traj] = st;
+}
+
 // One thread per (trajectory, segment) runs feas_segment; the first segment that is not Feasible decides.
 template <int N>
 __global__ void __launch_bounds__(kExtremaThreads, 1) input_feasibility_kernel(const FeasParams prm, const int tpb) {
   first_failing_segment(
       prm.B, prm.K, prm.times, tpb,
       [&](long long item, double T) { return feas_segment<N>(prm.coeffs + item * prm.D * N, T, prm); },
-      [&](long long traj, bool bad, int seg, int code) {
-        int res = code & 0xff, st = 0;
-        if (bad) {
-          res = kFeasIndeterminable;
-          st = 1;  // MTG_STATUS_BAD_TIME
-        } else if (code & kFeasCapacity) {
-          st = 4;  // MTG_STATUS_FEAS_CAPACITY
+      [&](long long traj, bool bad, int seg, int code) { feas_row(prm, traj, bad, seg, code); });
+}
+
+// ---- FeasibilityRecursive::checkInputFeasibility (reference mav_trajectory_generation_ros/src/
+// feasibility_recursive.cpp:42-304) -----------------------------------------------------------------------------------
+// Per position axis i and order k = 1, 2, 3 (velocity, acceleration, jerk) the roots of p_i^(k+1) in [0, T]: the
+// critical polynomial of extrema_critical with D = 1 at its own degree (M = N - 1), and only the points that
+// extrema_candidates flags as roots, a halving point where the polynomial is 0 to within rounding included (a
+// rest-to-rest segment is symmetric, and its speed peaks exactly at T / 2).  A list holds at most N - 2 - k roots plus kFeasRecSlack midpoints of intervals
+// left unresolved at the isolator's depth cap.  Each root's p_i^(k) is evaluated once per segment; a node evaluates
+// only its two ends.
+
+constexpr int kFeasRecSlack = 2;
+
+template <int N>
+__host__ __device__ constexpr int feas_rec_cap(int k) {  // entries of one (axis, order k) root list
+  return (N - 2 - k > 0 ? N - 2 - k : 0) + kFeasRecSlack;
+}
+template <int N>
+__host__ __device__ constexpr int feas_rec_base(int k) {  // first entry of order k's three lists
+  return k <= 1 ? 0 : feas_rec_base<N>(k - 1) + 3 * feas_rec_cap<N>(k - 1);
+}
+
+// p_i^(k)(t) with Polynomial::evaluate's arithmetic
+template <int N>
+__device__ __forceinline__ double feas_axis_value(const double* __restrict__ c, int i, int k, double t) {
+  double cd[N];
+#pragma unroll
+  for (int j = 0; j < N; ++j) cd[j] = c[i * N + j];
+  return range_horner_any<N>(cd, t, k);
+}
+
+// evaluateThrust: |p''(t) + (0, 0, g)|, the acceleration evaluated first and g added to z afterwards
+template <int N>
+__device__ __forceinline__ double feas_rec_thrust(const double* __restrict__ c, double g, double t) {
+  double sq = 0.0;
+#pragma unroll 1
+  for (int d = 0; d < 3; ++d) {
+    double a = feas_axis_value<N>(c, d, 2, t);
+    if (d == 2) a = __dadd_rn(a, g);
+    sq = __dadd_rn(sq, __dmul_rn(a, a));
+  }
+  return __dsqrt_rn(sq);
+}
+
+// std::max / std::min (the first argument on a tie or a NaN second argument)
+__device__ __forceinline__ double feas_max(double a, double b) { return a < b ? b : a; }
+__device__ __forceinline__ double feas_min(double a, double b) { return b < a ? b : a; }
+
+// The check of one segment (time T > 0 and finite): a FeasResult, or-ed with kFeasCapacity when a root list or the
+// walk ran out of room (the segment is then reported Indeterminable).
+template <int N>
+__device__ int feas_rec_segment(const double* __restrict__ c, double T, const FeasParams& prm) {
+  constexpr int L = feas_rec_base<N>(4);  // entries of all nine lists
+  if (prm.D != 3 && prm.D != 4) return kFeasIndeterminable;
+  const unsigned pr = prm.present;
+  const bool need[4] = {false, (pr & kFeasVMax) != 0, (pr & (kFeasFMin | kFeasFMax | kFeasOmegaXY)) != 0,
+                        (pr & kFeasOmegaXY) != 0};
+  double rt[L], rv[L];  // root times and their p_i^(k)
+  int cnt[9];
+  double yaw_max[2] = {0.0, 0.0};  // max |yaw'|, |yaw''| over 0, T and every candidate (computeMinMax on [0, T])
+  bool full = false;
+  // lists 0..8: (order k = 1 + q / 3, axis q % 3); 9, 10: yaw' and yaw'' (dim 3, D = 4) -- one inlined isolation
+#pragma unroll 1
+  for (int q = 0; q < 11; ++q) {
+    const bool yaw = q >= 9;
+    const int k = yaw ? q - 8 : 1 + q / 3, i = yaw ? 3 : q % 3;
+    if (!yaw) cnt[q] = 0;
+    if (yaw ? !(prm.D == 4 && (pr & (q == 9 ? kFeasOmegaZ : kFeasOmegaZDot))) : !need[k]) continue;
+    double g[N - 1];
+    extrema_critical<N, N - 1>(c + i * N, T, 1, k, 0.0, g);
+    if (yaw) {
+      double hi = fmax(fabs(feas_axis_value<N>(c, 3, k, 0.0)), fabs(feas_axis_value<N>(c, 3, k, T)));
+      extrema_candidates(g, [&](double tau, bool) { hi = fmax(hi, fabs(feas_axis_value<N>(c, 3, k, tau * T))); });
+      yaw_max[q - 9] = hi;
+      continue;
+    }
+    const int cap = feas_rec_cap<N>(k), o = feas_rec_base<N>(k) + i * cap;
+    int n = 0;
+    extrema_candidates<N - 1, true>(g, [&](double tau, bool root) {
+      if (!root) return;
+      if (n == cap) {
+        full = true;
+        return;
+      }
+      const double t = tau * T;
+      rt[o + n] = t;
+      rv[o + n] = feas_axis_value<N>(c, i, k, t);
+      ++n;
+    });
+    cnt[q] = n;
+  }
+  if (full) return kFeasIndeterminable | kFeasCapacity;
+  const double g = prm.gravity;
+  // recursiveFeasibility on one section [t1, t2]
+  const int r = feas_walk(T, prm.min_section_time, [&](double t1, double t2) -> int {
+    if (pr & (kFeasFMin | kFeasFMax)) {
+      const double f1 = feas_rec_thrust<N>(c, g, t1), f2 = feas_rec_thrust<N>(c, g, t2);
+      if ((pr & kFeasFMin) && feas_min(f1, f2) < prm.f_min) return kFeasThrustLow;
+      if ((pr & kFeasFMax) && feas_max(f1, f2) > prm.f_max) return kFeasThrustHigh;
+    }
+    if (pr & kFeasVMax) {
+      const double v1 = extrema_magnitude<N>(c, 3, 1, t1), v2 = extrema_magnitude<N>(c, 3, 1, t2);
+      if (feas_max(v1, v2) > prm.v_max) return kFeasVelocity;
+    }
+    double f_min_sqr = 0.0, f_max_sqr = 0.0, v_max_sqr = 0.0, j_max_sqr = 0.0;
+#pragma unroll 1
+    for (int q = 0; q < 9; ++q) {
+      const int k = 1 + q / 3, i = q % 3;
+      if (!need[k]) continue;
+      // selectMinMaxFromRoots: candidates t1, t2 and the roots in the closed [t1, t2]
+      double lo = DBL_MAX, hi = -DBL_MAX;
+      auto take = [&](double v) {
+        if (v < lo) lo = v;
+        if (v > hi) hi = v;
+      };
+      take(feas_axis_value<N>(c, i, k, t1));
+      take(feas_axis_value<N>(c, i, k, t2));
+      const int o = feas_rec_base<N>(k) + i * feas_rec_cap<N>(k);
+      for (int e = 0; e < cnt[q]; ++e)
+        if (!(rt[o + e] < t1 || rt[o + e] > t2)) take(rv[o + e]);
+      if (k == 1) {
+        if (feas_max(__dmul_rn(lo, lo), __dmul_rn(hi, hi)) > __dmul_rn(prm.v_max, prm.v_max)) return kFeasVelocity;
+        const double m = feas_max(fabs(lo), fabs(hi));
+        v_max_sqr = __dadd_rn(v_max_sqr, __dmul_rn(m, m));
+      } else if (k == 2) {
+        const double gi = i == 2 ? g : 0.0;  // gravity_[i]
+        const double f_lo = __dadd_rn(lo, gi), f_hi = __dadd_rn(hi, gi);
+        const double m = feas_max(fabs(f_lo), fabs(f_hi));
+        if ((pr & kFeasFMax) && m > prm.f_max) return kFeasThrustHigh;
+        if (!(__dmul_rn(f_lo, f_hi) < 0.0)) {
+          const double l = feas_min(fabs(f_lo), fabs(f_hi));
+          f_min_sqr = __dadd_rn(f_min_sqr, __dmul_rn(l, l));
         }
-        prm.result[traj] = res;
-        if (prm.segment) prm.segment[traj] = seg;
-        if (prm.status) prm.status[traj] = st;
-      });
+        f_max_sqr = __dadd_rn(f_max_sqr, __dmul_rn(m, m));
+      } else {
+        const double m = feas_max(fabs(lo), fabs(hi));
+        j_max_sqr = __dadd_rn(j_max_sqr, __dmul_rn(m, m));
+      }
+    }
+    const double f_lower = __dsqrt_rn(f_min_sqr), f_upper = __dsqrt_rn(f_max_sqr), v_upper = __dsqrt_rn(v_max_sqr);
+    const double omega_upper = f_min_sqr > 1.0e-6 ? __dsqrt_rn(__ddiv_rn(j_max_sqr, f_min_sqr)) : DBL_MAX;
+    if ((pr & kFeasFMin) && f_upper < prm.f_min) return kFeasThrustLow;
+    if ((pr & kFeasFMax) && f_lower > prm.f_max) return kFeasThrustHigh;
+    const bool split = ((pr & kFeasFMin) && f_lower < prm.f_min) || ((pr & kFeasFMax) && f_upper > prm.f_max) ||
+                       ((pr & kFeasVMax) && v_upper > prm.v_max) || ((pr & kFeasOmegaXY) && omega_upper > prm.omega_xy);
+    return split ? kFeasSplit : int(kFeasFeasible);
+  });
+  if (r != kFeasFeasible || prm.D != 4) return r;
+  if ((pr & kFeasOmegaZ) && yaw_max[0] > prm.omega_z) return kFeasYawRates;
+  if ((pr & kFeasOmegaZDot) && yaw_max[1] > prm.omega_z_dot) return kFeasYawAcc;
+  return kFeasFeasible;
+}
+
+// One thread per (trajectory, segment) runs feas_rec_segment; the first segment that is not Feasible decides.
+template <int N>
+__global__ void __launch_bounds__(kExtremaThreads, 1)
+    input_feasibility_recursive_kernel(const FeasParams prm, const int tpb) {
+  first_failing_segment(
+      prm.B, prm.K, prm.times, tpb,
+      [&](long long item, double T) { return feas_rec_segment<N>(prm.coeffs + item * prm.D * N, T, prm); },
+      [&](long long traj, bool bad, int seg, int code) { feas_row(prm, traj, bad, seg, code); });
 }
 
 }  // namespace mtg

@@ -114,6 +114,14 @@ class BatchPolynomialOptimization {
                              double gravity = kGravity) const {
     return core_.checkInputFeasibility(constraints, min_section_time, gravity, result, segment);
   }
+  // FeasibilityRecursive::checkInputFeasibilityTrajectory (reference mav_trajectory_generation_ros/src/
+  // feasibility_recursive.cpp) of every trajectory at its current coefficients, on the GPU, with the outputs of
+  // checkInputFeasibility.  min_section_time is FeasibilityRecursive::Settings' (its abs() is taken).
+  bool checkInputFeasibilityRecursive(const InputConstraints& constraints, double min_section_time,
+                                      std::vector<InputFeasibilityResult>* result, std::vector<int>* segment = nullptr,
+                                      double gravity = kGravity) const {
+    return core_.checkInputFeasibility(constraints, min_section_time, gravity, result, segment, true);
+  }
   // FeasibilityBase::checkHalfPlaneFeasibility (reference mav_trajectory_generation_ros/src/feasibility_base.cpp) of
   // every trajectory at its current coefficients against one set of at most MTG_MAX_HALF_PLANES planes, on the GPU:
   // feasible[b] (1 or 0), and segment[b], plane[b] = the first failing pair (-1 when the row is feasible or has a

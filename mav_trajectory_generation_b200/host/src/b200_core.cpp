@@ -641,8 +641,14 @@ bool BatchCore::scaleSegmentTimesWithViolation(double v_max, double a_max, std::
   return true;
 }
 
+namespace {
+typedef int (*InputFeasibilityEntry)(mtg_handle*, int32_t, int32_t, int32_t, int64_t, const double*, const double*,
+                                     const mtg_input_constraints*, int32_t*, int32_t*, int32_t*);
+}
+
 bool BatchCore::checkInputFeasibility(const InputConstraints& constraints, double min_section_time, double gravity,
-                                      std::vector<InputFeasibilityResult>* result, std::vector<int>* segment) const {
+                                      std::vector<InputFeasibilityResult>* result, std::vector<int>* segment,
+                                      bool recursive) const {
   CHECK_GT(B_, 0u) << "setup first";
   CHECK_NOTNULL(result);
   mtg_input_constraints ic = {};
@@ -650,14 +656,18 @@ bool BatchCore::checkInputFeasibility(const InputConstraints& constraints, doubl
   for (int q = 0; q < 6; ++q)
     if (constraints.getConstraint(q, values[q])) ic.present |= 1u << q;  // InputConstraintType order
   ic.gravity = gravity;
-  ic.min_section_time = std::abs(min_section_time);  // FeasibilityAnalytic::Settings::setMinSectionTimeS
+  ic.min_section_time = std::abs(min_section_time);  // Settings::setMinSectionTimeS
+  const InputFeasibilityEntry entry =
+      recursive ? mtg_input_feasibility_recursive_batch_host_f64 : mtg_input_feasibility_batch_host_f64;
+  const char* name =
+      recursive ? "mtg_input_feasibility_recursive_batch_host_f64" : "mtg_input_feasibility_batch_host_f64";
   std::vector<int32_t> res(B_, 0), seg(B_, -1);
   HandleLock lock;
   mtg_handle* h = defaultHandle();
-  const int rc = mtg_input_feasibility_batch_host_f64(h, N_, topo_.K, topo_.D, static_cast<int64_t>(B_), times_,
-                                                      coeffs_, &ic, res.data(), seg.data(), nullptr);
+  const int rc = entry(h, N_, topo_.K, topo_.D, static_cast<int64_t>(B_), times_, coeffs_, &ic, res.data(), seg.data(),
+                       nullptr);
   if (rc != MTG_OK) {
-    LOG(ERROR) << "mtg_input_feasibility_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+    LOG(ERROR) << name << " failed (rc=" << rc << "): " << mtg_last_error(h);
     return false;
   }
   result->resize(B_);

@@ -1,12 +1,14 @@
-// b200_feasibility.cpp -- InputConstraints, FeasibilityBase::checkInputFeasibilityTrajectory and
-// FeasibilityAnalytic::checkInputFeasibility for one segment on the host (reference
-// mav_trajectory_generation_ros/src/input_constraints.cpp, feasibility_base.cpp, feasibility_analytic.cpp), on the
-// extremum candidates of b200_extrema.cpp.  The batched GPU form is mtg_input_feasibility_batch_f64.
+// b200_feasibility.cpp -- InputConstraints, FeasibilityBase::checkInputFeasibilityTrajectory,
+// FeasibilityAnalytic::checkInputFeasibility and FeasibilityRecursive::checkInputFeasibility for one segment on the
+// host (reference mav_trajectory_generation_ros/src/input_constraints.cpp, feasibility_base.cpp,
+// feasibility_analytic.cpp, feasibility_recursive.cpp), on the extremum candidates and roots of b200_extrema.cpp.  The
+// batched GPU forms are mtg_input_feasibility_batch_f64 and mtg_input_feasibility_recursive_batch_f64.
 #include <algorithm>
 #include <cmath>
 #include <limits>
 
 #include "mav_trajectory_generation_ros/feasibility_analytic.h"
+#include "mav_trajectory_generation_ros/feasibility_recursive.h"
 
 namespace mav_trajectory_generation {
 
@@ -220,6 +222,126 @@ InputFeasibilityResult FeasibilityAnalytic::rollPitchFeasibility(const Segment& 
       rollPitchFeasibility(segment, thrust_segment, thrust_candidates, jerk_candidates, t_1, t_half);
   if (left != kInputFeasible) return left;
   return rollPitchFeasibility(segment, thrust_segment, thrust_candidates, jerk_candidates, t_half, t_2);
+}
+
+}  // namespace mav_trajectory_generation
+
+// ---- FeasibilityRecursive (reference src/feasibility_recursive.cpp) -------------------------------------------------
+// std::pow(x, 2) of the reference is x * x here: an optimised x86 build computes it with one multiplication.
+
+namespace mav_trajectory_generation {
+
+namespace {
+inline double square(double x) { return x * x; }
+}  // namespace
+
+InputFeasibilityResult FeasibilityRecursive::checkInputFeasibility(const Segment& segment) const {
+  if (segment.D() != 3 && segment.D() != 4) return kInputIndeterminable;
+  const InputConstraints& ic = input_constraints_;
+  // per position axis, the roots of the derivative of each order the sections bound
+  Roots roots_acc, roots_jerk, roots_snap;
+  const bool need[3] = {ic.hasConstraint(kVMax),
+                        ic.hasConstraint(kFMin) || ic.hasConstraint(kFMax) || ic.hasConstraint(kOmegaXYMax),
+                        ic.hasConstraint(kOmegaXYMax)};
+  Roots* lists[3] = {&roots_acc, &roots_jerk, &roots_snap};
+  const int orders[3] = {derivative_order::ACCELERATION, derivative_order::JERK, derivative_order::SNAP};
+  for (int q = 0; q < 3; ++q) {
+    if (!need[q]) continue;
+    lists[q]->resize(3);
+    for (int i = 0; i < 3; ++i)
+      if (!segment[i].getRoots(orders[q], &(*lists[q])[i])) return kInputIndeterminable;
+  }
+  const InputFeasibilityResult result =
+      recursiveFeasibility(segment, roots_acc, roots_jerk, roots_snap, 0.0, segment.getTime());
+  if (result != kInputFeasible || segment.D() != 4) return result;
+  // yaw rate and acceleration over the whole segment (independent of the translation in the rigid-body model)
+  const int yaw_orders[2] = {derivative_order::ANGULAR_VELOCITY, derivative_order::ANGULAR_ACCELERATION};
+  const int types[2] = {kOmegaZMax, kOmegaZDotMax};
+  const InputFeasibilityResult fails[2] = {kInputInfeasibleYawRates, kInputInfeasibleYawAcc};
+  for (int q = 0; q < 2; ++q) {
+    double limit;
+    if (!ic.getConstraint(types[q], &limit)) continue;
+    std::pair<double, double> lo, hi;
+    if (!segment[3].computeMinMax(0.0, segment.getTime(), yaw_orders[q], &lo, &hi)) return kInputIndeterminable;
+    if (std::max(std::abs(lo.second), std::abs(hi.second)) > limit) return fails[q];
+  }
+  return kInputFeasible;
+}
+
+// One section [t_1, t_2]: the end points first, then bounds from the single-axis extrema; a section whose bounds are
+// not conclusive is halved, left half first.
+InputFeasibilityResult FeasibilityRecursive::recursiveFeasibility(const Segment& segment, const Roots& roots_acc,
+                                                                  const Roots& roots_jerk, const Roots& roots_snap,
+                                                                  double t_1, double t_2) const {
+  if (t_2 - t_1 < settings_.getMinSectionTimeS()) return kInputIndeterminable;
+  const InputConstraints& ic = input_constraints_;
+  double f_min_limit = 0.0, f_max_limit = 0.0, v_max_limit = 0.0, omega_xy_limit = 0.0;
+  const bool has_f_min = ic.getConstraint(kFMin, &f_min_limit), has_f_max = ic.getConstraint(kFMax, &f_max_limit);
+  const bool has_v_max = ic.getConstraint(kVMax, &v_max_limit);
+  const bool has_omega_xy = ic.getConstraint(kOmegaXYMax, &omega_xy_limit);
+  // thrust and speed at the section's ends
+  if (has_f_min || has_f_max) {
+    const double f_1 = evaluateThrust(segment, t_1), f_2 = evaluateThrust(segment, t_2);
+    if (has_f_min && std::min(f_1, f_2) < f_min_limit) return kInputInfeasibleThrustLow;
+    if (has_f_max && std::max(f_1, f_2) > f_max_limit) return kInputInfeasibleThrustHigh;
+  }
+  if (has_v_max) {
+    const double v_1 = segment.evaluate(t_1, derivative_order::VELOCITY).head(3).norm();
+    const double v_2 = segment.evaluate(t_2, derivative_order::VELOCITY).head(3).norm();
+    if (std::max(v_1, v_2) > v_max_limit) return kInputInfeasibleVelocity;
+  }
+  // squared bounds summed over the axes
+  double f_min_sqr = 0.0, f_max_sqr = 0.0, v_max_sqr = 0.0, j_max_sqr = 0.0;
+  if (has_v_max) {
+    for (int i = 0; i < 3; ++i) {
+      std::pair<double, double> lo, hi;
+      segment[i].selectMinMaxFromRoots(t_1, t_2, derivative_order::VELOCITY, roots_acc[i], &lo, &hi);
+      // one axis alone faster than the limit
+      if (std::max(square(lo.second), square(hi.second)) > square(v_max_limit)) return kInputInfeasibleVelocity;
+      v_max_sqr += square(std::max(std::abs(lo.second), std::abs(hi.second)));
+    }
+  }
+  if (has_f_min || has_f_max || has_omega_xy) {
+    for (int i = 0; i < 3; ++i) {
+      std::pair<double, double> lo, hi;
+      segment[i].selectMinMaxFromRoots(t_1, t_2, derivative_order::ACCELERATION, roots_jerk[i], &lo, &hi);
+      const double f_lo = lo.second + gravity_[i], f_hi = hi.second + gravity_[i];
+      // one axis alone above the thrust limit
+      if (has_f_max && std::max(std::abs(f_lo), std::abs(f_hi)) > f_max_limit) return kInputInfeasibleThrustHigh;
+      // an axis whose thrust changes sign contributes nothing to the lower bound
+      if (!(f_lo * f_hi < 0.0)) f_min_sqr += square(std::min(std::abs(f_lo), std::abs(f_hi)));
+      f_max_sqr += square(std::max(std::abs(f_lo), std::abs(f_hi)));
+    }
+  }
+  if (has_omega_xy) {
+    for (int i = 0; i < 3; ++i) {
+      std::pair<double, double> lo, hi;
+      segment[i].selectMinMaxFromRoots(t_1, t_2, derivative_order::JERK, roots_snap[i], &lo, &hi);
+      j_max_sqr += square(std::max(std::abs(lo.second), std::abs(hi.second)));
+    }
+  }
+  const double f_lower = std::sqrt(f_min_sqr), f_upper = std::sqrt(f_max_sqr), v_upper = std::sqrt(v_max_sqr);
+  // Mueller's roll / pitch rate bound |j| / |f|, unbounded where the thrust may vanish
+  const double omega_xy_upper =
+      f_min_sqr > 1.0e-6 ? std::sqrt(j_max_sqr / f_min_sqr) : std::numeric_limits<double>::max();
+  if (has_f_min && f_upper < f_min_limit) return kInputInfeasibleThrustLow;
+  if (has_f_max && f_lower > f_max_limit) return kInputInfeasibleThrustHigh;
+  if ((has_f_min && f_lower < f_min_limit) || (has_f_max && f_upper > f_max_limit) ||
+      (has_v_max && v_upper > v_max_limit) || (has_omega_xy && omega_xy_upper > omega_xy_limit)) {
+    const double t_half = (t_1 + t_2) / 2;
+    const InputFeasibilityResult left = recursiveFeasibility(segment, roots_acc, roots_jerk, roots_snap, t_1, t_half);
+    if (left != kInputFeasible) return left;
+    return recursiveFeasibility(segment, roots_acc, roots_jerk, roots_snap, t_half, t_2);
+  }
+  return kInputFeasible;
+}
+
+// |p''(t) + gravity| over the position dimensions, the acceleration evaluated first
+double FeasibilityRecursive::evaluateThrust(const Segment& segment, double time) const {
+  const Eigen::VectorXd a = segment.evaluate(time, derivative_order::ACCELERATION);
+  double sq = 0.0;
+  for (int i = 0; i < 3; ++i) sq += square(a[i] + gravity_[i]);
+  return std::sqrt(sq);
 }
 
 }  // namespace mav_trajectory_generation
