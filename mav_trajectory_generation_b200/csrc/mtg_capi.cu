@@ -201,6 +201,8 @@ constexpr int kV5Early = 2;
 constexpr int kV4MaxK = 8;
 // warps per CTA of the chunked kernel's instantiations (WaypointEntry::k3)
 constexpr int kChunkedWarps[2] = {1, 4};
+// the paired form has mbarriers for the largest C that plan_chunked() picks
+static_assert(mtg::ChunkedPairLayout<10, 3, kRingDepth>::kMaxChunk >= 24, "paired K3: C up to 24");
 typedef void (*SweepKernel)(const mtg::WaypointParams);                    // v1, v2
 typedef void (*TmemKernel)(const mtg::WaypointParams, const CUtensorMap);  // v3, cost-only
 typedef void (*V4Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV4, const CUtensorMap);
@@ -215,6 +217,8 @@ struct WaypointEntry {
   ChunkedKernel k3[2];            // K3: any K, kChunkedWarps[i] warps per CTA
   size_t (*k3_smem[2])(int C);    // with C resident blocks per lane
   int k3_park;                    // doubles per thread of one vertex block that K3 parks in global memory
+  ChunkedKernel k3_pair;          // K3 in warp pairs (one tile's inward sweep beside the last tile's outward one)
+  size_t (*k3_pair_smem)(int C);
   // null where the shape has no such instantiation
   SweepKernel v1;                 // one thread per trajectory (cross-checks and profiles)
   size_t (*v1_smem)(int K);
@@ -245,6 +249,8 @@ WaypointEntry waypoint_row() {
   e.k3_smem[0] = mtg::ChunkedLayout<N, D, kRingDepth, 1>::bytes;
   e.k3_smem[1] = mtg::ChunkedLayout<N, D, kRingDepth, 4>::bytes;
   e.k3_park = mtg::ChunkedLayout<N, D, kRingDepth, 4>::kPark;
+  e.k3_pair = mtg::twisted_chunked_pair_kernel<N, R, D, kRingDepth>;
+  e.k3_pair_smem = mtg::ChunkedPairLayout<N, D, kRingDepth>::bytes;
   if constexpr ((FLAGS & kV1) != 0) {
     e.v1 = mtg::waypoint_solve_kernel<N, R, D>;
     e.v1_smem = mtg::V1Layout<N, D>::bytes;
@@ -514,7 +520,9 @@ struct WaypointPlan {
 
 // K3: the chunked twisted kernel -- any K, fixed on-chip footprint; the vertex blocks beyond the C resident ones
 // are parked in global memory.
-int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, int64_t B, WaypointPlan* pl) {
+// With `pairs` (the default route), the paired form takes the solve where it fits: see below.
+int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, int64_t B, bool pairs,
+                 WaypointPlan* pl) {
   const int nmax = (p->K + 1) / 2 - 1;
   // Auto: one-warp CTAs (shared memory then comes in 31-52 KB steps instead of 124-206 KB ones), no L2 hints, at
   // most kAutoParkWarps warps per SM while any block is parked and as many as fit otherwise; among the chunks up to
@@ -559,17 +567,49 @@ int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, in
     h->error = "chunked kernel: no launch configuration fits";
     return MTG_ERR_ALLOC;
   }
-  const int W = kChunkedWarps[best_i];
   pl->family = Family::Chunked;
+  pl->evict_first = h->l2_hints;
+  // The paired form (twisted_chunked_pair_kernel): 64-thread CTAs that run one tile's inward sweep beside the last
+  // tile's outward sweep on one tile's resident blocks.  Auto: while every block of a lane fits in shared memory
+  // (nmax <= kPairMaxBlocks, K <= 16), C = nmax -- nothing parked -- at kAutoPairs pairs per SM.  Measured with
+  // tools/k3_sweep.py on an H100 80GB HBM3 at N = 10, D = 3, 700 W power limit (ms per solve, spread of the round
+  // medians <= 0.03 ms), against the one-warp auto plan above (K = 16: 2.59, K = 50: 3.09, K = 100: 3.08 in the
+  // same runs), at 2 / 3 / 4 pairs per SM:
+  //   K = 16:  C = 5: 2.43 / 2.74 / 3.06   C = 6: 2.31 / 2.44   C = 7: 2.20 / 2.36
+  //   K = 50:  C = 4: 3.30 / 3.16 / 3.58   C = 5: 3.20 / 3.12 / 3.52
+  //   K = 100: C = 4: 3.28 / 3.13 / 3.55   C = 5: 3.23 / 3.10 / 3.51
+  // More pairs lose the L1 they take, and with blocks parked the pairs do not beat the one-warp plan.  Forced,
+  // CHUNK_BLOCKS sets C and CTAS_PER_SM caps the warps per SM (pairs = CTAS_PER_SM / 2) at any K.  The pairs need an
+  // inward sweep (K >= 3); CHUNK_WARPS or L2_HINTS select the one-warp form.
+  constexpr int kPairMaxBlocks = 7;
+  constexpr int kAutoPairs = 2;
+  const bool forced = h->chunk_blocks > 0 || h->ctas_per_sm > 0;
+  if (pairs && h->chunk_warps == 0 && h->l2_hints == 0 && nmax >= 1 && (forced || nmax <= kPairMaxBlocks)) {
+    const int C = h->chunk_blocks > 0 || nmax > kPairMaxBlocks ? best_C : nmax;
+    const size_t smem = e.k3_pair_smem(C);
+    const int cap = h->ctas_per_sm > 0 ? h->ctas_per_sm / 2 : kAutoPairs;
+    int ctas = 0, carveout = 0;
+    if (cap >= 1) MTG_TRY(chunked_residency(h, (const void*)e.k3_pair, smem, cap, 64, &ctas, &carveout));
+    if (ctas >= (forced ? 1 : kAutoPairs)) {
+      pl->fn = (const void*)e.k3_pair;
+      pl->threads = 64;
+      pl->smem = smem;
+      pl->blocks = std::min<int64_t>((B + 15) / 16, int64_t(ctas) * h->sm_count);
+      pl->chunk = C;
+      if (nmax > C) pl->park_bytes = size_t(nmax - C) * e.k3_park * size_t(pl->blocks) * 64 * sizeof(double);
+      pl->carveout = carveout;
+      return MTG_OK;
+    }
+  }
+  const int npark = nmax - best_C;  // parked vertex blocks per lane
+  pl->chunk = best_C;
+  const int W = kChunkedWarps[best_i];
   pl->fn = (const void*)e.k3[best_i];
   pl->threads = 32 * W;
   pl->smem = best_smem;
   pl->blocks = std::min<int64_t>((B + 16 * W - 1) / (16 * W), int64_t(best_ctas) * h->sm_count);
-  pl->chunk = best_C;
-  const int npark = nmax - best_C;  // parked vertex blocks per lane
   if (npark > 0) pl->park_bytes = size_t(npark) * e.k3_park * size_t(pl->blocks) * pl->threads * sizeof(double);
   pl->carveout = best_carveout;
-  pl->evict_first = h->l2_hints;
   return MTG_OK;
 }
 
@@ -587,7 +627,8 @@ int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, in
 //     >= 1), then at most CTAS_PER_SM; CTAS_PER_SM = 9 launches one CTA per tile instead of persistent CTAs.
 //  5. For V in {0, 3, 4, 5, 6}, every fused call, V = 2 when v2's state does not fit in shared memory and V = 1 when
 //     neither v1's nor v2's does: v3 while its factor leaves >= 2 CTAs per SM (counted with the plain kernel's
-//     registers, fused calls too); beyond, K3 for a plain call and no fused kernel for a fused one.
+//     registers, fused calls too); beyond, K3 for a plain call (with V = 0 its paired form where plan_chunked
+//     takes it) and no fused kernel for a fused one.
 //  6. V = 1 where v1 is compiled and fits: v1.  Otherwise v2.
 // v5 and v4 draw tiles from a global counter when DYNAMIC_TILES = 1, and in auto mode when every warp has many tiles
 // (v5: >= 8 and K > 8; v4: >= 16), where the counter balances the tail; otherwise tiles go round-robin, since the
@@ -599,7 +640,7 @@ int plan_waypoint(mtg_handle* h, const mtg_problem* p, const Layout& L, const Wa
   const int V = h->waypoint_variant, K = p->K;
   const int64_t B = prm.B;
   if (!a16(prm.coeffs)) return MTG_ERR_ALLOC;
-  if (V == 5 && !fused) return plan_chunked(h, p, e, B, pl);
+  if (V == 5 && !fused) return plan_chunked(h, p, e, B, false, pl);
   const bool inputs_a16 = fused ? a16(prm.positions) : a16(prm.times) && a16(prm.dfix);
   if ((V == 6 || (V == 0 && h->tma_inputs != 0)) && B % 16 == 0 && inputs_a16 && e.v5) {
     const void* fn = (const void*)(fused ? e.v5_fused : e.v5);
@@ -658,7 +699,7 @@ int plan_waypoint(mtg_handle* h, const mtg_problem* p, const Layout& L, const Wa
     const size_t smem = e.v3_smem(K);
     bool fits = false;
     MTG_TRY(v3_fits(h, (const void*)e.v3, smem, &fits));
-    if (!fits) return fused ? MTG_ERR_ALLOC : plan_chunked(h, p, e, B, pl);
+    if (!fits) return fused ? MTG_ERR_ALLOC : plan_chunked(h, p, e, B, V == 0, pl);
     pl->family = Family::Tmem;
     pl->fn = (const void*)(fused ? e.v3_fused : e.v3);
     pl->blocks = (B + 63) / 64;

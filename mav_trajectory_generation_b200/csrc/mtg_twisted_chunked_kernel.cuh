@@ -25,7 +25,7 @@
 // of the warps per CTA, of the warps per SM and of the L2 hints.
 #pragma once
 
-#include "mtg_twisted_tmem_v4_kernel.cuh"
+#include "mtg_twisted_tmem_v5_kernel.cuh"
 
 namespace mtg {
 
@@ -352,6 +352,354 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
     }
   }
 
+  if (lane == 0) bulk_wait_all();
+}
+
+// ---- K3 in warp pairs ---------------------------------------------------------------------------------------------
+// A 64-thread CTA runs the tiles blockIdx.x, blockIdx.x + gridDim.x, ... of K3 with two warps in lockstep: warp 0
+// (inward) runs tile j's prologue, inward sweep and middle vertex while warp 1 (outward) runs tile j-1's outward
+// sweep and final segment.  Lane l of both warps works on the same trajectory lane and the same column of shared
+// memory, and both call the sweep functions of the one-warp kernel with the same arguments in the same order, so
+// the results are bitwise equal to it.
+//
+// The two tiles in flight share one tile's C resident blocks.  The outward sweep of tile j-1 pops vertex n-k+1 at
+// its k-th step; for k > n-C that pop leaves its slot empty (no parked block is refilled into it), and block k of
+// tile j -- the first one that is not parked -- takes exactly that slot.  So the slot of vertex v alternates with the
+// tile's parity: (v-1) % C on even tiles, (n-v) % C on odd ones.  Parked blocks stay the outer ones of each tile
+// (the refill distance stays C-1 steps) and the parking area has one half per parity.
+//
+// Handshakes (mbarriers, one arrival per lane):
+//   freed[s]  outward -> inward: the slot s has been read for the last time in this tile
+//   ready     inward -> outward: the middle vertex is done and the handoff (starting ed of each lane) written
+// Neither side can run two phases ahead of the other: tile j's inward step n waits for tile j-1's last pop, which
+// follows that tile's wait on `ready` and the landing of all its refills; this needs n >= 1 (K >= 3).
+// tests/test_k3_pair_schedule.py walks this schedule on the host.
+template <int N, int D, int RD>
+struct ChunkedPairLayout {
+  static constexpr int h = N / 2;
+  static constexpr int m = h - 1;
+  static constexpr int kSlots = sweep_state_slots<N, D, true>();
+  static constexpr int kPark = kSlots + 1;
+  static constexpr int kPro = 2 * D + m * D + 1;     // x0, x1, u0[m], T0
+  static constexpr int kRing = RD * (1 + D);         // inward warp's input ring
+  static constexpr int kEnd = D + m * D + 1;         // outward warp: x0, u0[m], T0 of the final segment
+  static constexpr int kHand = h * D;                // handoff: the starting ed of the outward sweep
+  static constexpr int kMaxChunk = 31;               // mbarriers: freed[C], ready
+  static constexpr size_t kBarBytes = 8 * (kMaxChunk + 1);
+  static constexpr size_t stage_bytes = tmem_stage_bytes<N, D, 32>();  // the outward warp's staging tile
+  static constexpr int pro = kRing;
+  static constexpr int end = pro + kPro;
+  static constexpr int hand = end + kEnd;
+  static constexpr int times = hand + kHand;         // then C slot times, then C blocks
+  __host__ __device__ static constexpr size_t region(int C) { return size_t(times) + C; }
+  __host__ __device__ static constexpr size_t bytes(int C) {
+    return stage_bytes + kBarBytes + tmem_slot_bytes(region(C) + size_t(C) * kSlots, 32);
+  }
+};
+
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// bulk::mbar_wait with the loop in C++, so that one kernel can wait at several places
+__device__ __forceinline__ void mbar_wait_parity(uint32_t bar, uint32_t parity) {
+  uint32_t done = 0;
+  while (!done)
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(bar), "r"(parity)
+        : "memory");
+}
+
+// 64 threads, at most 4 CTAs per SM by registers (cap 255)
+template <int N, int R, int D, int RD>
+__global__ void __launch_bounds__(64, 4)
+    twisted_chunked_pair_kernel(const WaypointParams prm, const ChunkedLaunch cl,
+                                const __grid_constant__ CUtensorMap tmap) {
+  constexpr int h = N / 2;
+  constexpr int m = h - 1;
+  using Lay = ChunkedPairLayout<N, D, RD>;
+  constexpr int kSlots = Lay::kSlots;
+  constexpr int kPark = Lay::kPark;
+  constexpr int kPro = Lay::kPro;
+  static_assert(RD >= 2, "ring depth");
+  using G = H1Imm<N, R>;
+  using AI = A1InvImm<N>;
+  using S = sweep::Sweep<N, D, G>;
+
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  const int lane = int(threadIdx.x & 31);
+  const bool inward = threadIdx.x < 32;
+  const int half = lane & 1;
+  const int K = prm.K;
+  const int nf = prm.n_fixed;
+  const int M = (K + 1) >> 1;
+  const int nh = half ? K - M - 1 : M - 1;
+  const int n = M - 1;
+  const int C = cl.chunk;
+  const int npark = n - C;
+
+  double2* stage = reinterpret_cast<double2*>(smem_raw);
+  const uint32_t bar0 = smem_u32(smem_raw + Lay::stage_bytes);  // freed[s] at bar0 + 8 s, ready at bar0 + 8 C
+  const uint32_t ready = bar0 + 8u * uint32_t(C);
+  double* base = reinterpret_cast<double*>(smem_raw + Lay::stage_bytes + Lay::kBarBytes) + lane;
+  auto SL = [&](int slot) -> double* { return base + size_t(slot) * 32; };
+  auto PF = [&](int buf, int slot) -> double* { return SL(buf * (1 + D) + slot); };
+  auto PRO = [&](int slot) -> double* { return SL(Lay::pro + slot); };
+  auto END = [&](int slot) -> double* { return SL(Lay::end + slot); };
+  auto HAND = [&](int slot) -> double* { return SL(Lay::hand + slot); };
+  auto HT = [&](int b) -> double* { return SL(Lay::times + b); };
+  auto SP = [&](int blk, int slot) -> double* { return SL(int(Lay::region(C)) + blk * kSlots + slot); };
+  // slot of vertex v in the j-th tile of this CTA
+  auto slot_of = [&](int v, long long j) -> int { return (j & 1) ? (n - v) % C : (v - 1) % C; };
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s <= C; ++s) bulk::mbar_init(bar0 + 8u * uint32_t(s), 32);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  const sweep::Frame<N> fr{K, half};
+  const int e0 = fr.e0();
+  const long long n_wtiles = (prm.B + 15) >> 4;
+  const long long wt_stride = gridDim.x;
+  const long long gthreads = (long long)gridDim.x * 64;
+  // parking column of this lane in the half of tile parity p
+  auto PK = [&](long long j, int b, int slot) -> double* {
+    return cl.ckpt + ((long long)b * kPark + slot) * gthreads + ((long long)blockIdx.x * 64 + (j & 1) * 32 + lane);
+  };
+
+  struct Ptrs {
+    const double* tt;
+    const double* fx;
+    long long traj;
+    bool valid;
+  };
+  auto tile_ptrs = [&](long long w) -> Ptrs {
+    Ptrs p;
+    p.traj = w * 16 + (lane >> 1);
+    p.valid = p.traj < prm.B;
+    if (!p.valid) p.traj = prm.B - 1;
+    p.tt = prm.times + p.traj * K;
+    p.fx = prm.dfix + p.traj * (long long)D * nf;
+    return p;
+  };
+  auto xaddr = [&](const Ptrs& p, int v, int d) -> const double* { return p.fx + d * nf + fr.pidx(v); };
+  const int np = (K - 1) * m;
+
+  if (inward) {
+    // ================================================================ warp 0: prologue, inward sweep, middle
+    auto pro_issue = [&](const Ptrs& p) {
+#pragma unroll
+      for (int d = 0; d < D; ++d) {
+        cp_async8_stream(PRO(d), xaddr(p, 0, d), cl.evict_first);
+        cp_async8_stream(PRO(D + d), xaddr(p, 1, d), cl.evict_first);
+#pragma unroll
+        for (int b = 0; b < m; ++b) cp_async8_stream(PRO(2 * D + b * D + d), p.fx + d * nf + e0 + b, cl.evict_first);
+      }
+      cp_async8_stream(PRO(kPro - 1), p.tt + fr.seg(0), cl.evict_first);
+    };
+    auto ring_issue = [&](const Ptrs& p, int v) {
+      const int j = v < K ? v : K - 1;
+      const int vn = v + 1 <= K ? v + 1 : K;
+      const int buf = v % RD;
+      cp_async8_stream(PF(buf, 0), p.tt + fr.seg(j), cl.evict_first);
+#pragma unroll
+      for (int d = 0; d < D; ++d) cp_async8_stream(PF(buf, 1 + d), xaddr(p, vn, d), cl.evict_first);
+    };
+
+    long long wt = blockIdx.x;
+    if (wt < n_wtiles) {
+      pro_issue(tile_ptrs(wt));
+      cp_async_commit();
+    }
+    for (long long j = 0; wt < n_wtiles; wt += wt_stride, ++j) {
+      const Ptrs P = tile_ptrs(wt);
+#pragma unroll
+      for (int q = 1; q < RD; ++q) {
+        if (q <= nh) ring_issue(P, q);
+        cp_async_commit();
+      }
+      cp_async_wait_group<RD - 1>();
+
+      int stat = 0;
+      double Wp[m][m], yp[m][D], Cee[m][m], cps[m], cpe[m], xm[D], xc[D];
+      {
+#pragma unroll
+        for (int d = 0; d < D; ++d) {
+          xm[d] = *PRO(d);
+          xc[d] = *PRO(D + d);
+        }
+        const double T0 = *PRO(kPro - 1);
+        if (bad_segment_time(T0)) stat |= kStatusBadTime;
+        const double iT0 = fast_rcp(T0);
+        double pw[N - 1];
+        segment_powers<N, R>(T0, iT0, pw);
+        S::end_blocks(pw, Cee, cps, cpe);
+        S::carry_fold(pw, [&](int b, int d) { return fr.sgn(b) * *PRO(2 * D + b * D + d); }, Wp, yp);
+      }
+
+      for (int v = 1; v <= n; ++v) {
+        double sv[kSlots];
+        double T;
+        if (v <= nh) {
+          cp_async_wait_group<RD - 2>();
+          double xn[D];
+#pragma unroll
+          for (int d = 0; d < D; ++d) xn[d] = *PF(v % RD, 1 + d);
+          T = *PF(v % RD, 0);
+          if (v + RD - 1 <= nh) ring_issue(P, v + RD - 1);
+          cp_async_commit();
+          if (bad_segment_time(T)) stat |= kStatusBadTime;
+          const double iT = fast_rcp(T);
+          double pw[N - 1];
+          segment_powers<N, R>(T, iT, pw);
+
+          double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
+          S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
+          S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
+          S::pack(L, inv, yp, xc, sv);
+          S::end_blocks(pw, Cee, cps, cpe);
+#pragma unroll
+          for (int d = 0; d < D; ++d) {
+            xm[d] = xc[d];
+            xc[d] = xn[d];
+          }
+        }
+        __syncwarp();
+        if (v <= npark) {  // warp-uniform
+#pragma unroll
+          for (int i = 0; i < kSlots; ++i) *PK(j, v - 1, i) = sv[i];
+          *PK(j, v - 1, kSlots) = T;
+        } else {
+          const int b = slot_of(v, j);
+          if (j > 0) mbar_wait_parity(bar0 + 8u * uint32_t(b), uint32_t((j - 1) & 1));  // freed by the last tile
+          if (v <= nh) *HT(b) = T;
+#pragma unroll
+          for (int i = 0; i < kSlots; ++i) *SP(b, i) = sv[i];
+        }
+      }
+      // the prologue region is this warp's own: the next tile's inputs land during the middle vertex
+      if (wt + wt_stride < n_wtiles) {
+        pro_issue(tile_ptrs(wt + wt_stride));
+        cp_async_commit();
+      }
+
+      double um[m][D];
+      S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
+      if (P.valid && half == 0 && prm.status != nullptr) prm.status[P.traj] = stat;
+      if (half == 0 && prm.dfree != nullptr && P.valid) {
+        double* __restrict__ df = prm.dfree + P.traj * (long long)D * np;
+        const int vo = fr.vert(nh + 1);
+#pragma unroll
+        for (int d = 0; d < D; ++d)
+#pragma unroll
+          for (int q = 0; q < m; ++q) df[d * np + (vo - 1) * m + q] = fr.sgn(q) * um[q][d];
+      }
+#pragma unroll
+      for (int d = 0; d < D; ++d) {
+        *HAND(d) = xc[d];
+#pragma unroll
+        for (int q = 0; q < m; ++q) *HAND((1 + q) * D + d) = um[q][d];
+      }
+      mbar_arrive(ready);
+    }
+    return;
+  }
+
+  // ================================================================== warp 1: outward sweep, final segment
+  double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
+  const int nhF = M - 1, nhB = K - M - 1;
+  const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB, cl.evict_first != 0};
+
+  long long j = 0;
+  for (long long wt = blockIdx.x; wt < n_wtiles; wt += wt_stride, ++j) {
+    const Ptrs P = tile_ptrs(wt);
+    const long long traj0 = wt * 16;
+    const bool valid = P.valid;
+    // what the final segment reads besides ed, many steps ahead of its use
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+      cp_async8_stream(END(d), xaddr(P, 0, d), cl.evict_first);
+#pragma unroll
+      for (int b = 0; b < m; ++b) cp_async8_stream(END(D + b * D + d), P.fx + d * nf + e0 + b, cl.evict_first);
+    }
+    cp_async8_stream(END(Lay::kEnd - 1), P.tt + fr.seg(0), cl.evict_first);
+    cp_async_commit();
+
+    double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + P.traj * (long long)D * np : nullptr;
+    auto store_free = [&](int v_own, const double (&u)[h][D]) {
+      if (df != nullptr && valid) {
+        const int vo = fr.vert(v_own);
+#pragma unroll
+        for (int d = 0; d < D; ++d)
+#pragma unroll
+          for (int q = 0; q < m; ++q) df[d * np + (vo - 1) * m + q] = fr.sgn(q) * u[1 + q][d];
+      }
+    };
+
+    mbar_wait_parity(ready, uint32_t(j & 1));
+    double ed[h][D];
+#pragma unroll
+    for (int d = 0; d < D; ++d)
+#pragma unroll
+      for (int k = 0; k < h; ++k) ed[k][d] = *HAND(k * D + d);
+
+    for (int v = n; v >= 1; --v) {
+      const int b = slot_of(v, j);
+      if (v <= npark) cp_async_wait_at_most(C - 1);
+      const bool act = v <= nh;
+      const double T = act ? *HT(b) : 1.0;
+      const double iT = fast_rcp(T);
+      double pw[N - 1];
+      segment_powers<N, R>(T, iT, pw);
+      double sv[kSlots];
+#pragma unroll
+      for (int i = 0; i < kSlots; ++i) sv[i] = *SP(b, i);
+      if (v - C >= 1) {  // warp-uniform: the slot takes parked block v-C
+#pragma unroll
+        for (int i = 0; i < kSlots; ++i) cp_async8(SP(b, i), PK(j, v - C - 1, i));
+        cp_async8(HT(b), PK(j, v - C - 1, kSlots));
+      } else {
+        mbar_arrive(bar0 + 8u * uint32_t(b));  // the slot is the next tile's
+      }
+      cp_async_commit();
+      double tE[m][D];
+      S::couple(pw, ed, tE);
+      double sd[h][D];
+      if (act) {
+        double xv[D];
+#pragma unroll
+        for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
+        S::back_substitute(sv, tE, xv, sd);
+        store_free(v, sd);
+      }
+      __syncwarp();
+      out.emit(v, v, T, iT, sd, ed, traj0);
+      if (act) {
+#pragma unroll
+        for (int d = 0; d < D; ++d)
+#pragma unroll
+          for (int k = 0; k < h; ++k) ed[k][d] = sd[k][d];
+      }
+    }
+    {  // own segment 0: the fixed end vertex
+      double sd[h][D];
+      cp_async_wait_group<0>();
+#pragma unroll
+      for (int d = 0; d < D; ++d) {
+        sd[0][d] = *END(d);
+#pragma unroll
+        for (int b = 0; b < m; ++b) sd[1 + b][d] = fr.sgn(b) * *END(D + b * D + d);
+      }
+      const double T = *END(Lay::kEnd - 1);
+      const double iT = fast_rcp(T);
+      __syncwarp();
+      out.emit(0, 0, T, iT, sd, ed, traj0);
+    }
+  }
   if (lane == 0) bulk_wait_all();
 }
 

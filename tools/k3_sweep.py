@@ -3,13 +3,15 @@
 Times K3 (N = 10, r = 4, D = 3) at K = 8, 16, 50 and 100 over
   * C: vertex blocks per lane kept in shared memory (--cs, default 2 to 6),
   * warps per SM, from 4 up to the most that fit, as one-warp CTAs (W = 1) and as four-warp CTAs (W = 4),
+  * pairs per SM of the paired form (W = 2: twisted_chunked_pair_kernel, which the default route launches), from 2
+    up to the most that fit,
   * L2 cache hints on the streamed inputs and coefficient stores on and off (--hints, default both),
 in one process.  Every configuration is timed in each of --rounds rounds (the order alternates between rounds), with
 CUDA events around --steps solves after --warmup solves; the line of a configuration gives the median of its round
 medians and the spread of the round medians.  `same` says whether its coefficients are bitwise equal to those of the
 first configuration of the same K.  The card name and power limit are read in the same run.
 
-  python tools/k3_sweep.py [--ks 8,16,50,100] [--cs 2,3,4,5,6] [--hints 0,1] [--rounds 3] [--out DIR]
+  python tools/k3_sweep.py [--ks 8,16,50,100] [--cs 2,3,4,5,6] [--ws 1,4,2] [--hints 0,1] [--rounds 3] [--out DIR]
 """
 import argparse
 import json
@@ -33,9 +35,13 @@ MAX_WARPS_BY_REGS = 8     # K3 at N = 10, D = 3 uses 248-250 registers per threa
 
 
 def k3_smem(C, W):
-    """Dynamic shared memory of K3 at N = 10, D = 3 (ChunkedLayout<10, 3, 3, W>::bytes, ring depth 3)"""
+    """Dynamic shared memory of K3 at N = 10, D = 3 (ChunkedLayout<10, 3, 3, W>::bytes, ring depth 3; W = 2:
+    ChunkedPairLayout<10, 3, 3>::bytes)"""
     h, slots = N // 2, 25
     pro = 2 * D + (h - 1) * D + 1
+    if W == 2:  # ring, prologue, final-segment inputs, handoff, times, blocks; one staging tile; mbarriers
+        region = 3 * (1 + D) + pro + (D + (h - 1) * D + 1) + h * D + C
+        return 32 * (D * h * 16) + 256 + 32 * 8 * (region + C * slots)
     region = 3 * (1 + D) + C + D + 1
     return 32 * W * (D * h * 16 + 8 * (region + max(C * slots, pro)))
 
@@ -44,17 +50,22 @@ def max_warps(C, W):
     return min(MAX_WARPS_BY_REGS, SMEM_PER_SM // (k3_smem(C, W) + 1024) * W)
 
 
-def configs(K, cs, hint_modes):
+def configs(K, cs, ws, hint_modes):
     nmax = (K + 1) // 2 - 1
     out = []
     for C in cs:
         if C > nmax:
             continue
         for hints in hint_modes:
-            for w in range(4, max_warps(C, 1) + 1):
-                out.append(dict(C=C, W=1, warps=w, hints=hints))
-            for w in range(4, max_warps(C, 4) + 1, 4):
-                out.append(dict(C=C, W=4, warps=w, hints=hints))
+            if 1 in ws:
+                for w in range(4, max_warps(C, 1) + 1):
+                    out.append(dict(C=C, W=1, warps=w, hints=hints))
+            if 4 in ws:
+                for w in range(4, max_warps(C, 4) + 1, 4):
+                    out.append(dict(C=C, W=4, warps=w, hints=hints))
+        if 2 in ws:  # the paired form runs without hints
+            for w in range(4, max_warps(C, 2) + 1, 2):
+                out.append(dict(C=C, W=2, warps=w, hints=0))
     return out
 
 
@@ -72,6 +83,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--ks", default="8,16,50,100")
     ap.add_argument("--cs", default="2,3,4,5,6")
+    ap.add_argument("--ws", default="1,4,2", help="CTA forms: 1 and 4 warps, 2 = warp pairs")
     ap.add_argument("--hints", default="0,1")
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--steps", type=int, default=5)
@@ -89,15 +101,17 @@ def main():
         prob = m.Problem(N, R, K, D)
         times, dfix = synth(N, K, D, B, dev)
         out = torch.empty((B, K, D, N), device=dev, dtype=torch.float64)
-        cfgs = configs(K, [int(c) for c in args.cs.split(",")], [int(x) for x in args.hints.split(",")])
+        cfgs = configs(K, [int(c) for c in args.cs.split(",")], [int(w) for w in args.ws.split(",")],
+                       [int(x) for x in args.hints.split(",")])
         per = [[] for _ in cfgs]
         same = [True] * len(cfgs)
         ref = None
 
         def run(cf):
-            s.set_option(m.capi.OPT_WAYPOINT_VARIANT, 5)
+            # the paired form is the default route's; the one-warp and four-warp forms are forced
+            s.set_option(m.capi.OPT_WAYPOINT_VARIANT, 0 if cf["W"] == 2 else 5)
             s.set_option(m.capi.OPT_CHUNK_BLOCKS, cf["C"])
-            s.set_option(m.capi.OPT_CHUNK_WARPS, cf["W"])
+            s.set_option(m.capi.OPT_CHUNK_WARPS, 0 if cf["W"] == 2 else cf["W"])
             s.set_option(m.capi.OPT_CTAS_PER_SM, cf["warps"])
             s.set_option(m.capi.OPT_L2_HINTS, cf["hints"])
             s.solve_linear(prob, times, dfix, coeffs=out)
