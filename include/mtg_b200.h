@@ -57,7 +57,8 @@ extern "C" {
 #define MTG_STATUS_BAD_TIME 1     /* some segment time <= 0, NaN or +inf (reference: CHECK_GT, linear_impl.h:297) */
 #define MTG_STATUS_NOT_SPD 2      /* non-positive / NaN / infinite pivot in the R_pp factorisation */
 #define MTG_STATUS_FEAS_CAPACITY 4 /* input feasibility: a candidate list (48 entries) or the roll/pitch walk (64 levels)
-                                      ran out of room; the segment is reported Indeterminable */
+                                      ran out of room, or (sampling) a segment needs more than 2^24 samples; the
+                                      segment is reported Indeterminable */
 
 /* which kernel family a problem is routed to (introspection for tests / profiles) */
 #define MTG_KERNEL_WAYPOINT 1     /* specialised block-tridiagonal Cholesky kernels, waypoint topology */
@@ -336,6 +337,32 @@ int mtg_input_feasibility_recursive_batch_f64(mtg_handle* h, int32_t N, int32_t 
                                               const mtg_input_constraints* constraints, int32_t* result,
                                               int32_t* segment, int32_t* status, void* stream);
 
+/* FeasibilitySampling::checkInputFeasibility per segment and checkInputFeasibilityTrajectory per trajectory
+ * (reference mav_trajectory_generation_ros/src/feasibility_sampling.cpp).  Same outputs, refusals of the limits and
+ * gravity, bad-time rule and D rule as mtg_input_feasibility_batch_f64; min_section_time is neither read nor
+ * validated, and sampling_interval (FeasibilitySampling::Settings, reference default 0.01 s) takes its place.  Per
+ * segment the samples are t = 0, fl(t + sampling_interval), ... while t <= T (the reference's running fp64 sum, not
+ * k * sampling_interval, so T itself may be missed), and at each one the flat state goes through mav_msgs'
+ * EigenMavStateFromEigenTrajectoryPoint with the given gravity:
+ *   f = a + (0, 0, g), thrust = |f|, zb = f * (1 / thrust), xc = (cos yaw, sin yaw, 0), yb = normalized(zb x xc),
+ *   xb = yb x zb, acceleration_B = R^T (zb thrust) with R = [xb yb zb], h = (1 / thrust) (j - (zb . j) zb),
+ *   omega_B = (-h . yb, h . xb, yaw_rate zb_z), omega_dot_B,z = yaw_acc zb_z
+ * (yaw, yaw rate, yaw acceleration from dim 3 when D = 4, through the quaternion round trip of setFromYaw / getYaw;
+ * 0 when D = 3).  The checks, in order, the first failing sample and check deciding: only when f_min or f_max is
+ * present |acceleration_B| < f_min (ThrustLow) and > f_max (ThrustHigh); |v| over dims 0..2 > v_max (Velocity);
+ * |omega_B,xy| > omega_xy_max (RollPitchRates); |omega_B,z| > omega_z_max (YawRates); |omega_dot_B,z| >
+ * omega_z_dot_max (YawAcc).  Values use Polynomial::evaluate's Horner and one rounding per operation; a NaN state (a
+ * thrust of exactly 0) passes every comparison, as in the reference.  This is the only entry that returns
+ * MTG_FEAS_ROLL_PITCH_RATES; it never returns MTG_FEAS_INDETERMINABLE for a good row with D 3 or 4 below the cap.
+ *   status MTG_STATUS_FEAS_CAPACITY (result Indeterminable): fl(T / sampling_interval) > 2^24 for the deciding
+ *   segment, which is then not sampled at all.
+ * Refused (MTG_ERR_BAD_ARG, no launch): everything mtg_input_feasibility_batch_f64 refuses except min_section_time,
+ * and a sampling_interval <= 0, NaN or infinite. */
+int mtg_input_feasibility_sampling_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                             const double* seg_times, const double* coeffs,
+                                             const mtg_input_constraints* constraints, double sampling_interval,
+                                             int32_t* result, int32_t* segment, int32_t* status, void* stream);
+
 /* FeasibilityBase::checkHalfPlaneFeasibility per segment and per trajectory (reference
  * mav_trajectory_generation_ros/src/feasibility_base.cpp:109-154): a segment passes plane (point q, normal n) when
  * (p(t) - q) . n > 0 at 0, T and every real root in [0, T] of the derivative of the projection n . p(t); the first
@@ -413,6 +440,10 @@ int mtg_input_feasibility_recursive_batch_host_f64(mtg_handle* h, int32_t N, int
                                                    const double* seg_times, const double* coeffs,
                                                    const mtg_input_constraints* constraints, int32_t* result,
                                                    int32_t* segment, int32_t* status);
+int mtg_input_feasibility_sampling_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                                  const double* seg_times, const double* coeffs,
+                                                  const mtg_input_constraints* constraints, double sampling_interval,
+                                                  int32_t* result, int32_t* segment, int32_t* status);
 int mtg_half_plane_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
                                               const double* seg_times, const double* coeffs, int32_t n_planes,
                                               const mtg_half_plane* planes, int32_t* feasible, int32_t* segment,

@@ -40,7 +40,8 @@ EXPORTED_SYMBOLS = [
     "mtg_scale_times_with_violation_batch_host_f64", "mtg_input_feasibility_batch_f64",
     "mtg_input_feasibility_batch_host_f64", "mtg_half_plane_feasibility_batch_f64",
     "mtg_half_plane_feasibility_batch_host_f64", "mtg_input_feasibility_recursive_batch_f64",
-    "mtg_input_feasibility_recursive_batch_host_f64",
+    "mtg_input_feasibility_recursive_batch_host_f64", "mtg_input_feasibility_sampling_batch_f64",
+    "mtg_input_feasibility_sampling_batch_host_f64",
 ]
 TIME_COST_SQUARED, TIME_COST_RICHTER = 0, 1
 STATUS_FEAS_CAPACITY = 4
@@ -256,6 +257,10 @@ def load():
                                                        C.POINTER(MtgInputConstraints), dp, dp, dp]
     L.mtg_input_feasibility_recursive_batch_f64.argtypes = L.mtg_input_feasibility_batch_f64.argtypes
     L.mtg_input_feasibility_recursive_batch_host_f64.argtypes = L.mtg_input_feasibility_batch_host_f64.argtypes
+    L.mtg_input_feasibility_sampling_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
+                                                           C.POINTER(MtgInputConstraints), dbl, dp, dp, dp, vp]
+    L.mtg_input_feasibility_sampling_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
+                                                                C.POINTER(MtgInputConstraints), dbl, dp, dp, dp]
     L.mtg_half_plane_feasibility_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, C.c_int32,
                                                        C.POINTER(MtgHalfPlane), dp, dp, dp, dp, vp]
     L.mtg_half_plane_feasibility_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
@@ -524,7 +529,15 @@ class Solver:
         return self._input_feasibility("mtg_input_feasibility_recursive_batch_f64", seg_times, coeffs, limits,
                                        min_section_time, gravity, stream)
 
-    def _input_feasibility(self, entry, seg_times, coeffs, limits, min_section_time, gravity, stream):
+    def check_input_feasibility_sampling(self, seg_times, coeffs, limits, sampling_interval=0.01, gravity=GRAVITY,
+                                         stream=None):
+        """Batched FeasibilitySampling::checkInputFeasibilityTrajectory: (result [B], segment [B], status [B]), int32.
+        limits as for check_input_feasibility; samples every sampling_interval seconds from the start of each
+        segment (an MtgInputConstraints' min_section_time is ignored)."""
+        return self._input_feasibility("mtg_input_feasibility_sampling_batch_f64", seg_times, coeffs, limits, 0.05,
+                                       gravity, stream, (float(sampling_interval),))
+
+    def _input_feasibility(self, entry, seg_times, coeffs, limits, min_section_time, gravity, stream, extra=()):
         import torch
         B, K, D, N = coeffs.shape
         dev = coeffs.device
@@ -533,7 +546,7 @@ class Solver:
         segment = torch.empty((B,), dtype=torch.int32, device=dev)
         status = torch.empty((B,), dtype=torch.int32, device=dev)
         s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
-        rc = getattr(self.lib, entry)(self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(), C.byref(ic),
+        rc = getattr(self.lib, entry)(self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(), C.byref(ic), *extra,
                                       result.data_ptr(), segment.data_ptr(), status.data_ptr(), s)
         self._check(rc, entry)
         return result, segment, status
@@ -691,11 +704,20 @@ class Solver:
         return self._input_feasibility_host("mtg_input_feasibility_recursive_batch_host_f64", seg_times, coeffs,
                                             limits, result, segment, status, min_section_time, gravity)
 
+    def check_input_feasibility_sampling_host(self, seg_times, coeffs, limits, result, segment=None, status=None,
+                                              sampling_interval=0.01, gravity=GRAVITY):
+        """check_input_feasibility_sampling into host buffers: result [B], segment [B] or None, status [B] or None
+        (int32)."""
+        return self._input_feasibility_host("mtg_input_feasibility_sampling_batch_host_f64", seg_times, coeffs,
+                                            limits, result, segment, status, 0.05, gravity,
+                                            (float(sampling_interval),))
+
     def _input_feasibility_host(self, entry, seg_times, coeffs, limits, result, segment, status, min_section_time,
-                                gravity):
+                                gravity, extra=()):
         B, K, D, N = coeffs.shape
         ic = limits if isinstance(limits, MtgInputConstraints) else input_constraints(limits, min_section_time, gravity)
         rc = getattr(self.lib, entry)(self.h, N, K, D, B, self._hptr(seg_times), self._hptr(coeffs), C.byref(ic),
+                                      *extra,
                                       self._hptr(result), self._hptr(segment), self._hptr(status))
         self._check(rc, entry)
         return result

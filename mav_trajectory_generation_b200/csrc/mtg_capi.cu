@@ -87,7 +87,7 @@ struct mtg_handle {
   struct FnInfo {
     const void* fn;
     int regs;             // cudaFuncGetAttributes().numRegs
-    size_t max_dyn_smem;  // cudaFuncAttributeMaxDynamicSharedMemorySize as last set (0: never)
+    size_t max_dyn_smem;  // cudaFuncAttributeMaxDynamicSharedMemorySize, at most its real value (0: not yet known)
     int carveout;         // cudaFuncAttributePreferredSharedMemoryCarveout as last set (-1: never)
   };
   std::vector<FnInfo> fns;
@@ -372,12 +372,22 @@ mtg_handle::FnInfo* fn_info(mtg_handle* h, const void* fn) {
 }
 
 // Make sure `fn` may be launched with `bytes` of dynamic shared memory (raises the function attribute when needed).
+// The attribute belongs to the function in the device's context, so every handle of the process shares it, while
+// each handle caches what it knows.  It is therefore only ever raised: under one process-wide lock, to `bytes` when
+// its current value is smaller.  A handle's cached value then stays at or below the real one, even after another
+// handle has needed less (setting the smaller value would make this handle's next larger launch fail).
 int ensure_dyn_smem(mtg_handle* h, const void* fn, size_t bytes) {
   mtg_handle::FnInfo* f = fn_info(h, fn);
   if (!f) return MTG_ERR_CUDA;
   if (bytes <= f->max_dyn_smem) return MTG_OK;
-  MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  f->max_dyn_smem = bytes;
+  static std::mutex attr_lock;
+  std::lock_guard<std::mutex> lock(attr_lock);
+  cudaFuncAttributes attr;
+  MTG_CUDA(h, cudaFuncGetAttributes(&attr, fn));
+  const size_t current = size_t(std::max(attr.maxDynamicSharedSizeBytes, 0));
+  if (current < bytes)
+    MTG_CUDA(h, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  f->max_dyn_smem = std::max(current, bytes);
   return MTG_OK;
 }
 
@@ -1748,25 +1758,42 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
       });
 }
 
-// FeasibilityAnalytic: N even in [4, 12]; the limits are final values (the host mirror's InputConstraints applies
-// addConstraint's corrections), each present one not NaN and >= 0 (+inf never fails); gravity finite; min_section_time
-// > 0 and finite.  Any D: rows with D not 3 or 4 are Indeterminable, as in the reference.
-static bool valid_feasibility(int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
-                              const double* coeffs, const mtg_input_constraints* ic, const int32_t* result) {
+// Every input-feasibility entry: N even in [4, 12]; the limits are final values (the host mirror's InputConstraints
+// applies addConstraint's corrections), each present one not NaN and >= 0 (+inf never fails); gravity finite.  Any D:
+// rows with D not 3 or 4 are Indeterminable, as in the reference.
+static bool valid_input_limits(int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                               const double* coeffs, const mtg_input_constraints* ic, const int32_t* result) {
   if (N < 4 || N > MTG_MAX_N || (N & 1) || K < 1 || D < 1 || !ic) return false;
   if (ic->present & ~uint32_t(MTG_INPUT_ALL)) return false;
   const double limits[6] = {ic->f_min, ic->f_max, ic->v_max, ic->omega_xy_max, ic->omega_z_max, ic->omega_z_dot_max};
   for (int q = 0; q < 6; ++q)
     if ((ic->present >> q & 1u) && !(limits[q] >= 0.0)) return false;
-  if (!std::isfinite(ic->gravity) || !(ic->min_section_time > 0.0) || !std::isfinite(ic->min_section_time))
-    return false;
+  if (!std::isfinite(ic->gravity)) return false;
   return valid_rows(B, {seg_times, coeffs, result});
 }
 
-// recursive: FeasibilityRecursive (input_feasibility_recursive_kernel), else FeasibilityAnalytic
+// FeasibilityAnalytic and FeasibilityRecursive: also min_section_time > 0 and finite
+static bool valid_feasibility(int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                              const double* coeffs, const mtg_input_constraints* ic, const int32_t* result) {
+  return valid_input_limits(N, K, D, B, seg_times, coeffs, ic, result) && ic->min_section_time > 0.0 &&
+         std::isfinite(ic->min_section_time);
+}
+
+// FeasibilitySampling: also sampling_interval > 0 and finite; min_section_time is not read
+static bool valid_sampling(int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times, const double* coeffs,
+                           const mtg_input_constraints* ic, double sampling_interval, const int32_t* result) {
+  return valid_input_limits(N, K, D, B, seg_times, coeffs, ic, result) && sampling_interval > 0.0 &&
+         std::isfinite(sampling_interval);
+}
+
+enum class FeasKind { Analytic, Recursive, Sampling };
+
+// Analytic: input_feasibility_kernel; Recursive: input_feasibility_recursive_kernel; Sampling:
+// input_feasibility_sampling_kernel (a warp per segment) at sampling_interval
 static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                                     const double* coeffs, const mtg_input_constraints* ic, int32_t* result,
-                                    int32_t* segment, int32_t* status, cudaStream_t s, bool recursive = false) {
+                                    int32_t* segment, int32_t* status, cudaStream_t s,
+                                    FeasKind kind = FeasKind::Analytic, double sampling_interval = 0.0) {
   mtg::FeasParams fp;
   fp.K = K;
   fp.D = D;
@@ -1779,6 +1806,7 @@ static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t
   fp.omega_z_dot = ic->omega_z_dot_max;
   fp.gravity = ic->gravity;
   fp.min_section_time = ic->min_section_time;
+  fp.sampling_interval = sampling_interval;
   fp.B = B;
   fp.times = seg_times;
   fp.coeffs = coeffs;
@@ -1788,8 +1816,9 @@ static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t
   const int tpb = std::max(1, mtg::kExtremaThreads / K);
   const size_t smem = size_t(tpb) * K * sizeof(int);
   if (smem > h->smem_optin) {
-    h->error = recursive ? "mtg_input_feasibility_recursive_batch_f64: K too large"
-                         : "mtg_input_feasibility_batch_f64: K too large";
+    h->error = kind == FeasKind::Recursive  ? "mtg_input_feasibility_recursive_batch_f64: K too large"
+               : kind == FeasKind::Sampling ? "mtg_input_feasibility_sampling_batch_f64: K too large"
+                                            : "mtg_input_feasibility_batch_f64: K too large";
     return MTG_ERR_BAD_ARG;
   }
   typedef void (*FeasFn)(const mtg::FeasParams, const int);
@@ -1800,7 +1829,13 @@ static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t
       mtg::input_feasibility_recursive_kernel<4>, mtg::input_feasibility_recursive_kernel<6>,
       mtg::input_feasibility_recursive_kernel<8>, mtg::input_feasibility_recursive_kernel<10>,
       mtg::input_feasibility_recursive_kernel<12>};
-  const FeasFn fn = (recursive ? kFeasRec : kFeas)[N / 2 - 2];
+  static const FeasFn kFeasSampling[MTG_MAX_N / 2 - 1] = {
+      mtg::input_feasibility_sampling_kernel<4>, mtg::input_feasibility_sampling_kernel<6>,
+      mtg::input_feasibility_sampling_kernel<8>, mtg::input_feasibility_sampling_kernel<10>,
+      mtg::input_feasibility_sampling_kernel<12>};
+  const FeasFn fn = (kind == FeasKind::Recursive  ? kFeasRec
+                     : kind == FeasKind::Sampling ? kFeasSampling
+                                                  : kFeas)[N / 2 - 2];
   MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
   const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
   fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(fp, tpb);
@@ -1825,7 +1860,18 @@ int mtg_input_feasibility_recursive_batch_f64(mtg_handle* h, int32_t N, int32_t 
                                               int32_t* segment, int32_t* status, void* stream) {
   return run_entry(h, valid_feasibility(N, K, D, B, seg_times, coeffs, constraints, result), B, [&] {
     return launch_input_feasibility(h, N, K, D, B, seg_times, coeffs, constraints, result, segment, status,
-                                    (cudaStream_t)stream, true);
+                                    (cudaStream_t)stream, FeasKind::Recursive);
+  });
+}
+
+// FeasibilitySampling: the analytic entry's arguments, sampling_interval instead of min_section_time
+int mtg_input_feasibility_sampling_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                             const double* seg_times, const double* coeffs,
+                                             const mtg_input_constraints* constraints, double sampling_interval,
+                                             int32_t* result, int32_t* segment, int32_t* status, void* stream) {
+  return run_entry(h, valid_sampling(N, K, D, B, seg_times, coeffs, constraints, sampling_interval, result), B, [&] {
+    return launch_input_feasibility(h, N, K, D, B, seg_times, coeffs, constraints, result, segment, status,
+                                    (cudaStream_t)stream, FeasKind::Sampling, sampling_interval);
   });
 }
 
@@ -2079,7 +2125,25 @@ int mtg_input_feasibility_recursive_batch_host_f64(mtg_handle* h, int32_t N, int
                             {nullptr, segment, 4},
                             {nullptr, status, 4}};
     return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
-      return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s, true);
+      return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s,
+                                      FeasKind::Recursive);
+    });
+  });
+}
+
+int mtg_input_feasibility_sampling_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                                  const double* seg_times, const double* coeffs,
+                                                  const mtg_input_constraints* constraints, double sampling_interval,
+                                                  int32_t* result, int32_t* segment, int32_t* status) {
+  return run_entry(h, valid_sampling(N, K, D, B, seg_times, coeffs, constraints, sampling_interval, result), B, [&] {
+    const HostBuf bufs[] = {{seg_times, nullptr, size_t(K) * 8},
+                            {coeffs, nullptr, size_t(K) * D * N * 8},
+                            {nullptr, result, 4},
+                            {nullptr, segment, 4},
+                            {nullptr, status, 4}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
+      return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s,
+                                      FeasKind::Sampling, sampling_interval);
     });
   });
 }

@@ -51,6 +51,7 @@ struct FeasParams {
   unsigned present;
   double f_min, f_max, v_max, omega_xy, omega_z, omega_z_dot;
   double gravity, min_section_time;
+  double sampling_interval;  // FeasibilitySampling only
   long long B;
   const double* __restrict__ times;   // [B][K]
   const double* __restrict__ coeffs;  // [B][K][D][N]
@@ -207,22 +208,25 @@ __device__ int feas_segment(const double* __restrict__ c, double T, const FeasPa
 
 // The tile loop of the feasibility kernels.  Work item = (trajectory, segment), as max_magnitude_kernel: each
 // segment's code goes to shared memory, then one thread per trajectory takes the first segment whose code is not 0.
-// segment_code(item, T) checks one segment with a good time T (item = trajectory * K + segment) and returns 0 when it
-// passes; row(traj, bad, seg, code) writes one trajectory's outputs: bad when some segment time is <= 0 or non-finite
-// (seg = -1, code = 0 then), else the first failing segment and its code, or seg = -1 and code = 0.
+// W consecutive threads share one work item (W = 1: a thread per segment; W = 32: a warp per segment, every lane
+// calling segment_code with the same arguments and lane 0 storing its code).  segment_code(item, T) checks one segment
+// with a good time T (item = trajectory * K + segment) and returns 0 when it passes; row(traj, bad, seg, code) writes
+// one trajectory's outputs: bad when some segment time is <= 0 or non-finite (seg = -1, code = 0 then), else the first
+// failing segment and its code, or seg = -1 and code = 0.
 // dynamic shared memory: [tpb * K] codes
-template <typename SegmentCode, typename Row>
+template <int W = 1, typename SegmentCode, typename Row>
 __device__ __forceinline__ void first_failing_segment(long long B, int K, const double* __restrict__ times, int tpb,
                                                       SegmentCode&& segment_code, Row&& row) {
   extern __shared__ int feas_sm[];
   for (long long t0 = (long long)blockIdx.x * tpb; t0 < B; t0 += (long long)gridDim.x * tpb) {
     const int ntraj = int(B - t0 < tpb ? B - t0 : tpb);
     const int items = ntraj * K;
-    for (int it = threadIdx.x; it < items; it += blockDim.x) {
+    for (int it = threadIdx.x / W; it < items; it += blockDim.x / W) {
       const long long item = t0 * K + it;
       const double T = times[item];
       const bool bad = !(T > 0.0) || !isfinite(T);
-      feas_sm[it] = bad ? 0 : segment_code(item, T);
+      const int code = bad ? 0 : segment_code(item, T);
+      if (threadIdx.x % W == 0) feas_sm[it] = code;
     }
     __syncthreads();
     for (int lt = threadIdx.x; lt < ntraj; lt += blockDim.x) {
@@ -431,6 +435,173 @@ __global__ void __launch_bounds__(kExtremaThreads, 1)
   first_failing_segment(
       prm.B, prm.K, prm.times, tpb,
       [&](long long item, double T) { return feas_rec_segment<N>(prm.coeffs + item * prm.D * N, T, prm); },
+      [&](long long traj, bool bad, int seg, int code) { feas_row(prm, traj, bad, seg, code); });
+}
+
+// ---- FeasibilitySampling::checkInputFeasibility (reference mav_trajectory_generation_ros/src/
+// feasibility_sampling.cpp) ------------------------------------------------------------------------------------------
+// The samples are t = 0, fl(t + dt), ... while t <= T: the reference's running fp64 sum, not k * dt.  At each sample
+// the flat state (velocity, acceleration and jerk of dims 0..2; for D = 4 yaw, yaw rate and yaw acceleration of dim 3,
+// else 0) goes through mav_msgs' EigenMavStateFromEigenTrajectoryPoint:
+//   f = a + (0, 0, g), thrust = |f|, zb = f * (1 / thrust), xc = (cos yaw, sin yaw, 0), yb = normalized(zb x xc),
+//   xb = yb x zb, acceleration_B = R^T (zb * thrust) with R = [xb yb zb], h = (1 / thrust) (j - (zb . j) zb),
+//   omega_B = (-h . yb, h . xb, yaw_rate zb_z), omega_dot_B,z = yaw_acc zb_z,
+// and the reference's checks run in order: |acceleration_B| against f_min, f_max (only when one of them is present),
+// |v| against v_max, |omega_B,xy|, |omega_B,z|, |omega_dot_B,z|.  Yaw goes through setFromYaw / getYaw (a quaternion
+// about z and atan2 back).  Every operation is rounded on its own (no contraction), dot products and squared norms sum
+// in index order.  A thrust of exactly 0 makes the state NaN, and NaN passes every comparison, as in the reference.
+
+constexpr double kFeasSampleCap = 16777216.0;  // 2^24: a segment with fl(T / dt) above it is not sampled
+constexpr int kFeasHoist = 12;  // hoisted coefficient rows per warp: (dims 0..2) x (orders 1..3), then yaw orders 0..2
+
+// fl(B(k, j) c_j) of dim d, order k at row (d < 3 ? 3 d + k - 1 : 9 + k); Horner over them is Polynomial::evaluate's
+template <int N>
+__device__ __forceinline__ int feas_hoist_row(int d, int k) {
+  return (d < 3 ? 3 * d + k - 1 : 9 + k) * N;
+}
+
+template <int N, int K>
+__device__ __forceinline__ double feas_hoisted_horner(const double* __restrict__ h, double t) {
+  double acc = h[N - 1];
+#pragma unroll
+  for (int j = N - 2; j >= K; --j) acc = __dadd_rn(__dmul_rn(acc, t), h[j]);
+  return acc;
+}
+
+struct FeasVec3 {
+  double x, y, z;
+};
+__device__ __forceinline__ double feas_dot(const FeasVec3& a, const FeasVec3& b) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y)), __dmul_rn(a.z, b.z));
+}
+__device__ __forceinline__ FeasVec3 feas_cross(const FeasVec3& a, const FeasVec3& b) {
+  return {__dsub_rn(__dmul_rn(a.y, b.z), __dmul_rn(a.z, b.y)), __dsub_rn(__dmul_rn(a.z, b.x), __dmul_rn(a.x, b.z)),
+          __dsub_rn(__dmul_rn(a.x, b.y), __dmul_rn(a.y, b.x))};
+}
+__device__ __forceinline__ FeasVec3 feas_scale(double s, const FeasVec3& a) {
+  return {__dmul_rn(s, a.x), __dmul_rn(s, a.y), __dmul_rn(s, a.z)};
+}
+
+// The check of one sample at time t: 0 (passes) or a FeasResult.  h: this segment's hoisted products.  Only what a
+// present limit needs is evaluated.
+template <int N>
+__device__ __forceinline__ int feas_sample(const double* __restrict__ h, double t, const FeasParams& prm) {
+  const unsigned pr = prm.present;
+  const bool yaw4 = prm.D == 4;
+  const bool thrust_check = (pr & (kFeasFMin | kFeasFMax)) != 0;
+  const bool need_r = thrust_check || (pr & kFeasOmegaXY);
+  double thrust = 0.0, inv = 0.0;
+  FeasVec3 zb = {0.0, 0.0, 0.0}, yb = zb, xb = zb;
+  if (need_r || (yaw4 && (pr & (kFeasOmegaZ | kFeasOmegaZDot)))) {
+    const FeasVec3 f = {feas_hoisted_horner<N, 2>(h + feas_hoist_row<N>(0, 2), t),
+                        feas_hoisted_horner<N, 2>(h + feas_hoist_row<N>(1, 2), t),
+                        __dadd_rn(feas_hoisted_horner<N, 2>(h + feas_hoist_row<N>(2, 2), t), prm.gravity)};
+    thrust = __dsqrt_rn(feas_dot(f, f));
+    inv = __ddiv_rn(1.0, thrust);
+    zb = feas_scale(inv, f);
+  }
+  if (need_r) {
+    double cy = 1.0, sy = 0.0;  // D = 3: yaw 0
+    if (yaw4) {                 // setFromYaw, then getYaw: atan2(2 (w z + x y), 1 - 2 (y y + z z)) with x = y = 0
+      double qz, qw;
+      sincos(__dmul_rn(0.5, feas_hoisted_horner<N, 0>(h + feas_hoist_row<N>(3, 0), t)), &qz, &qw);
+      const double yaw = atan2(__dmul_rn(2.0, __dadd_rn(__dmul_rn(qw, qz), __dmul_rn(0.0, 0.0))),
+                               __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(__dmul_rn(0.0, 0.0), __dmul_rn(qz, qz)))));
+      sincos(yaw, &sy, &cy);
+    }
+    yb = feas_cross(zb, {cy, sy, 0.0});
+    const double n2 = feas_dot(yb, yb);
+    if (n2 > 0.0) {  // Eigen's normalized(): a zero vector stays as it is
+      const double n = __dsqrt_rn(n2);
+      yb = {__ddiv_rn(yb.x, n), __ddiv_rn(yb.y, n), __ddiv_rn(yb.z, n)};
+    }
+    xb = feas_cross(yb, zb);
+  }
+  if (thrust_check) {
+    const FeasVec3 w = feas_scale(thrust, zb), ab = {feas_dot(xb, w), feas_dot(yb, w), feas_dot(zb, w)};
+    const double thrust_b = __dsqrt_rn(feas_dot(ab, ab));
+    if ((pr & kFeasFMin) && thrust_b < prm.f_min) return kFeasThrustLow;
+    if ((pr & kFeasFMax) && thrust_b > prm.f_max) return kFeasThrustHigh;
+  }
+  if (pr & kFeasVMax) {
+    const FeasVec3 v = {feas_hoisted_horner<N, 1>(h + feas_hoist_row<N>(0, 1), t),
+                        feas_hoisted_horner<N, 1>(h + feas_hoist_row<N>(1, 1), t),
+                        feas_hoisted_horner<N, 1>(h + feas_hoist_row<N>(2, 1), t)};
+    if (__dsqrt_rn(feas_dot(v, v)) > prm.v_max) return kFeasVelocity;
+  }
+  if (pr & kFeasOmegaXY) {
+    const FeasVec3 j = {feas_hoisted_horner<N, 3>(h + feas_hoist_row<N>(0, 3), t),
+                        feas_hoisted_horner<N, 3>(h + feas_hoist_row<N>(1, 3), t),
+                        feas_hoisted_horner<N, 3>(h + feas_hoist_row<N>(2, 3), t)};
+    const double zj = feas_dot(zb, j);
+    const FeasVec3 hw = feas_scale(inv, {__dsub_rn(j.x, __dmul_rn(zj, zb.x)), __dsub_rn(j.y, __dmul_rn(zj, zb.y)),
+                                         __dsub_rn(j.z, __dmul_rn(zj, zb.z))});
+    const double wx = -feas_dot(hw, yb), wy = feas_dot(hw, xb);
+    if (__dsqrt_rn(__dadd_rn(__dmul_rn(wx, wx), __dmul_rn(wy, wy))) > prm.omega_xy) return kFeasRollPitchRates;
+  }
+  // D = 3: yaw rate and acceleration are 0, and 0 * zb_z never exceeds a limit >= 0
+  if (yaw4 && (pr & kFeasOmegaZ) &&
+      fabs(__dmul_rn(feas_hoisted_horner<N, 1>(h + feas_hoist_row<N>(3, 1), t), zb.z)) > prm.omega_z)
+    return kFeasYawRates;
+  if (yaw4 && (pr & kFeasOmegaZDot) &&
+      fabs(__dmul_rn(feas_hoisted_horner<N, 2>(h + feas_hoist_row<N>(3, 2), t), zb.z)) > prm.omega_z_dot)
+    return kFeasYawAcc;
+  return kFeasFeasible;
+}
+
+// The check of one segment (time T > 0 and finite) by one warp: every lane returns the same FeasResult, or
+// Indeterminable | kFeasCapacity when fl(T / dt) > 2^24.  The warp first stores the hoisted products fl(B(k, j) c_j) in
+// h (kFeasHoist N doubles, rows beyond D unused), then walks the samples in chunks of 32: every lane carries the same
+// running sum and keeps the value after `lane` additions, so the times are the reference's bit for bit.  A ballot over
+// the chunk's codes gives the first failing sample; a chunk that reaches past T is the last one.  Under the cap the sum
+// always advances: dt >= T 2^-24, far above the rounding unit of any t <= T.
+template <int N>
+__device__ int feas_sampling_segment(const double* __restrict__ c, double T, double* __restrict__ h,
+                                     const FeasParams& prm) {
+  if (prm.D != 3 && prm.D != 4) return kFeasIndeterminable;
+  const double dt = prm.sampling_interval;
+  if (__ddiv_rn(T, dt) > kFeasSampleCap) return kFeasIndeterminable | kFeasCapacity;
+  const int lane = threadIdx.x & 31;
+  const int rows = prm.D == 4 ? kFeasHoist : 9;
+  for (int q = lane; q < rows * N; q += 32) {
+    const int r = q / N, j = q - r * N;
+    const int d = r < 9 ? r / 3 : 3, k = r < 9 ? r % 3 + 1 : r - 9;
+    double b = 1.0;  // B(k, j) = j! / (j - k)!, an exact integer
+    for (int w = 0; w < k; ++w) b *= double(j - w);
+    h[q] = j < k ? 0.0 : __dmul_rn(b, c[d * N + j]);
+  }
+  __syncwarp();
+  double s = 0.0;  // the running sum at the chunk's first sample
+  int code = kFeasFeasible;
+  while (true) {
+    double t = 0.0;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      if (i == lane) t = s;
+      s = __dadd_rn(s, dt);
+    }
+    const bool in = t <= T;
+    const int mine = in ? feas_sample<N>(h, t, prm) : int(kFeasFeasible);
+    const unsigned fail = __ballot_sync(0xffffffffu, mine != kFeasFeasible);
+    if (fail) {
+      code = __shfl_sync(0xffffffffu, mine, __ffs(fail) - 1);
+      break;
+    }
+    if (__ballot_sync(0xffffffffu, !in)) break;
+  }
+  __syncwarp();  // h is rewritten by the warp's next segment
+  return code;
+}
+
+// One warp per (trajectory, segment) runs feas_sampling_segment; the first segment that is not Feasible decides.
+template <int N>
+__global__ void __launch_bounds__(kExtremaThreads, 1)
+    input_feasibility_sampling_kernel(const FeasParams prm, const int tpb) {
+  __shared__ double hoist[kExtremaThreads / 32][kFeasHoist * N];
+  double* __restrict__ h = hoist[threadIdx.x / 32];
+  first_failing_segment<32>(
+      prm.B, prm.K, prm.times, tpb,
+      [&](long long item, double T) { return feas_sampling_segment<N>(prm.coeffs + item * prm.D * N, T, h, prm); },
       [&](long long traj, bool bad, int seg, int code) { feas_row(prm, traj, bad, seg, code); });
 }
 

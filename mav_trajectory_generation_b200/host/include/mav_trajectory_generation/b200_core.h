@@ -121,11 +121,14 @@ class BatchCore {
   // PolynomialOptimizationNonLinear::scaleSegmentTimesWithViolation: solve at times_, stretch times_, re-solve into
   // coeffs_ with d_fixed_; status_ receives the OR of the three steps' status bits
   bool scaleSegmentTimesWithViolation(double v_max, double a_max, std::vector<uint8_t>* within_range);
-  // FeasibilityAnalytic (recursive: FeasibilityRecursive) ::checkInputFeasibilityTrajectory of the current
-  // coefficients (result, segment: [B]; segment nullable, -1 where the row is feasible or has a bad segment time)
-  bool checkInputFeasibility(const InputConstraints& constraints, double min_section_time, double gravity,
+  // which reference checker checkInputFeasibility runs
+  enum class InputChecker { kAnalytic, kRecursive, kSampling };
+  // FeasibilityAnalytic, FeasibilityRecursive or FeasibilitySampling ::checkInputFeasibilityTrajectory of the current
+  // coefficients (result, segment: [B]; segment nullable, -1 where the row is feasible or has a bad segment time).
+  // interval is the checker's Settings value, min_section_time or the sampling interval; its abs() is taken.
+  bool checkInputFeasibility(const InputConstraints& constraints, double interval, double gravity,
                              std::vector<InputFeasibilityResult>* result, std::vector<int>* segment,
-                             bool recursive = false) const;
+                             InputChecker checker = InputChecker::kAnalytic) const;
   // FeasibilityBase::checkHalfPlaneFeasibility of the current coefficients (feasible, segment, plane: [B]; segment and
   // plane nullable, -1 where the row is feasible or has a bad segment time)
   bool checkHalfPlaneFeasibility(const HalfPlane::Vector& planes, std::vector<uint8_t>* feasible,

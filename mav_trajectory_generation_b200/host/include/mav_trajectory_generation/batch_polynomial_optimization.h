@@ -120,7 +120,18 @@ class BatchPolynomialOptimization {
   bool checkInputFeasibilityRecursive(const InputConstraints& constraints, double min_section_time,
                                       std::vector<InputFeasibilityResult>* result, std::vector<int>* segment = nullptr,
                                       double gravity = kGravity) const {
-    return core_.checkInputFeasibility(constraints, min_section_time, gravity, result, segment, true);
+    return core_.checkInputFeasibility(constraints, min_section_time, gravity, result, segment,
+                                       b200::BatchCore::InputChecker::kRecursive);
+  }
+  // FeasibilitySampling::checkInputFeasibilityTrajectory (reference mav_trajectory_generation_ros/src/
+  // feasibility_sampling.cpp) of every trajectory at its current coefficients, on the GPU, with the outputs of
+  // checkInputFeasibility.  sampling_interval is FeasibilitySampling::Settings' (its abs() is taken; 0 is refused).  A
+  // segment that would need more than 2^24 samples is Indeterminable.
+  bool checkInputFeasibilitySampling(const InputConstraints& constraints, double sampling_interval,
+                                     std::vector<InputFeasibilityResult>* result, std::vector<int>* segment = nullptr,
+                                     double gravity = kGravity) const {
+    return core_.checkInputFeasibility(constraints, sampling_interval, gravity, result, segment,
+                                       b200::BatchCore::InputChecker::kSampling);
   }
   // FeasibilityBase::checkHalfPlaneFeasibility (reference mav_trajectory_generation_ros/src/feasibility_base.cpp) of
   // every trajectory at its current coefficients against one set of at most MTG_MAX_HALF_PLANES planes, on the GPU:

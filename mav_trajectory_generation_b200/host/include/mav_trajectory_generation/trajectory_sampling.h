@@ -60,6 +60,40 @@ struct EigenTrajectoryPoint {
 };
 typedef std::vector<EigenTrajectoryPoint> EigenTrajectoryPointVector;
 
+// mav_msgs::EigenMavState (mav_msgs/eigen_mav_msgs.h), mirrored as a plain struct like EigenTrajectoryPoint with the
+// fields the conversion below fills: world-frame position and velocity, body-frame acceleration (the thrust direction
+// scaled by its magnitude), body-frame angular velocity and acceleration.  The orientation is not mirrored.
+struct EigenMavState {
+  Eigen::Vector3d position_W, velocity_W, acceleration_B;
+  Eigen::Vector3d angular_velocity_B, angular_acceleration_B;
+};
+
+// mav_msgs' EigenMavStateFromEigenTrajectoryPoint (mav_msgs/conversions.h), the flat-state to full-state map of
+// Mellinger and Kumar (2011) restated here, not checked against mav_msgs:
+//   f = a + (0, 0, g), thrust = |f|, zb = f * (1 / thrust), xc = (cos yaw, sin yaw, 0), yb = normalized(zb x xc),
+//   xb = yb x zb, acceleration_B = R^T (zb thrust) with R = [xb yb zb], h = (1 / thrust) (j - (zb . j) zb),
+//   angular_velocity_B = (-h . yb, h . xb, yaw_rate zb_z), angular_acceleration_B = (0, 0, yaw_acc zb_z)
+// with yaw = flat_state.getYaw().  Only the z components of the angular acceleration are part of the restatement; x and
+// y are left 0.  A thrust of exactly 0 gives a NaN state.
+inline void EigenMavStateFromEigenTrajectoryPoint(const EigenTrajectoryPoint& flat_state, double gravity,
+                                                  EigenMavState* state) {
+  const double yaw = flat_state.getYaw();
+  const Eigen::Vector3d xc(std::cos(yaw), std::sin(yaw), 0.0);
+  Eigen::Vector3d f = flat_state.acceleration_W;
+  f[2] += gravity;
+  const double thrust = f.norm(), inv = 1.0 / thrust;
+  const Eigen::Vector3d zb = f * inv;
+  const Eigen::Vector3d yb = zb.cross(xc).normalized();
+  const Eigen::Vector3d xb = yb.cross(zb);
+  const Eigen::Vector3d w = zb * thrust;
+  state->position_W = flat_state.position_W;
+  state->velocity_W = flat_state.velocity_W;
+  state->acceleration_B = Eigen::Vector3d(xb.dot(w), yb.dot(w), zb.dot(w));
+  const Eigen::Vector3d h = (flat_state.jerk_W - zb * zb.dot(flat_state.jerk_W)) * inv;
+  state->angular_velocity_B = Eigen::Vector3d(-h.dot(yb), h.dot(xb), flat_state.getYawRate() * zb[2]);
+  state->angular_acceleration_B = Eigen::Vector3d(0.0, 0.0, flat_state.getYawAcc() * zb[2]);
+}
+
 }  // namespace mav_msgs
 
 namespace mav_trajectory_generation {

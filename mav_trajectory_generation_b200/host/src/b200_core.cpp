@@ -646,9 +646,9 @@ typedef int (*InputFeasibilityEntry)(mtg_handle*, int32_t, int32_t, int32_t, int
                                      const mtg_input_constraints*, int32_t*, int32_t*, int32_t*);
 }
 
-bool BatchCore::checkInputFeasibility(const InputConstraints& constraints, double min_section_time, double gravity,
+bool BatchCore::checkInputFeasibility(const InputConstraints& constraints, double interval, double gravity,
                                       std::vector<InputFeasibilityResult>* result, std::vector<int>* segment,
-                                      bool recursive) const {
+                                      InputChecker checker) const {
   CHECK_GT(B_, 0u) << "setup first";
   CHECK_NOTNULL(result);
   mtg_input_constraints ic = {};
@@ -656,16 +656,27 @@ bool BatchCore::checkInputFeasibility(const InputConstraints& constraints, doubl
   for (int q = 0; q < 6; ++q)
     if (constraints.getConstraint(q, values[q])) ic.present |= 1u << q;  // InputConstraintType order
   ic.gravity = gravity;
-  ic.min_section_time = std::abs(min_section_time);  // Settings::setMinSectionTimeS
-  const InputFeasibilityEntry entry =
-      recursive ? mtg_input_feasibility_recursive_batch_host_f64 : mtg_input_feasibility_batch_host_f64;
-  const char* name =
-      recursive ? "mtg_input_feasibility_recursive_batch_host_f64" : "mtg_input_feasibility_batch_host_f64";
+  // Settings::setMinSectionTimeS / setSamplingIntervalS
+  const double setting = std::abs(interval);
   std::vector<int32_t> res(B_, 0), seg(B_, -1);
   HandleLock lock;
   mtg_handle* h = defaultHandle();
-  const int rc = entry(h, N_, topo_.K, topo_.D, static_cast<int64_t>(B_), times_, coeffs_, &ic, res.data(), seg.data(),
-                       nullptr);
+  const int64_t B = static_cast<int64_t>(B_);
+  const char* name;
+  int rc;
+  if (checker == InputChecker::kSampling) {
+    name = "mtg_input_feasibility_sampling_batch_host_f64";
+    ic.min_section_time = 0.05;  // not read by the sampling check
+    rc = mtg_input_feasibility_sampling_batch_host_f64(h, N_, topo_.K, topo_.D, B, times_, coeffs_, &ic, setting,
+                                                       res.data(), seg.data(), nullptr);
+  } else {
+    const bool recursive = checker == InputChecker::kRecursive;
+    const InputFeasibilityEntry entry =
+        recursive ? mtg_input_feasibility_recursive_batch_host_f64 : mtg_input_feasibility_batch_host_f64;
+    name = recursive ? "mtg_input_feasibility_recursive_batch_host_f64" : "mtg_input_feasibility_batch_host_f64";
+    ic.min_section_time = setting;
+    rc = entry(h, N_, topo_.K, topo_.D, B, times_, coeffs_, &ic, res.data(), seg.data(), nullptr);
+  }
   if (rc != MTG_OK) {
     LOG(ERROR) << name << " failed (rc=" << rc << "): " << mtg_last_error(h);
     return false;

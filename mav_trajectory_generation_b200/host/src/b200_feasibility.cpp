@@ -1,14 +1,18 @@
 // b200_feasibility.cpp -- InputConstraints, FeasibilityBase::checkInputFeasibilityTrajectory,
-// FeasibilityAnalytic::checkInputFeasibility and FeasibilityRecursive::checkInputFeasibility for one segment on the
-// host (reference mav_trajectory_generation_ros/src/input_constraints.cpp, feasibility_base.cpp,
-// feasibility_analytic.cpp, feasibility_recursive.cpp), on the extremum candidates and roots of b200_extrema.cpp.  The
-// batched GPU forms are mtg_input_feasibility_batch_f64 and mtg_input_feasibility_recursive_batch_f64.
+// FeasibilityAnalytic::checkInputFeasibility, FeasibilityRecursive::checkInputFeasibility and
+// FeasibilitySampling::checkInputFeasibility for one segment on the host (reference
+// mav_trajectory_generation_ros/src/input_constraints.cpp, feasibility_base.cpp, feasibility_analytic.cpp,
+// feasibility_recursive.cpp, feasibility_sampling.cpp), on the extremum candidates and roots of b200_extrema.cpp.  The
+// batched GPU forms are mtg_input_feasibility_batch_f64, mtg_input_feasibility_recursive_batch_f64 and
+// mtg_input_feasibility_sampling_batch_f64.
 #include <algorithm>
 #include <cmath>
 #include <limits>
 
 #include "mav_trajectory_generation_ros/feasibility_analytic.h"
 #include "mav_trajectory_generation_ros/feasibility_recursive.h"
+#include "mav_trajectory_generation_ros/feasibility_sampling.h"
+#include "mav_trajectory_generation/trajectory_sampling.h"
 
 namespace mav_trajectory_generation {
 
@@ -342,6 +346,54 @@ double FeasibilityRecursive::evaluateThrust(const Segment& segment, double time)
   double sq = 0.0;
   for (int i = 0; i < 3; ++i) sq += square(a[i] + gravity_[i]);
   return std::sqrt(sq);
+}
+
+}  // namespace mav_trajectory_generation
+
+// ---- FeasibilitySampling (reference src/feasibility_sampling.cpp) ---------------------------------------------------
+
+namespace mav_trajectory_generation {
+
+InputFeasibilityResult FeasibilitySampling::checkInputFeasibility(const Segment& segment) const {
+  if (segment.D() != 3 && segment.D() != 4) return kInputIndeterminable;
+  const InputConstraints& ic = input_constraints_;
+  double f_min, f_max, v_max, omega_xy_max, omega_z_max, omega_z_dot_max;
+  const bool has_f_min = ic.getConstraint(kFMin, &f_min), has_f_max = ic.getConstraint(kFMax, &f_max);
+  const bool has_v_max = ic.getConstraint(kVMax, &v_max), has_omega_xy = ic.getConstraint(kOmegaXYMax, &omega_xy_max);
+  const bool has_omega_z = ic.getConstraint(kOmegaZMax, &omega_z_max);
+  const bool has_omega_z_dot = ic.getConstraint(kOmegaZDotMax, &omega_z_dot_max);
+  // the sample times are a running sum, as in the reference (T itself is missed when the sum overshoots it)
+  for (double t = 0.0; t <= segment.getTime(); t += settings_.getSamplingIntervalS()) {
+    const Eigen::VectorXd position = segment.evaluate(t, derivative_order::POSITION);
+    const Eigen::VectorXd velocity = segment.evaluate(t, derivative_order::VELOCITY);
+    const Eigen::VectorXd acc = segment.evaluate(t, derivative_order::ACCELERATION);
+    mav_msgs::EigenTrajectoryPoint flat_state;
+    sampling_detail::head3(position, &flat_state.position_W);
+    sampling_detail::head3(velocity, &flat_state.velocity_W);
+    sampling_detail::head3(acc, &flat_state.acceleration_W);
+    sampling_detail::head3(segment.evaluate(t, derivative_order::JERK), &flat_state.jerk_W);
+    flat_state.setFromYawRate(0.0);
+    flat_state.setFromYawAcc(0.0);
+    if (segment.D() == 4) {
+      flat_state.setFromYaw(position[3]);
+      flat_state.setFromYawRate(velocity[3]);
+      flat_state.setFromYawAcc(acc[3]);
+    }
+    mav_msgs::EigenMavState state;
+    mav_msgs::EigenMavStateFromEigenTrajectoryPoint(flat_state, gravity_[2], &state);
+    if (has_f_min || has_f_max) {
+      const double thrust = state.acceleration_B.norm();
+      if (has_f_min && thrust < f_min) return kInputInfeasibleThrustLow;
+      if (has_f_max && thrust > f_max) return kInputInfeasibleThrustHigh;
+    }
+    if (has_v_max && state.velocity_W.norm() > v_max) return kInputInfeasibleVelocity;
+    // roll / pitch and yaw rates assume independent axes (rigid-body model)
+    if (has_omega_xy && state.angular_velocity_B.head(2).norm() > omega_xy_max) return kInputInfeasibleRollPitchRates;
+    if (has_omega_z && std::fabs(state.angular_velocity_B[2]) > omega_z_max) return kInputInfeasibleYawRates;
+    if (has_omega_z_dot && std::fabs(state.angular_acceleration_B[2]) > omega_z_dot_max)
+      return kInputInfeasibleYawAcc;
+  }
+  return kInputFeasible;
 }
 
 }  // namespace mav_trajectory_generation
