@@ -391,6 +391,61 @@ int mtg_half_plane_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, in
                                          const mtg_half_plane* planes, int32_t* feasible, int32_t* segment,
                                          int32_t* plane, int32_t* status, void* stream);
 
+/* Flat states: mav_msgs::EigenTrajectoryPoint of sampleTrajectoryInRange, sampleWholeTrajectory and
+ * sampleTrajectoryAtTime (reference src/trajectory_sampling.cpp:27-110), one fixed record of MTG_FLAT_STATE_DOUBLES
+ * doubles per sample, fields at the offsets below:
+ *   position_W, velocity_W, acceleration_W, jerk_W, snap_W   dims 0..2 of derivatives 0..4 (Polynomial::evaluate's
+ *                                                            arithmetic: bit for bit mtg_evaluate_range_batch_f64's)
+ *   orientation (w, x, y, z), angular_velocity_W, angular_acceleration_W:
+ *     D = 4: setFromYaw / setFromYawRate / setFromYawAcc of dim 3: (cos y/2, 0, 0, sin y/2), (0, 0, y'), (0, 0, y'')
+ *     D = 6: the rotation vector phi of dims 3..5: orientation exp(phi) with w >= 0, angular velocity J(phi) phi' and
+ *            acceleration J phi'' + J' phi' (J the left Jacobian of SO(3)).  The reference converts through
+ *            Eigen::Quaterniond(Matrix3d), whose sign can make w < 0 past a rotation angle of 2 pi / 3: the same
+ *            rotation with the opposite sign.
+ *     other D >= 3: identity, zero angular terms.
+ * degrees_of_freedom is not stored: DOF6 when D = 6, DOF4 otherwise.  Trigonometry is the device's, a few ulps from
+ * glibc's. */
+#define MTG_FLAT_STATE_DOUBLES 25
+#define MTG_FLAT_STATE_POSITION 0
+#define MTG_FLAT_STATE_VELOCITY 3
+#define MTG_FLAT_STATE_ACCELERATION 6
+#define MTG_FLAT_STATE_JERK 9
+#define MTG_FLAT_STATE_SNAP 12
+#define MTG_FLAT_STATE_ORIENTATION 15
+#define MTG_FLAT_STATE_ANGULAR_VELOCITY 19
+#define MTG_FLAT_STATE_ANGULAR_ACCELERATION 22
+
+/* sampleTrajectoryInRange (whole = 0) / sampleWholeTrajectory (whole = 1) for B trajectories at once.  The samples are
+ * those of mtg_evaluate_range_batch_f64 over [min_time, max_time] (the reference's walk, replayed exactly); with
+ * whole = 1 min_time and max_time are not read and each row uses [0, its total time], the left-to-right sum of its
+ * segment times (Trajectory::getMaxTime).
+ *   states     [B][max_samples][MTG_FLAT_STATE_DOUBLES]   (records >= n_samples[b] are zero)
+ *   time_ns    [B][max_samples] int64 or NULL: (int64)((min_time + sampling_interval * s) * 1e9), each operation
+ *              rounded on its own, truncated toward zero (min_time = 0 when whole = 1); 0 past n_samples[b]
+ *   n_samples  [B]  the number of states the reference would produce (may exceed max_samples: only the first
+ *              max_samples are stored); -1 where the reference returns false: min_time < 0, max_time above the row's
+ *              total time, or D < 3 (every row).  A min_time beyond the trajectory gives 0 (the reference logs an error
+ *              and returns true with no states).
+ * N in [1, 12].  Refused (MTG_ERR_BAD_ARG, no launch): sampling_interval <= 0 or non-finite, max_samples < 0, K < 1,
+ * D < 1, B < 0, a null seg_times, coeffs or n_samples with B > 0, a null states with B > 0 and max_samples > 0. */
+int mtg_sample_flat_states_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                     const double* coeffs, double min_time, double max_time, double sampling_interval,
+                                     int32_t whole, int32_t max_samples, double* states, int64_t* time_ns,
+                                     int32_t* n_samples, void* stream);
+
+/* sampleTrajectoryAtTime for B trajectories, each at its own time sample_times[b] (B vehicles at one control tick).
+ * The segment follows Trajectory::evaluate (mtg_evaluate_batch_f64's conventions: a time on a vertex belongs to the
+ * segment on its right, the total time is the end of the last segment).
+ *   states   [B][MTG_FLAT_STATE_DOUBLES]
+ *   time_ns  [B] int64 or NULL: (int64)(t * 1e9)
+ *   ok       [B] 1, or 0 with a zero record and time stamp where the reference returns false: t outside [0, the row's
+ *            total time] (a NaN t included), or D < 3.
+ * N in [1, 12].  Refused (MTG_ERR_BAD_ARG, no launch): K < 1, D < 1, B < 0, a null seg_times, coeffs, sample_times, states
+ * or ok with B > 0. */
+int mtg_sample_flat_state_at_time_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                            const double* seg_times, const double* coeffs, const double* sample_times,
+                                            double* states, int64_t* time_ns, int32_t* ok, void* stream);
+
 /* ---- the hot path, HOST pointers (what PolynomialOptimization<N>::solveLinear() calls) ---- */
 /* Same contract with host buffers: each call refuses what its device entry refuses, before any copy, and
  * returns when the results are in the host buffers.  Pinned buffers (mtg_host_alloc) make the copies
@@ -448,6 +503,14 @@ int mtg_half_plane_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t 
                                               const double* seg_times, const double* coeffs, int32_t n_planes,
                                               const mtg_half_plane* planes, int32_t* feasible, int32_t* segment,
                                               int32_t* plane, int32_t* status);
+int mtg_sample_flat_states_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                          const double* seg_times, const double* coeffs, double min_time,
+                                          double max_time, double sampling_interval, int32_t whole, int32_t max_samples,
+                                          double* states, int64_t* time_ns, int32_t* n_samples);
+int mtg_sample_flat_state_at_time_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                                 const double* seg_times, const double* coeffs,
+                                                 const double* sample_times, double* states, int64_t* time_ns,
+                                                 int32_t* ok);
 
 /* ---- memory helpers (so host code above the ABI needs no CUDA headers) -------------------- */
 void* mtg_host_alloc(mtg_handle* h, uint64_t bytes);   /* pinned */

@@ -47,7 +47,9 @@ def _sources(d, exts):
 
 
 def build_cuda(force=False, verbose=False):
-    deps = _sources(CSRC, (".cu", ".cuh", ".h")) + [os.path.join(ROOT, "include", "mtg_b200.h")]
+    deps = _sources(CSRC, (".cu", ".cuh", ".h")) + [os.path.join(ROOT, "include", "mtg_b200.h"),
+                                                    os.path.join(HOST, "include", "mav_trajectory_generation",
+                                                                 "rotation_vector_kinematics.h")]
     if force or _newer(LIB_CUDA, deps):
         cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + \
               ["-o", LIB_CUDA, os.path.join(CSRC, "mtg_capi.cu")]

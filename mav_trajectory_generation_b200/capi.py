@@ -41,8 +41,17 @@ EXPORTED_SYMBOLS = [
     "mtg_input_feasibility_batch_host_f64", "mtg_half_plane_feasibility_batch_f64",
     "mtg_half_plane_feasibility_batch_host_f64", "mtg_input_feasibility_recursive_batch_f64",
     "mtg_input_feasibility_recursive_batch_host_f64", "mtg_input_feasibility_sampling_batch_f64",
-    "mtg_input_feasibility_sampling_batch_host_f64",
+    "mtg_input_feasibility_sampling_batch_host_f64", "mtg_sample_flat_states_batch_f64",
+    "mtg_sample_flat_state_at_time_batch_f64", "mtg_sample_flat_states_batch_host_f64",
+    "mtg_sample_flat_state_at_time_batch_host_f64",
 ]
+# mav_msgs::EigenTrajectoryPoint as one record of MTG_FLAT_STATE_DOUBLES doubles: the slice of each field
+FLAT_STATE_DOUBLES = 25
+FLAT_STATE_FIELDS = {
+    "position_W": slice(0, 3), "velocity_W": slice(3, 6), "acceleration_W": slice(6, 9), "jerk_W": slice(9, 12),
+    "snap_W": slice(12, 15), "orientation_W_B": slice(15, 19),  # (w, x, y, z)
+    "angular_velocity_W": slice(19, 22), "angular_acceleration_W": slice(22, 25),
+}
 TIME_COST_SQUARED, TIME_COST_RICHTER = 0, 1
 STATUS_FEAS_CAPACITY = 4
 # InputFeasibilityResult
@@ -265,6 +274,12 @@ def load():
                                                        C.POINTER(MtgHalfPlane), dp, dp, dp, dp, vp]
     L.mtg_half_plane_feasibility_batch_host_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp,
                                                             C.c_int32, C.POINTER(MtgHalfPlane), dp, dp, dp, dp]
+    L.mtg_sample_flat_states_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, dbl, dbl, dbl,
+                                                   C.c_int32, C.c_int32, dp, dp, dp, vp]
+    L.mtg_sample_flat_states_batch_host_f64.argtypes = L.mtg_sample_flat_states_batch_f64.argtypes[:-1]
+    L.mtg_sample_flat_state_at_time_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, dp, dp,
+                                                          dp, dp, vp]
+    L.mtg_sample_flat_state_at_time_batch_host_f64.argtypes = L.mtg_sample_flat_state_at_time_batch_f64.argtypes[:-1]
     for name in EXPORTED_SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export what the header declares
     _lib = L
@@ -423,6 +438,51 @@ class Solver:
                                                    st.data_ptr() if want_times else None, s)
         self._check(rc, "mtg_evaluate_range_batch_f64")
         return out, n, st
+
+    def sample_flat_states(self, seg_times, coeffs, min_time, max_time, sampling_interval, max_samples=None,
+                           stream=None, _whole=0):
+        """Batched sampleTrajectoryInRange: (states [B][S][FLAT_STATE_DOUBLES], time_ns [B][S] int64, n_samples [B]
+        int32).  Fields are the FLAT_STATE_FIELDS slices of the last axis; records past n_samples[b] are zero and
+        n_samples[b] is -1 where the reference returns false.  max_samples=None sizes S to the largest count, which
+        takes a counting pass and waits for it."""
+        import torch
+        B, K, D, N = coeffs.shape
+        s = stream if stream is not None else torch.cuda.current_stream(coeffs.device).cuda_stream
+        n = torch.empty((B,), dtype=torch.int32, device=coeffs.device)
+
+        def run(S, states, time_ns):
+            rc = self.lib.mtg_sample_flat_states_batch_f64(
+                self.h, N, K, D, B, seg_times.data_ptr(), coeffs.data_ptr(), float(min_time), float(max_time),
+                float(sampling_interval), int(_whole), int(S), states.data_ptr() if states is not None else None,
+                time_ns.data_ptr() if time_ns is not None else None, n.data_ptr(), s)
+            self._check(rc, "mtg_sample_flat_states_batch_f64")
+
+        if max_samples is None:
+            run(0, None, None)
+            max_samples = max(int(n.max().item()), 0) if B else 0
+        states = torch.empty((B, max_samples, FLAT_STATE_DOUBLES), dtype=torch.float64, device=coeffs.device)
+        time_ns = torch.empty((B, max_samples), dtype=torch.int64, device=coeffs.device)
+        run(max_samples, states, time_ns)
+        return states, time_ns, n
+
+    def sample_whole_trajectories(self, seg_times, coeffs, sampling_interval, max_samples=None, stream=None):
+        """Batched sampleWholeTrajectory: sample_flat_states over [0, each row's total time]."""
+        return self.sample_flat_states(seg_times, coeffs, 0.0, 0.0, sampling_interval, max_samples, stream, _whole=1)
+
+    def sample_flat_state_at_time(self, seg_times, coeffs, sample_times, stream=None):
+        """Batched sampleTrajectoryAtTime, row b at sample_times[b]: (states [B][FLAT_STATE_DOUBLES], time_ns [B] int64,
+        ok [B] int32; 0 with a zero record where the reference returns false)."""
+        import torch
+        B, K, D, N = coeffs.shape
+        states = torch.empty((B, FLAT_STATE_DOUBLES), dtype=torch.float64, device=coeffs.device)
+        time_ns = torch.empty((B,), dtype=torch.int64, device=coeffs.device)
+        ok = torch.empty((B,), dtype=torch.int32, device=coeffs.device)
+        s = stream if stream is not None else torch.cuda.current_stream(coeffs.device).cuda_stream
+        rc = self.lib.mtg_sample_flat_state_at_time_batch_f64(self.h, N, K, D, B, seg_times.data_ptr(),
+                                                              coeffs.data_ptr(), sample_times.data_ptr(),
+                                                              states.data_ptr(), time_ns.data_ptr(), ok.data_ptr(), s)
+        self._check(rc, "mtg_sample_flat_state_at_time_batch_f64")
+        return states, time_ns, ok
 
     def cost_gradient_mellinger(self, prob, seg_times, d_fixed, stream=None):
         """(cost [B], grad [B][K]) -- batched getCostAndGradientMellinger."""
@@ -651,6 +711,29 @@ class Solver:
             len(derivs), arr, int(out.shape[1]), self._hptr(out), self._hptr(n_samples), self._hptr(sampling_times))
         self._check(rc, "mtg_evaluate_range_batch_host_f64")
         return n_samples
+
+    def sample_flat_states_host(self, seg_times, coeffs, min_time, max_time, sampling_interval, states, n_samples,
+                                time_ns=None, whole=False):
+        """sample_flat_states (whole=True: sample_whole_trajectories) into host buffers: states
+        [B][max_samples][FLAT_STATE_DOUBLES], n_samples [B] int32, time_ns [B][max_samples] int64 or None
+        (max_samples is states.shape[1])."""
+        B, K, D, N = coeffs.shape
+        rc = self.lib.mtg_sample_flat_states_batch_host_f64(
+            self.h, N, K, D, B, self._hptr(seg_times), self._hptr(coeffs), float(min_time), float(max_time),
+            float(sampling_interval), int(bool(whole)), int(states.shape[1]), self._hptr(states), self._hptr(time_ns),
+            self._hptr(n_samples))
+        self._check(rc, "mtg_sample_flat_states_batch_host_f64")
+        return n_samples
+
+    def sample_flat_state_at_time_host(self, seg_times, coeffs, sample_times, states, ok, time_ns=None):
+        """sample_flat_state_at_time into host buffers: states [B][FLAT_STATE_DOUBLES], ok [B] int32, time_ns [B]
+        int64 or None."""
+        B, K, D, N = coeffs.shape
+        rc = self.lib.mtg_sample_flat_state_at_time_batch_host_f64(
+            self.h, N, K, D, B, self._hptr(seg_times), self._hptr(coeffs), self._hptr(sample_times),
+            self._hptr(states), self._hptr(time_ns), self._hptr(ok))
+        self._check(rc, "mtg_sample_flat_state_at_time_batch_host_f64")
+        return ok
 
     def max_magnitude_host(self, seg_times, coeffs, derivs, value, time=None, segment=None, status=None):
         B, K, D, N = coeffs.shape

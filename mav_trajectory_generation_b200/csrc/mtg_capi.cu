@@ -15,6 +15,7 @@
 #include "../../include/mtg_b200.h"
 #include "mtg_extrema_kernel.cuh"
 #include "mtg_feasibility_kernel.cuh"
+#include "mtg_flat_state_kernel.cuh"
 #include "mtg_generic_kernel.cuh"
 #include "mtg_half_plane_kernel.cuh"
 #include "mtg_twisted_kernel.cuh"
@@ -1065,6 +1066,29 @@ int stage_host(mtg_handle* h, int64_t B, Staging staging, const HostBuf (&bufs)[
   return MTG_OK;
 }
 
+// ---- flat-state kernel tables -------------------------------------------------------------------------------------
+int flat_attitude(int32_t D) { return D == 4 ? mtg::kAttYaw : D == 6 ? mtg::kAttRotationVector : mtg::kAttNone; }
+
+// kernel `Kern<N, ATT>` of every N in [1, 12] and attitude case, indexed [ATT][N - 1]
+template <template <int, int> class Kern, class Fn>
+Fn flat_state_kernel(int32_t N, int32_t D) {
+  static const Fn kTable[3][MTG_MAX_N] = {
+#define MTG_FLAT_ROW(A)                                                                                              \
+  {Kern<1, A>::fn, Kern<2, A>::fn, Kern<3, A>::fn, Kern<4, A>::fn,   Kern<5, A>::fn,  Kern<6, A>::fn,                \
+   Kern<7, A>::fn, Kern<8, A>::fn, Kern<9, A>::fn, Kern<10, A>::fn, Kern<11, A>::fn, Kern<12, A>::fn}
+      MTG_FLAT_ROW(mtg::kAttNone), MTG_FLAT_ROW(mtg::kAttYaw), MTG_FLAT_ROW(mtg::kAttRotationVector)};
+#undef MTG_FLAT_ROW
+  return kTable[flat_attitude(D)][N - 1];
+}
+template <int N, int ATT>
+struct FlatRangeKernel {
+  static constexpr void (*fn)(const mtg::RangeParams) = mtg::flat_state_range_kernel<N, ATT>;
+};
+template <int N, int ATT>
+struct FlatAtTimeKernel {
+  static constexpr void (*fn)(const mtg::FlatAtTimeParams) = mtg::flat_state_at_time_kernel<N, ATT>;
+};
+
 }  // namespace
 
 extern "C" {
@@ -1409,6 +1433,8 @@ static int launch_range(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t 
   rp.n_samples = n_samples;
   rp.sampling_times = sampling_times;
   rp.out = out;
+  rp.range_rule = mtg::kRangePlain;
+  rp.time_ns = nullptr;
   {
     const int threads = 128;
     const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
@@ -1452,6 +1478,107 @@ int mtg_evaluate_range_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D,
                                          max_samples, out, n_samples, sampling_times, (cudaStream_t)stream,
                                          mtg_handle::kPipe);
                    });
+}
+
+// ---- flat-state samplers ------------------------------------------------------------------------------------------
+static int64_t flat_state_blocks(mtg_handle* h, int64_t records) {
+  return std::min<int64_t>((records + mtg::kFlatStateThreads - 1) / mtg::kFlatStateThreads, int64_t(h->sm_count) * 16);
+}
+
+static bool valid_flat_range(int32_t N, int32_t K, int32_t D, int64_t B, double dt, int32_t max_samples, const double* seg_times,
+                             const double* coeffs, const double* states, const int32_t* n_samples) {
+  return N >= 1 && N <= MTG_MAX_N && K >= 1 && D >= 1 && max_samples >= 0 && dt > 0.0 && std::isfinite(dt) &&
+         valid_rows(B, {seg_times, coeffs, n_samples}) && (B == 0 || max_samples == 0 || states);
+}
+
+// range_walk_kernel under sampleTrajectoryInRange's rule, then flat_state_range_kernel
+static int launch_flat_range(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                             const double* coeffs, double min_time, double max_time, double dt, int32_t whole,
+                             int32_t max_samples, double* states, int64_t* time_ns, int32_t* n_samples, cudaStream_t s,
+                             int slot) {
+  const size_t ns = size_t(B) * size_t(std::max(max_samples, 1));
+  mtg_handle::Arena& ar = h->pack[slot];
+  const size_t o_idx = align_doubles(ns);  // t_local first (doubles), then seg_idx (int32)
+  MTG_TRY(arena_acquire(h, ar, (o_idx + align_doubles((ns + 1) / 2)) * 8, s));
+  mtg::RangeParams rp = {};
+  rp.N = N;
+  rp.K = K;
+  rp.D = D;
+  rp.max_samples = max_samples;
+  rp.B = B;
+  rp.t_start = min_time;
+  rp.t_end = max_time;
+  rp.dt = dt;
+  rp.times = seg_times;
+  rp.coeffs = coeffs;
+  rp.t_local = ar.p;
+  rp.seg_idx = reinterpret_cast<int*>(ar.p + o_idx);
+  rp.n_samples = n_samples;
+  rp.sampling_times = nullptr;
+  rp.out = states;
+  rp.range_rule = whole ? mtg::kRangeWhole : mtg::kRangeChecked;
+  rp.time_ns = reinterpret_cast<long long*>(time_ns);
+  {
+    const int threads = 128;
+    const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
+    mtg::range_walk_kernel<<<(unsigned)blocks, threads, 0, s>>>(rp);
+    MTG_CUDA(h, cudaGetLastError());
+    h->launches++;
+  }
+  if (max_samples > 0) {
+    typedef void (*Fn)(const mtg::RangeParams);
+    const Fn fn = flat_state_kernel<FlatRangeKernel, Fn>(N, D);
+    fn<<<(unsigned)flat_state_blocks(h, B * int64_t(max_samples)), mtg::kFlatStateThreads, 0, s>>>(rp);
+    MTG_CUDA(h, cudaGetLastError());
+    h->launches++;
+  }
+  return arena_release(h, ar, s);
+}
+
+int mtg_sample_flat_states_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                                     const double* coeffs, double min_time, double max_time, double sampling_interval,
+                                     int32_t whole, int32_t max_samples, double* states, int64_t* time_ns,
+                                     int32_t* n_samples, void* stream) {
+  return run_entry(
+      h, valid_flat_range(N, K, D, B, sampling_interval, max_samples, seg_times, coeffs, states, n_samples), B, [&] {
+        return launch_flat_range(h, N, K, D, B, seg_times, coeffs, min_time, max_time, sampling_interval, whole,
+                                 max_samples, states, time_ns, n_samples, (cudaStream_t)stream, mtg_handle::kPipe);
+      });
+}
+
+static int launch_flat_at_time(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
+                               const double* coeffs, const double* sample_times, double* states, int64_t* time_ns,
+                               int32_t* ok, cudaStream_t s) {
+  mtg::FlatAtTimeParams prm;
+  prm.K = K;
+  prm.D = D;
+  prm.B = B;
+  prm.times = seg_times;
+  prm.coeffs = coeffs;
+  prm.sample_times = sample_times;
+  prm.states = states;
+  prm.time_ns = reinterpret_cast<long long*>(time_ns);
+  prm.ok = ok;
+  typedef void (*Fn)(const mtg::FlatAtTimeParams);
+  const Fn fn = flat_state_kernel<FlatAtTimeKernel, Fn>(N, D);
+  fn<<<(unsigned)flat_state_blocks(h, B), mtg::kFlatStateThreads, 0, s>>>(prm);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  return MTG_OK;
+}
+
+static bool valid_flat_at_time(int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times, const double* coeffs,
+                               const double* sample_times, const double* states, const int32_t* ok) {
+  return N >= 1 && N <= MTG_MAX_N && K >= 1 && D >= 1 && valid_rows(B, {seg_times, coeffs, sample_times, states, ok});
+}
+
+int mtg_sample_flat_state_at_time_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                            const double* seg_times, const double* coeffs, const double* sample_times,
+                                            double* states, int64_t* time_ns, int32_t* ok, void* stream) {
+  return run_entry(h, valid_flat_at_time(N, K, D, B, seg_times, coeffs, sample_times, states, ok), B, [&] {
+    return launch_flat_at_time(h, N, K, D, B, seg_times, coeffs, sample_times, states, time_ns, ok,
+                               (cudaStream_t)stream);
+  });
 }
 
 static int launch_mellinger(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B,
@@ -2027,6 +2154,41 @@ int mtg_evaluate_range_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32
                                                              derivs, max_samples, d[2], d[3], d[4], s, slot);
                                        });
                    });
+}
+
+int mtg_sample_flat_states_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                          const double* seg_times, const double* coeffs, double min_time,
+                                          double max_time, double sampling_interval, int32_t whole, int32_t max_samples,
+                                          double* states, int64_t* time_ns, int32_t* n_samples) {
+  return run_entry(
+      h, valid_flat_range(N, K, D, B, sampling_interval, max_samples, seg_times, coeffs, states, n_samples), B, [&] {
+        const HostBuf bufs[] = {{seg_times, nullptr, size_t(K) * 8},
+                                {coeffs, nullptr, size_t(K) * D * N * 8},
+                                {nullptr, states, size_t(max_samples) * MTG_FLAT_STATE_DOUBLES * 8},
+                                {nullptr, time_ns, size_t(max_samples) * 8},
+                                {nullptr, n_samples, 4}};
+        return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+          return launch_flat_range(h, N, K, D, nb, d[0], d[1], min_time, max_time, sampling_interval, whole,
+                                   max_samples, d[2], d[3], d[4], s, slot);
+        });
+      });
+}
+
+int mtg_sample_flat_state_at_time_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
+                                                 const double* seg_times, const double* coeffs,
+                                                 const double* sample_times, double* states, int64_t* time_ns,
+                                                 int32_t* ok) {
+  return run_entry(h, valid_flat_at_time(N, K, D, B, seg_times, coeffs, sample_times, states, ok), B, [&] {
+    const HostBuf bufs[] = {{seg_times, nullptr, size_t(K) * 8},
+                            {coeffs, nullptr, size_t(K) * D * N * 8},
+                            {sample_times, nullptr, 8},
+                            {nullptr, states, size_t(MTG_FLAT_STATE_DOUBLES) * 8},
+                            {nullptr, time_ns, 8},
+                            {nullptr, ok, 4}};
+    return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
+      return launch_flat_at_time(h, N, K, D, nb, d[0], d[1], d[2], d[3], d[4], d[5], s);
+    });
+  });
 }
 
 int mtg_max_magnitude_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,

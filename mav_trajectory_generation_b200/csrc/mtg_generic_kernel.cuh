@@ -414,7 +414,15 @@ struct RangeParams {
   int* __restrict__ n_samples;         // [B]; -1: t_start beyond the trajectory (reference logs an error, no samples)
   double* __restrict__ sampling_times; // [B][max_samples] or null
   double* __restrict__ out;            // [B][max_samples][n_derivs][D]
+  // sampleTrajectoryInRange's rule around the walk (flat-state samplers only; kRangePlain for evaluateRange)
+  int range_rule;
+  long long* __restrict__ time_ns;     // flat-state samplers: [B][max_samples] or null
 };
+// kRangeChecked: n = -1 where t_start < 0, t_end exceeds the row's total time (the left-to-right sum of its segment
+// times, Trajectory::max_time_) or D < 3; a t_start beyond the trajectory gives 0 samples (the reference's
+// evaluateRange logs an error and sampleTrajectoryInRange still succeeds).  kRangeWhole: the same over [0, the row's
+// total] (sampleWholeTrajectory), t_start and t_end are not read.
+enum RangeRule { kRangePlain = 0, kRangeChecked = 1, kRangeWhole = 2 };
 
 // The walk is sequential per trajectory (the reference accumulates `+= dt`), so a thread owns a trajectory; its samples
 // are parked in shared memory 16 at a time and leave as row-contiguous runs written by half-warps (a lane storing its
@@ -434,27 +442,40 @@ __global__ void __launch_bounds__(128) range_walk_kernel(const RangeParams prm) 
     bool done = b >= prm.B;
     const double* __restrict__ tt = prm.times + (done ? 0 : b) * K;
     double accumulated = 0.0, Ti = 0.0, tis = 0.0;
+    double t_start = prm.t_start, t_end = prm.t_end;
     int i = 0, n = 0;
+    if (!done && prm.range_rule != kRangePlain) {
+      double total = 0.0;
+      for (int k = 0; k < K; ++k) total = __dadd_rn(total, tt[k]);
+      if (prm.range_rule == kRangeWhole) {
+        t_start = 0.0;
+        t_end = total;
+      }
+      if (prm.D < 3 || t_start < 0.0 || t_end > total) {
+        n = -1;
+        done = true;
+      }
+    }
     if (!done) {
       for (i = 0; i < K; ++i) {
         accumulated = __dadd_rn(accumulated, tt[i]);
-        if (accumulated > prm.t_start) break;
+        if (accumulated > t_start) break;
       }
-      if (prm.t_start > accumulated) {
-        n = -1;
+      if (t_start > accumulated) {
+        n = prm.range_rule == kRangePlain ? -1 : 0;
         done = true;
       } else if (i >= K) {
         done = true;
       } else {
         Ti = tt[i];
         accumulated = __dsub_rn(accumulated, Ti);
-        tis = __dsub_rn(prm.t_start, accumulated);
+        tis = __dsub_rn(t_start, accumulated);
       }
     }
     for (int n0 = 0;; n0 += kRangeChunk) {
       int cnt = 0;
       while (!done && cnt < kRangeChunk) {
-        if (!(accumulated < prm.t_end)) {
+        if (!(accumulated < t_end)) {
           done = true;
           break;
         }

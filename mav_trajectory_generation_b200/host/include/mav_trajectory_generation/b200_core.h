@@ -14,6 +14,7 @@
 
 #include "mav_trajectory_generation/segment.h"
 #include "mav_trajectory_generation/trajectory.h"
+#include "mav_trajectory_generation/trajectory_sampling.h"
 #include "mav_trajectory_generation/vertex.h"
 #include "mav_trajectory_generation_ros/feasibility_base.h"
 
@@ -133,6 +134,14 @@ class BatchCore {
   // plane nullable, -1 where the row is feasible or has a bad segment time)
   bool checkHalfPlaneFeasibility(const HalfPlane::Vector& planes, std::vector<uint8_t>* feasible,
                                  std::vector<int>* segment, std::vector<int>* plane) const;
+  // sampleTrajectoryInRange (whole = false) / sampleWholeTrajectory (whole = true, min_time and max_time unused) of
+  // every trajectory at its current coefficients: states[b], and ok[b] = the reference's return value (nullable;
+  // states[b] is empty where it is 0)
+  void sampleFlatStates(bool whole, double min_time, double max_time, double sampling_interval,
+                        std::vector<mav_msgs::EigenTrajectoryPointVector>* states, std::vector<uint8_t>* ok) const;
+  // sampleTrajectoryAtTime of trajectory b at sample_times[b] (states, ok: [B]; ok nullable, a zero state where 0)
+  void sampleFlatStatesAtTime(const std::vector<double>& sample_times, mav_msgs::EigenTrajectoryPointVector* states,
+                              std::vector<uint8_t>* ok) const;
   void getSegments(size_t b, Segment::Vector* segments) const;
 
   int N_;

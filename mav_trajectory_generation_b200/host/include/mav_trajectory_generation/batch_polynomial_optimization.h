@@ -141,6 +141,27 @@ class BatchPolynomialOptimization {
                                  std::vector<int>* segment = nullptr, std::vector<int>* plane = nullptr) const {
     return core_.checkHalfPlaneFeasibility(planes, feasible, segment, plane);
   }
+  // sampleTrajectoryInRange (reference src/trajectory_sampling.cpp:45-110) of every trajectory at its current
+  // coefficients, on the GPU: states[b] is what the reference fills, ok[b] its return value (0: min_time < 0,
+  // max_time beyond the trajectory or D < 3; states[b] is then empty).  Position ... snap are bit for bit the
+  // reference's; the orientation and angular terms use the device's trigonometry (a few ulps from glibc's) and, for
+  // D = 6, a quaternion with w >= 0.  sampleTrajectoryStartDuration is min_time = start, max_time = start + duration.
+  void sampleTrajectoriesInRange(double min_time, double max_time, double sampling_interval,
+                                 std::vector<mav_msgs::EigenTrajectoryPointVector>* states,
+                                 std::vector<uint8_t>* ok = nullptr) const {
+    core_.sampleFlatStates(false, min_time, max_time, sampling_interval, states, ok);
+  }
+  // sampleWholeTrajectory: the same over [0, each trajectory's total time]
+  void sampleWholeTrajectories(double sampling_interval, std::vector<mav_msgs::EigenTrajectoryPointVector>* states,
+                               std::vector<uint8_t>* ok = nullptr) const {
+    core_.sampleFlatStates(true, 0.0, 0.0, sampling_interval, states, ok);
+  }
+  // sampleTrajectoryAtTime of trajectory b at sample_times[b] (one time per trajectory): states[b], ok[b] (0 and a
+  // zero state where the time lies outside [0, the total time] or D < 3)
+  void sampleTrajectoriesAtTime(const std::vector<double>& sample_times, mav_msgs::EigenTrajectoryPointVector* states,
+                                std::vector<uint8_t>* ok = nullptr) const {
+    core_.sampleFlatStatesAtTime(sample_times, states, ok);
+  }
 
  private:
   b200::BatchCore core_;

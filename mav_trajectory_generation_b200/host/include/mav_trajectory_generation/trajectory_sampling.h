@@ -1,8 +1,10 @@
 // trajectory_sampling.h -- single-object sampling of a Trajectory / Segment into flat states (SURVEY.md 8f-3):
 // sampleTrajectoryAtTime, sampleTrajectoryInRange, sampleTrajectoryStartDuration, sampleWholeTrajectory,
 // sampleSegmentAtTime, sampleFlatStateAtTime (reference include/mav_trajectory_generation/trajectory_sampling.h,
-// src/trajectory_sampling.cpp:27-196).  The batched device form of the same sample set is
-// mtg_evaluate_range_batch_f64 / BatchPolynomialOptimization::evaluateRange with derivatives {0..4}.
+// src/trajectory_sampling.cpp:27-196).  The batched device forms are mtg_sample_flat_states_batch_f64 /
+// mtg_sample_flat_state_at_time_batch_f64 (BatchPolynomialOptimization::sampleTrajectoriesInRange,
+// sampleWholeTrajectories, sampleTrajectoriesAtTime), which share this mirror's rotation-vector arithmetic
+// (rotation_vector_kinematics.h).
 //
 // mav_msgs is not part of this tree, so mav_msgs::EigenTrajectoryPoint is mirrored as a plain struct with the same
 // field names and meaning (mav_msgs/eigen_mav_msgs.h): world-frame position ... snap, orientation quaternion,
@@ -20,6 +22,7 @@
 #include <cstdint>
 #include <vector>
 
+#include "mav_trajectory_generation/rotation_vector_kinematics.h"
 #include "mav_trajectory_generation/trajectory.h"
 
 namespace mav_msgs {
@@ -101,67 +104,16 @@ namespace mav_trajectory_generation {
 namespace sampling_detail {
 const double kNumNanosecondsPerSecond = 1.e9;
 
-struct V3 {
-  double v[3];
-};
-inline V3 cross(const V3& a, const V3& b) {
-  return {{a.v[1] * b.v[2] - a.v[2] * b.v[1], a.v[2] * b.v[0] - a.v[0] * b.v[2], a.v[0] * b.v[1] - a.v[1] * b.v[0]}};
-}
-inline double dot(const V3& a, const V3& b) { return a.v[0] * b.v[0] + a.v[1] * b.v[1] + a.v[2] * b.v[2]; }
-inline V3 axpy(double s, const V3& a, const V3& b) { return {{s * a.v[0] + b.v[0], s * a.v[1] + b.v[1], s * a.v[2] + b.v[2]}}; }
-
-// coefficients a = (1 - cos t)/t^2, b = (t - sin t)/t^3 of J = I + a [phi]x + b [phi]x^2 and their derivatives in t
-inline void jacobianCoefficients(double t, double* a, double* b, double* da, double* db) {
-  if (t < 1e-4) {  // series: the closed forms cancel catastrophically near 0
-    const double t2 = t * t;
-    *a = 0.5 - t2 / 24.0;
-    *b = 1.0 / 6.0 - t2 / 120.0;
-    *da = -t / 12.0;
-    *db = -t / 60.0;
-    return;
-  }
-  const double s = std::sin(t), c = std::cos(t);
-  *a = (1.0 - c) / (t * t);
-  *b = (t - s) / (t * t * t);
-  *da = (t * s - 2.0 * (1.0 - c)) / (t * t * t);
-  *db = ((1.0 - c) * t - 3.0 * (t - s)) / (t * t * t * t);
-}
-
 // orientation, world-frame angular velocity and acceleration of the rotation vector phi(t) with derivatives dphi, ddphi
+// (rotation_vector_kinematics.h, shared with the batched flat-state kernels)
 inline void rotationVectorKinematics(const V3& phi, const V3& dphi, const V3& ddphi, mav_msgs::Quaternion* q, V3* omega,
                                      V3* omega_dot) {
-  const double t = std::sqrt(dot(phi, phi));
-  if (t < 1e-12) {
-    *q = mav_msgs::Quaternion();
-  } else {
-    const double s = std::sin(0.5 * t) / t;
-    q->w = std::cos(0.5 * t);
-    q->x = s * phi.v[0];
-    q->y = s * phi.v[1];
-    q->z = s * phi.v[2];
-    if (q->w < 0.0) {  // the matrix -> quaternion conversion the reference goes through returns w >= 0
-      q->w = -q->w;
-      q->x = -q->x;
-      q->y = -q->y;
-      q->z = -q->z;
-    }
-  }
-  double a, b, da, db;
-  jacobianCoefficients(t, &a, &b, &da, &db);
-  auto applyJ = [&](const V3& x) {  // J x = x + a phi x x + b phi x (phi x x)
-    const V3 px = cross(phi, x);
-    return axpy(b, cross(phi, px), axpy(a, px, x));
-  };
-  *omega = applyJ(dphi);
-  // J' dphi with t' = phi . dphi / t:  a' phi x dphi + b' phi x (phi x dphi) + b (dphi x (phi x dphi))   (dphi x dphi = 0)
-  const double tdot = t > 1e-12 ? dot(phi, dphi) / t : 0.0;
-  const V3 pd = cross(phi, dphi);
-  V3 jd = {{0.0, 0.0, 0.0}};
-  jd = axpy(da * tdot, pd, jd);
-  jd = axpy(db * tdot, cross(phi, pd), jd);
-  jd = axpy(b, cross(dphi, pd), jd);
-  const V3 jdd = applyJ(ddphi);
-  *omega_dot = axpy(1.0, jdd, jd);
+  double c[4];
+  rotationVectorKinematics(phi, dphi, ddphi, c, omega, omega_dot);
+  q->w = c[0];
+  q->x = c[1];
+  q->y = c[2];
+  q->z = c[3];
 }
 
 inline V3 tail3(const Eigen::VectorXd& v) { return {{v[v.size() - 3], v[v.size() - 2], v[v.size() - 1]}}; }

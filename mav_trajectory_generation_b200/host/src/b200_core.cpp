@@ -567,6 +567,73 @@ void BatchCore::evaluateRange(double t_start, double t_end, double dt, const std
   CHECK_EQ(rc, MTG_OK) << mtg_last_error(h);
 }
 
+namespace {
+// one MTG_FLAT_STATE_DOUBLES record as the reference's EigenTrajectoryPoint of a D-dimensional trajectory
+void flatStateFromRecord(const double* r, int D, int64_t time_ns, mav_msgs::EigenTrajectoryPoint* p) {
+  Eigen::Vector3d* vecs[] = {&p->position_W, &p->velocity_W, &p->acceleration_W, &p->jerk_W, &p->snap_W};
+  for (int f = 0; f < 5; ++f)
+    for (int k = 0; k < 3; ++k) (*vecs[f])[k] = r[MTG_FLAT_STATE_POSITION + 3 * f + k];
+  const double* q = r + MTG_FLAT_STATE_ORIENTATION;
+  p->orientation_W_B.w = q[0];
+  p->orientation_W_B.x = q[1];
+  p->orientation_W_B.y = q[2];
+  p->orientation_W_B.z = q[3];
+  for (int k = 0; k < 3; ++k) {
+    p->angular_velocity_W[k] = r[MTG_FLAT_STATE_ANGULAR_VELOCITY + k];
+    p->angular_acceleration_W[k] = r[MTG_FLAT_STATE_ANGULAR_ACCELERATION + k];
+  }
+  p->time_from_start_ns = time_ns;
+  p->degrees_of_freedom = D == 6 ? mav_msgs::DOF6 : mav_msgs::DOF4;
+}
+}  // namespace
+
+void BatchCore::sampleFlatStates(bool whole, double min_time, double max_time, double sampling_interval,
+                                 std::vector<mav_msgs::EigenTrajectoryPointVector>* states,
+                                 std::vector<uint8_t>* ok) const {
+  CHECK_NOTNULL(states)->assign(B_, mav_msgs::EigenTrajectoryPointVector());
+  if (ok) ok->assign(B_, 0);
+  std::vector<int32_t> n(B_, 0);
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int K = topo_.K, D = topo_.D;
+  // a counting pass sizes the records: the reference's walk can start a segment early, so no closed form bounds it
+  int rc = mtg_sample_flat_states_batch_host_f64(h, N_, K, D, static_cast<int64_t>(B_), times_, coeffs_, min_time,
+                                                 max_time, sampling_interval, whole, 0, nullptr, nullptr, n.data());
+  CHECK_EQ(rc, MTG_OK) << mtg_last_error(h);
+  int32_t S = 0;
+  for (int32_t c : n) S = std::max(S, c);
+  std::vector<double> rec(B_ * size_t(S) * MTG_FLAT_STATE_DOUBLES);
+  std::vector<int64_t> ns(B_ * size_t(S));
+  rc = mtg_sample_flat_states_batch_host_f64(h, N_, K, D, static_cast<int64_t>(B_), times_, coeffs_, min_time,
+                                             max_time, sampling_interval, whole, S, rec.data(), ns.data(), n.data());
+  CHECK_EQ(rc, MTG_OK) << mtg_last_error(h);
+  for (size_t b = 0; b < B_; ++b) {
+    if (ok) (*ok)[b] = n[b] >= 0;
+    (*states)[b].resize(std::max(n[b], 0));
+    for (int32_t i = 0; i < n[b]; ++i) {
+      const size_t at = b * size_t(S) + i;
+      flatStateFromRecord(&rec[at * MTG_FLAT_STATE_DOUBLES], D, ns[at], &(*states)[b][i]);
+    }
+  }
+}
+
+void BatchCore::sampleFlatStatesAtTime(const std::vector<double>& sample_times,
+                                       mav_msgs::EigenTrajectoryPointVector* states, std::vector<uint8_t>* ok) const {
+  CHECK_EQ(sample_times.size(), B_);
+  std::vector<double> rec(B_ * MTG_FLAT_STATE_DOUBLES);
+  std::vector<int64_t> ns(B_);
+  std::vector<int32_t> good(B_);
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_sample_flat_state_at_time_batch_host_f64(h, N_, topo_.K, topo_.D, static_cast<int64_t>(B_),
+                                                              times_, coeffs_, sample_times.data(), rec.data(),
+                                                              ns.data(), good.data());
+  CHECK_EQ(rc, MTG_OK) << mtg_last_error(h);
+  CHECK_NOTNULL(states)->assign(B_, mav_msgs::EigenTrajectoryPoint());
+  if (ok) ok->assign(good.begin(), good.end());
+  for (size_t b = 0; b < B_; ++b) flatStateFromRecord(&rec[b * MTG_FLAT_STATE_DOUBLES], topo_.D, ns[b], &(*states)[b]);
+}
+
 void BatchCore::computeMaximaOfMagnitude(const std::vector<int>& derivatives, std::vector<Extremum>* maxima) const {
   CHECK(!derivatives.empty() && derivatives.size() <= 8);
   const size_t nd = derivatives.size();
