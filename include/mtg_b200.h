@@ -261,6 +261,62 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
                                              double* seg_times_out, int32_t* within_range, double* maxima,
                                              int32_t* status, void* stream);
 
+/* Result codes of mtg_optimize_time_mellinger_batch_f64: the public nlopt_result values, so that callers of the
+ * reference read stopping reasons as before. */
+#define MTG_OPTIMIZE_RESULT_FAILURE (-1)
+#define MTG_OPTIMIZE_RESULT_ROUNDOFF_LIMITED (-4)
+#define MTG_OPTIMIZE_RESULT_SUCCESS 1
+#define MTG_OPTIMIZE_RESULT_FTOL_REACHED 3
+#define MTG_OPTIMIZE_RESULT_XTOL_REACHED 4
+#define MTG_OPTIMIZE_RESULT_MAXEVAL_REACHED 5
+
+/* The stopping rules of NonlinearOptimizationParameters that the Mellinger outer loop reads.  A negative tolerance
+ * disables its test.  Reference defaults: f_abs -1, f_rel 0.05, x_rel -1, x_abs -1, initial_stepsize_rel 0.1,
+ * max_iterations 3000. */
+typedef struct mtg_mellinger_params {
+  double f_abs, f_rel, x_rel, x_abs;
+  double initial_stepsize_rel; /* <= 0: 0.1 ("heuristic if negative") */
+  int32_t max_iterations;      /* gradient evaluations; < 0: no limit */
+} mtg_mellinger_params;
+
+/* PolynomialOptimizationNonLinear::optimize() with kMellingerOuterLoop (impl/polynomial_optimization_nonlinear_impl.h:
+ * 171-259) for B trajectories: a descent on the segment times with the gradient of
+ * mtg_cost_gradient_mellinger_batch_f64, times bounded below by 0.1 s, then mtg_scale_times_with_violation_batch_f64.
+ * The reference drives the descent with NLopt; this entry defines its own projected-gradient descent, per row, with
+ * x = the K segment times, l = 0.1, and k counting gradient evaluations from 0:
+ *   1. (J_k, g_k) = getCostAndGradientMellinger(x_k), exactly as mtg_cost_gradient_mellinger_batch_f64.
+ *   2. alpha_0 = fl(fl(initial_stepsize_rel * max_i x_0,i) / max_i |g_0,i|).
+ *   3. Every g_k,i == 0 (always for K = 1): stop, SUCCESS.
+ *   4. Candidates j = 0..7 at step a_j = fl(alpha_k * 2^(1-j)): x_j,i = max(l, fl(x_k,i - fl(a_j * g_k,i))) (two roundings,
+ *      no FMA, `v > l ? v : l`).  J_j = computeCost() of the solve at x_j.
+ *   5. Accept the smallest j with J_j <= fl(J_k + fl(1e-4 * s_j)), s_j = sum_i fl(g_k,i * fl(x_j,i - x_k,i)) summed left
+ *      to right: x_k+1 = x_j, alpha_k+1 = a_j.  No candidate accepted: stop, ROUNDOFF_LIMITED, keep x_k (so the cost
+ *      never rises above the start).
+ *   6. After an accepted step, in this order: k+1 >= max_iterations (when >= 0): MAXEVAL_REACHED; |J_j - J_k| <=
+ *      f_rel * |J_j| or <= f_abs: FTOL_REACHED; for every i, |x_k+1,i - x_k,i| <= x_rel * |x_k+1,i| or <= x_abs:
+ *      XTOL_REACHED.  Otherwise iterate.  max_iterations == 0: every valid row stops at once with MAXEVAL_REACHED.
+ * Then every row that iterated goes through mtg_scale_times_with_violation_batch_f64 at (v_max, a_max).
+ * Outputs: seg_times_out [B][K] the scaled times (may be seg_times), coeffs [B][K][D][N] the re-solve at them;
+ * relative_times [B][K] the times before scaling (the reference's "RELATIVE Solution"); cost [B] computeCost() at the
+ * final times (getCost()); iterations [B] accepted steps; result [B] MTG_OPTIMIZE_RESULT_*; within_range, maxima as the
+ * scaling entry; status [B] the scaling's status bits, with MTG_STATUS_NOT_SPD when the loop stopped on a failed solve.
+ * Everything after seg_times_out is nullable.  Edge rows:
+ *   a segment time <= 0 or non-finite: FAILURE, status MTG_STATUS_BAD_TIME, times unchanged, 0 iterations;
+ *   a start time in (0, 0.1): FAILURE, neither iterated nor scaled (decision: the reference returns before the scaling
+ *     when its optimiser aborts without a cost, which NLopt does for a start below the lower bound); coeffs are the
+ *     solve at the start times;
+ *   any solve of a row reporting MTG_STATUS_NOT_SPD (gradient or candidates): FAILURE, keeps x_k, then scaled.
+ * A row's result does not depend on the other rows of the batch.  Unlike the other entries this one WAITS on `stream`
+ * once per iteration: it reads the number of rows still iterating (pinned memory, one event wait), and every
+ * launch after that covers only those rows.  Refused (MTG_ERR_BAD_ARG, no launch): what
+ * mtg_scale_times_with_violation_batch_f64 refuses, a null params, and params with every tolerance negative and
+ * max_iterations < 0. */
+int mtg_optimize_time_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                          const double* d_fixed, const mtg_mellinger_params* params, double v_max,
+                                          double a_max, double* coeffs, double* seg_times_out, double* relative_times,
+                                          double* cost, int32_t* iterations, int32_t* result, int32_t* within_range,
+                                          double* maxima, int32_t* status, void* stream);
+
 /* FeasibilityAnalytic::checkInputFeasibility per segment and checkInputFeasibilityTrajectory per trajectory (reference
  * mav_trajectory_generation_ros/src/feasibility_analytic.cpp, feasibility_base.cpp).  result[b] is an MTG_FEAS_* code
  * (InputFeasibilityResult): the first segment that is not Feasible decides, in the reference's order of checks --
@@ -486,6 +542,12 @@ int mtg_scale_times_with_violation_batch_host_f64(mtg_handle* h, const mtg_probl
                                                   const double* seg_times, const double* d_fixed, double v_max,
                                                   double a_max, double* coeffs, double* seg_times_out,
                                                   int32_t* within_range, double* maxima, int32_t* status);
+int mtg_optimize_time_mellinger_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                               const double* d_fixed, const mtg_mellinger_params* params, double v_max,
+                                               double a_max, double* coeffs, double* seg_times_out,
+                                               double* relative_times, double* cost, int32_t* iterations,
+                                               int32_t* result, int32_t* within_range, double* maxima,
+                                               int32_t* status);
 
 int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
                                          const double* seg_times, const double* coeffs,

@@ -6,4 +6,4 @@ Python here is plumbing for tests and benchmarks; the product is the C-ABI libra
 from . import _build  # noqa: F401
 from .capi import (KERNEL_GENERIC, KERNEL_NOFREE, KERNEL_WAYPOINT, STATUS_BAD_TIME,  # noqa: F401
                    STATUS_NOT_SPD, TIME_COST_RICHTER, TIME_COST_SQUARED, Problem, Solver, load,
-                   time_objective_params)
+                   time_objective_params, mellinger_params)

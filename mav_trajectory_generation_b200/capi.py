@@ -43,7 +43,8 @@ EXPORTED_SYMBOLS = [
     "mtg_input_feasibility_recursive_batch_host_f64", "mtg_input_feasibility_sampling_batch_f64",
     "mtg_input_feasibility_sampling_batch_host_f64", "mtg_sample_flat_states_batch_f64",
     "mtg_sample_flat_state_at_time_batch_f64", "mtg_sample_flat_states_batch_host_f64",
-    "mtg_sample_flat_state_at_time_batch_host_f64",
+    "mtg_sample_flat_state_at_time_batch_host_f64", "mtg_optimize_time_mellinger_batch_f64",
+    "mtg_optimize_time_mellinger_batch_host_f64",
 ]
 # mav_msgs::EigenTrajectoryPoint as one record of MTG_FLAT_STATE_DOUBLES doubles: the slice of each field
 FLAT_STATE_DOUBLES = 25
@@ -69,6 +70,29 @@ GRAVITY = 9.81
 class MtgProblem(C.Structure):
     _fields_ = [("N", C.c_int32), ("r", C.c_int32), ("K", C.c_int32), ("D", C.c_int32),
                 ("fixed_mask", C.POINTER(C.c_uint8))]
+
+
+class MtgMellingerParams(C.Structure):
+    _fields_ = [("f_abs", C.c_double), ("f_rel", C.c_double), ("x_rel", C.c_double), ("x_abs", C.c_double),
+                ("initial_stepsize_rel", C.c_double), ("max_iterations", C.c_int32)]
+
+
+# nlopt_result values of mtg_optimize_time_mellinger_batch_f64
+(OPTIMIZE_RESULT_FAILURE, OPTIMIZE_RESULT_ROUNDOFF_LIMITED, OPTIMIZE_RESULT_SUCCESS, OPTIMIZE_RESULT_FTOL_REACHED, OPTIMIZE_RESULT_XTOL_REACHED,
+ OPTIMIZE_RESULT_MAXEVAL_REACHED) = (-1, -4, 1, 3, 4, 5)
+# NonlinearOptimizationParameters' defaults
+MELLINGER_DEFAULTS = dict(f_abs=-1.0, f_rel=0.05, x_rel=-1.0, x_abs=-1.0, initial_stepsize_rel=0.1,
+                          max_iterations=3000)
+
+
+def mellinger_params(**kw):
+    """mtg_mellinger_params: MELLINGER_DEFAULTS updated by kw."""
+    unknown = set(kw) - set(MELLINGER_DEFAULTS)
+    if unknown:
+        raise ValueError(f"unknown Mellinger parameters {sorted(unknown)}")
+    v = dict(MELLINGER_DEFAULTS, **kw)
+    return MtgMellingerParams(float(v["f_abs"]), float(v["f_rel"]), float(v["x_rel"]), float(v["x_abs"]),
+                              float(v["initial_stepsize_rel"]), int(v["max_iterations"]))
 
 
 class MtgLayout(C.Structure):
@@ -280,6 +304,10 @@ def load():
     L.mtg_sample_flat_state_at_time_batch_f64.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, i64, dp, dp, dp, dp,
                                                           dp, dp, vp]
     L.mtg_sample_flat_state_at_time_batch_host_f64.argtypes = L.mtg_sample_flat_state_at_time_batch_f64.argtypes[:-1]
+    L.mtg_optimize_time_mellinger_batch_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp,
+                                                        C.POINTER(MtgMellingerParams), dbl, dbl, dp, dp, dp, dp, dp,
+                                                        dp, dp, dp, dp, vp]
+    L.mtg_optimize_time_mellinger_batch_host_f64.argtypes = L.mtg_optimize_time_mellinger_batch_f64.argtypes[:-1]
     for name in EXPORTED_SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export what the header declares
     _lib = L
@@ -575,6 +603,36 @@ class Solver:
         self._check(rc, "mtg_scale_times_with_violation_batch_f64")
         return coeffs, seg_times_out, within, maxima, status
 
+    def optimize_time_mellinger(self, prob, seg_times, d_fixed, v_max, a_max, params=None, seg_times_out=None,
+                                stream=None):
+        """Batched PolynomialOptimizationNonLinear::optimize() with kMellingerOuterLoop (mtg_b200.h states the
+        descent): -> dict of coeffs [B][K][D][N], seg_times (scaled) [B][K], relative_times [B][K], cost [B],
+        iterations [B], result [B] (OPTIMIZE_RESULT_*), within_range [B], maxima [B][2], status [B].  params: a
+        mellinger_params() (defaults: the reference's).  Waits on the stream once per iteration."""
+        import torch
+        B = seg_times.shape[0]
+        dev = seg_times.device
+        if params is None:
+            params = mellinger_params()
+        out = dict(coeffs=torch.empty((B, prob.K, prob.D, prob.N), dtype=torch.float64, device=dev),
+                   seg_times=seg_times_out if seg_times_out is not None else torch.empty_like(seg_times),
+                   relative_times=torch.empty_like(seg_times),
+                   cost=torch.empty((B,), dtype=torch.float64, device=dev),
+                   iterations=torch.empty((B,), dtype=torch.int32, device=dev),
+                   result=torch.empty((B,), dtype=torch.int32, device=dev),
+                   within_range=torch.empty((B,), dtype=torch.int32, device=dev),
+                   maxima=torch.empty((B, 2), dtype=torch.float64, device=dev),
+                   status=torch.empty((B,), dtype=torch.int32, device=dev))
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.mtg_optimize_time_mellinger_batch_f64(
+            self.h, C.byref(prob.c), B, seg_times.data_ptr(), d_fixed.data_ptr(), C.byref(params), float(v_max),
+            float(a_max), *[out[k].data_ptr() for k in self._MELLINGER_OUTPUTS], s)
+        self._check(rc, "mtg_optimize_time_mellinger_batch_f64")
+        return out
+
+    _MELLINGER_OUTPUTS = ("coeffs", "seg_times", "relative_times", "cost", "iterations", "result", "within_range",
+                          "maxima", "status")
+
     def check_input_feasibility(self, seg_times, coeffs, limits, min_section_time=0.05, gravity=GRAVITY, stream=None):
         """Batched FeasibilityAnalytic::checkInputFeasibilityTrajectory: (result [B], segment [B], status [B]), int32.
         limits: {name: value} over INPUT_LIMITS (absent name = no limit; default_input_limits() gives the reference's
@@ -763,6 +821,25 @@ class Solver:
             self._hptr(status))
         self._check(rc, "mtg_scale_to_constraints_batch_host_f64")
         return seg_times_out
+
+    def optimize_time_mellinger_host(self, prob, seg_times, d_fixed, v_max, a_max, params=None):
+        """optimize_time_mellinger on host numpy arrays (one copy in, the loop, one copy out): a dict of numpy
+        arrays with the same keys."""
+        B, K = seg_times.shape
+        if params is None:
+            params = mellinger_params()
+        seg_times = np.ascontiguousarray(seg_times, dtype=np.float64)
+        d_fixed = np.ascontiguousarray(d_fixed, dtype=np.float64)
+        f8, i4 = np.float64, np.int32
+        out = dict(coeffs=np.empty((B, K, prob.D, prob.N), f8), seg_times=np.empty((B, K), f8),
+                   relative_times=np.empty((B, K), f8), cost=np.empty(B, f8), iterations=np.empty(B, i4),
+                   result=np.empty(B, i4), within_range=np.empty(B, i4), maxima=np.empty((B, 2), f8),
+                   status=np.empty(B, i4))
+        rc = self.lib.mtg_optimize_time_mellinger_batch_host_f64(
+            self.h, C.byref(prob.c), B, seg_times.ctypes.data, d_fixed.ctypes.data, C.byref(params), float(v_max),
+            float(a_max), *[out[k].ctypes.data for k in self._MELLINGER_OUTPUTS])
+        self._check(rc, "mtg_optimize_time_mellinger_batch_host_f64")
+        return out
 
     def scale_times_with_violation_host(self, prob, seg_times, d_fixed, v_max, a_max, coeffs, seg_times_out,
                                         within_range=None, maxima=None, status=None):

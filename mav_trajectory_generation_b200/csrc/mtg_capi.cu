@@ -18,6 +18,7 @@
 #include "mtg_flat_state_kernel.cuh"
 #include "mtg_generic_kernel.cuh"
 #include "mtg_half_plane_kernel.cuh"
+#include "mtg_mellinger_loop_kernel.cuh"
 #include "mtg_twisted_kernel.cuh"
 #include "mtg_twisted_tmem_kernel.cuh"
 #include "mtg_twisted_tmem_v4_kernel.cuh"
@@ -82,6 +83,9 @@ struct mtg_handle {
   Arena pack[kPipe + 1];     // times + d_fixed produced by nfabian_pack_kernel; Mellinger expansion
   Arena counters[kPipe + 1]; // dynamic tile counter of the persistent kernels (event-ordered like the scratch arenas: two
                              // launches of one slot on different caller streams must not share a live counter)
+  Arena optim[kPipe + 1];    // Mellinger outer loop: compact row lists and per-row state across its iterations
+  int* pinned_count = nullptr;        // the outer loop's active-row count, read back once per iteration
+  cudaEvent_t count_ev = nullptr;
   // What is known about each kernel function launched so far, queried or set once per function so that a repeated
   // B = 1 solveLinear() call makes no attribute call.  The dynamic shared memory limit is a property of the function
   // (shared by every K routed to it): only ever raised.
@@ -230,6 +234,7 @@ struct WaypointEntry {
   size_t (*v5_smem)(int K, int nf, int nbuf), (*v5_fused_smem)(int K, int nf, int nbuf);
   bool (*early_fits)(int K);      // the EARLY instantiations may run for this K
   TmemKernel cost;                // computeCost of the solution without writing coefficients (v3 layout)
+  TmemKernel cost_ls;             // the same with the line-search time generator (Mellinger outer loop)
 };
 enum : int { kV1 = 1, kCost = 2 };
 // The row of (N, R, D).  FLAGS adds v1 and the cost-only kernel; MINB > 0 adds v4 and v5 with MINB blocks per SM in
@@ -268,7 +273,10 @@ WaypointEntry waypoint_row() {
     e.v5_fused_smem = mtg::V5Layout<N, D, true>::bytes;
     e.early_fits = mtg::V5Layout<N, D, false>::template early_fits<kV5Early>;
   }
-  if constexpr ((FLAGS & kCost) != 0) e.cost = mtg::twisted_tmem_kernel<N, R, D, false, true>;
+  if constexpr ((FLAGS & kCost) != 0) {
+    e.cost = mtg::twisted_tmem_kernel<N, R, D, false, true>;
+    e.cost_ls = mtg::twisted_tmem_line_search_kernel<N, R, D>;
+  }
   return e;
 }
 const WaypointEntry kWaypoints[] = {
@@ -831,14 +839,18 @@ int launch_masked(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int
 // Fused cost-only solve (SURVEY.md 8f-2): nx problems -> cost_x[nx].  With mel_k1 > 0 the nx = B * mel_k1 problems
 // are the Mellinger expansion of the B trajectories in (times, dfix), generated inside the kernel.
 // Returns MTG_ERR_ALLOC when no fused kernel / launch configuration exists (caller falls back).
+// With ls_grad set the nx = rows * kLineSearchSteps problems are the line-search candidates of the rows in (times, dfix)
+// at steps ls_alpha (mtg::WaypointParams).  status_x [nx] or null: every problem's solve status.
 int launch_cost_fused(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t nx, const double* times,
-                      const double* dfix, double* cost_x, int mel_k1, double inc, double lower, cudaStream_t stream) {
+                      const double* dfix, double* cost_x, int mel_k1, double inc, double lower, cudaStream_t stream,
+                      int32_t* status_x = nullptr, const double* ls_grad = nullptr, const double* ls_alpha = nullptr) {
   const Layout& L = topo->layout;
   const WaypointEntry* e = find_waypoint(p, L);
   if (!e || !e->cost || L.n_free == 0) return MTG_ERR_ALLOC;
+  const TmemKernel fn = ls_grad ? e->cost_ls : e->cost;
   const size_t smem = e->v3_smem(p->K);
   bool fits = false;
-  MTG_TRY(v3_fits(h, (const void*)e->cost, smem, &fits));
+  MTG_TRY(v3_fits(h, (const void*)fn, smem, &fits));
   if (!fits) return MTG_ERR_ALLOC;  // large K: unfused path (chunked kernel + cost kernel)
   mtg::WaypointParams prm{};  // no coefficient output, no fused inputs
   prm.K = p->K;
@@ -847,13 +859,16 @@ int launch_cost_fused(mtg_handle* h, const mtg_problem* p, CachedTopology* topo,
   prm.times = times;
   prm.dfix = dfix;
   prm.cost = cost_x;
+  prm.status = status_x;
   prm.mel_k1 = mel_k1;
   prm.mel_inc = inc;
   prm.mel_lower = lower;
-  MTG_TRY(ensure_dyn_smem(h, (const void*)e->cost, smem));
+  prm.ls_grad = ls_grad;
+  prm.ls_alpha = ls_alpha;
+  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
   CUtensorMap tmap;
-  std::memset(&tmap, 0, sizeof(tmap));  // unused by the cost-only instantiation
-  e->cost<<<(unsigned)((nx + 63) / 64), mtg::kTmemThreads, smem, stream>>>(prm, tmap);
+  std::memset(&tmap, 0, sizeof(tmap));  // unused by the cost-only instantiations
+  fn<<<(unsigned)((nx + 63) / 64), mtg::kTmemThreads, smem, stream>>>(prm, tmap);
   MTG_CUDA(h, cudaGetLastError());
   h->launches++;
   return MTG_OK;
@@ -1138,7 +1153,7 @@ void mtg_destroy(mtg_handle* h) {
     cudaFree(t.d_vcol);
   }
   for (int i = 0; i <= mtg_handle::kPipe; ++i) {
-    for (mtg_handle::Arena* a : {&h->scratch[i], &h->pack[i], &h->counters[i]}) {
+    for (mtg_handle::Arena* a : {&h->scratch[i], &h->pack[i], &h->counters[i], &h->optim[i]}) {
       if (a->p) cudaFree(a->p);
       if (a->ev) cudaEventDestroy(a->ev);
     }
@@ -1147,6 +1162,8 @@ void mtg_destroy(mtg_handle* h) {
     if (h->dev_buf[i]) cudaFree(h->dev_buf[i]);
     if (h->streams[i]) cudaStreamDestroy(h->streams[i]);
   }
+  if (h->pinned_count) cudaFreeHost(h->pinned_count);
+  if (h->count_ev) cudaEventDestroy(h->count_ev);
   delete h;
 }
 
@@ -1581,9 +1598,10 @@ int mtg_sample_flat_state_at_time_batch_f64(mtg_handle* h, int32_t N, int32_t K,
   });
 }
 
+// status_x [B][K+1] or null: the status of every solve (the unperturbed one first)
 static int launch_mellinger(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B,
                             const double* seg_times, const double* d_fixed, double* cost, double* grad, cudaStream_t s,
-                            int slot) {
+                            int slot, int32_t* status_x = nullptr) {
   const Layout& L = topo->layout;
   const size_t K = p->K, D = p->D, N = p->N, nf = L.n_fixed;
   mtg_handle::Arena& ar = h->pack[slot];
@@ -1591,7 +1609,8 @@ static int launch_mellinger(mtg_handle* h, const mtg_problem* p, CachedTopology*
     // fused path: one cost-only launch over the B*(K+1) expanded problems (expansion generated in the kernel, no
     // perturbed inputs or coefficients ever written), then the finite differences
     MTG_TRY(arena_acquire(h, ar, size_t(B) * (K + 1) * 8, s));
-    const int rc = launch_cost_fused(h, p, topo, B * int64_t(K + 1), seg_times, d_fixed, ar.p, int(K + 1), 0.1, 0.1, s);
+    const int rc =
+        launch_cost_fused(h, p, topo, B * int64_t(K + 1), seg_times, d_fixed, ar.p, int(K + 1), 0.1, 0.1, s, status_x);
     if (rc == MTG_OK) {
       const int threads = 128;
       const int64_t gb = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
@@ -1631,7 +1650,8 @@ static int launch_mellinger(mtg_handle* h, const mtg_problem* p, CachedTopology*
     mtg::mellinger_expand_kernel<<<(unsigned)blocks, threads, 0, s>>>(mp);
     MTG_CUDA(h, cudaGetLastError());
     h->launches++;
-    MTG_TRY(launch_solve(h, p, topo, nx, t_x, f_x, nullptr, c_x, nullptr, nullptr, s, false, nullptr, slot));
+    MTG_TRY(launch_solve(h, p, topo, nx, t_x, f_x, nullptr, c_x, nullptr,
+                         status_x ? status_x + b0 * int64_t(K + 1) : nullptr, s, false, nullptr, slot));
     MTG_TRY(launch_cost(h, p, nx, t_x, c_x, j_x, s));
     const int64_t gb = std::min<int64_t>((nb + threads - 1) / threads, int64_t(h->sm_count) * 16);
     mtg::mellinger_gradient_kernel<<<(unsigned)gb, threads, 0, s>>>(nb, p->K, j_x, cost ? cost + b0 : nullptr,
@@ -1846,7 +1866,7 @@ static bool valid_violation(const mtg_problem* p, int64_t B, double v_max, doubl
 static int launch_scale_with_violation(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B,
                                        const double* seg_times, const double* d_fixed, double v_max, double a_max,
                                        double* coeffs, double* seg_times_out, int32_t* within_range, double* maxima,
-                                       int32_t* status, cudaStream_t s, int slot) {
+                                       int32_t* status, cudaStream_t s, int slot, const int32_t* pass = nullptr) {
   // scratch: status of the first solve [B], of the scaling [B], of the re-solve [B]
   const size_t o_sc = align_doubles((size_t(B) + 1) / 2), o_re = 2 * o_sc;
   mtg_handle::Arena& ar = h->pack[slot];
@@ -1859,14 +1879,19 @@ static int launch_scale_with_violation(mtg_handle* h, const mtg_problem* p, Cach
   // nonlinear_impl.h:366-406: the solve at the given times (trajectory_.scaleSegmentTimesToMeetConstraints acts on
   // the solved trajectory), the stretch in place on coeffs, then solveLinear() at the stretched times
   MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, st_solve, s, false, nullptr, slot));
+  const int threads = 128;
+  const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
+  if (pass) {  // rows with a non-zero pass[] are not stretched (the scaling passes failed solves through)
+    mtg::or_status_kernel<<<(unsigned)blocks, threads, 0, s>>>(B, pass, st_solve);
+    MTG_CUDA(h, cudaGetLastError());
+    h->launches++;
+  }
   MTG_TRY(launch_scale_to_constraints(h, p->N, p->K, p->D, B, seg_times, coeffs, v_max, a_max, seg_times_out, coeffs,
                                       st_solve, within_range, maxima, st_scale, s));
   MTG_TRY(launch_solve(h, p, topo, B, seg_times_out, d_fixed, nullptr, coeffs, nullptr, st_resolve, s, false, nullptr,
                        slot));
   if (status) {
     MTG_CUDA(h, cudaMemcpyAsync(status, st_scale, sizeof(int32_t) * size_t(B), cudaMemcpyDeviceToDevice, s));
-    const int threads = 128;
-    const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
     mtg::or_status_kernel<<<(unsigned)blocks, threads, 0, s>>>(B, st_resolve, status);
     MTG_CUDA(h, cudaGetLastError());
     h->launches++;
@@ -1882,6 +1907,188 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
       h, valid_violation(p, B, v_max, a_max, seg_times, d_fixed, coeffs, seg_times_out), p, B, [&](CachedTopology* topo) {
         return launch_scale_with_violation(h, p, topo, B, seg_times, d_fixed, v_max, a_max, coeffs, seg_times_out,
                                            within_range, maxima, status, (cudaStream_t)stream, mtg_handle::kPipe);
+      });
+}
+
+// ---- the Mellinger outer loop (PolynomialOptimizationNonLinear::optimize with kMellingerOuterLoop) -----------------
+static bool valid_mellinger_params(const mtg_mellinger_params* q) {
+  if (!q) return false;
+  const bool any_tol = q->f_rel >= 0.0 || q->f_abs >= 0.0 || q->x_rel >= 0.0 || q->x_abs >= 0.0;
+  return any_tol || q->max_iterations >= 0;  // otherwise nothing would stop a row
+}
+
+static bool valid_optimize(const mtg_problem* p, int64_t B, const mtg_mellinger_params* q, double v_max, double a_max,
+                           const double* seg_times, const double* d_fixed, const double* coeffs,
+                           const double* seg_times_out) {
+  return valid_violation(p, B, v_max, a_max, seg_times, d_fixed, coeffs, seg_times_out) && valid_mellinger_params(q);
+}
+
+// The candidate costs Jc [rows][kLineSearchSteps] and solve statuses st_c of the compact rows in `lp`: one cost-only
+// launch where the fused kernel exists, else expand + solve + cost in chunks (as launch_mellinger's unfused path).
+static int launch_line_search(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, const mtg::MelLoopParams& lp,
+                              double* Jc, int32_t* st_c, cudaStream_t s, int slot) {
+  constexpr int kL = mtg::kLineSearchSteps;
+  const int64_t rows = lp.rows;
+  if (h->mellinger_unfused == 0) {  // MTG_OPT_MELLINGER_UNFUSED selects the unfused path here as for the gradient
+    const int rc =
+        launch_cost_fused(h, p, topo, rows * kL, lp.x, lp.dfix, Jc, 0, 0.0, lp.lower, s, st_c, lp.g, lp.alpha);
+    if (rc != MTG_ERR_ALLOC) return rc;
+  }
+  const size_t K = p->K, D = p->D, N = p->N, dnf = lp.dnf;
+  const size_t per_x = (K + dnf + K * D * N) * 8;  // times + d_fixed + coeffs of one candidate
+  int64_t chunk = std::max<int64_t>(1, int64_t((size_t(384) << 20) / (per_x * kL)));
+  chunk = std::min<int64_t>(chunk, rows);
+  const size_t nx_max = size_t(chunk) * kL;
+  const size_t o_f = align_doubles(nx_max * K), o_c = o_f + align_doubles(nx_max * dnf),
+               need = (o_c + align_doubles(nx_max * K * D * N)) * 8;
+  mtg_handle::Arena& ar = h->pack[slot];
+  MTG_TRY(arena_acquire(h, ar, need, s));
+  for (int64_t r0 = 0; r0 < rows; r0 += chunk) {
+    const int64_t nr = std::min<int64_t>(chunk, rows - r0), nx = nr * kL;
+    mtg::MelLoopParams cp = lp;
+    cp.rows = int(nr);
+    cp.x = lp.x + r0 * K;
+    cp.g = lp.g + r0 * K;
+    cp.alpha = lp.alpha + r0;
+    cp.dfix = lp.dfix + r0 * dnf;
+    const int threads = 128;
+    const int64_t blocks = std::min<int64_t>((nx + threads - 1) / threads, int64_t(h->sm_count) * 16);
+    mtg::line_search_expand_kernel<<<(unsigned)blocks, threads, 0, s>>>(cp, ar.p, ar.p + o_f);
+    MTG_CUDA(h, cudaGetLastError());
+    h->launches++;
+    MTG_TRY(launch_solve(h, p, topo, nx, ar.p, ar.p + o_f, nullptr, ar.p + o_c, nullptr, st_c + r0 * kL, s, false,
+                         nullptr, slot));
+    MTG_TRY(launch_cost(h, p, nx, ar.p, ar.p + o_c, Jc + r0 * kL, s));
+  }
+  return arena_release(h, ar, s);
+}
+
+// The number of compact rows the last kernel on `s` listed: one copy into pinned memory and one event wait.
+static int read_count(mtg_handle* h, const int32_t* d_count, cudaStream_t s, int* out) {
+  if (!h->pinned_count) MTG_CUDA(h, cudaHostAlloc((void**)&h->pinned_count, sizeof(int), cudaHostAllocDefault));
+  if (!h->count_ev) MTG_CUDA(h, cudaEventCreateWithFlags(&h->count_ev, cudaEventDisableTiming));
+  MTG_CUDA(h, cudaMemcpyAsync(h->pinned_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, s));
+  MTG_CUDA(h, cudaEventRecord(h->count_ev, s));
+  MTG_CUDA(h, cudaEventSynchronize(h->count_ev));
+  *out = *h->pinned_count;
+  return MTG_OK;
+}
+
+static int launch_optimize_mellinger(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B,
+                                     const double* seg_times, const double* d_fixed, const mtg_mellinger_params* q,
+                                     double v_max, double a_max, double* coeffs, double* seg_times_out,
+                                     double* relative_times, double* cost, int32_t* iterations, int32_t* result,
+                                     int32_t* within_range, double* maxima, int32_t* status, cudaStream_t s, int slot) {
+  constexpr int kL = mtg::kLineSearchSteps;
+  const size_t K = p->K, dnf = size_t(p->D) * topo->layout.n_fixed, nB = size_t(B);
+  const size_t ni = align_doubles((nB + 1) / 2);  // one int32 per row, in doubles
+  // arena: [2][B][K] x, [2][B] alpha, [2][B][dnf] d_fixed, [B][K] g, [B] J, [B][kL] Jc | int32: [2][B] idx, [B][K+1]
+  // st_g, [B][kL] st_c, [B] iters, result, pass, opt_status, scale status, and the count
+  size_t off = 0;
+  auto take = [&](size_t doubles) {
+    const size_t o = off;
+    off += align_doubles(doubles);
+    return o;
+  };
+  const size_t o_x[2] = {take(nB * K), take(nB * K)}, o_a[2] = {take(nB), take(nB)},
+               o_f[2] = {take(nB * dnf), take(nB * dnf)}, o_g = take(nB * K), o_J = take(nB), o_Jc = take(nB * kL),
+               o_idx[2] = {take((nB + 1) / 2), take((nB + 1) / 2)}, o_stg = take((nB * (K + 1) + 1) / 2),
+               o_stc = take((nB * kL + 1) / 2), o_it = take(ni), o_res = take(ni), o_pass = take(ni),
+               o_ost = take(ni), o_sst = take(ni), o_cnt = take(1);
+  mtg_handle::Arena& ar = h->optim[slot];
+  MTG_TRY(arena_acquire(h, ar, off * 8, s));
+  double* base = ar.p;
+  auto ip = [&](size_t o) { return reinterpret_cast<int32_t*>(base + o); };
+  int32_t* d_count = ip(o_cnt);
+
+  mtg::MelLoopParams lp{};
+  lp.K = p->K;
+  lp.dnf = int(dnf);
+  lp.B = B;
+  lp.max_iterations = q->max_iterations;
+  lp.f_abs = q->f_abs;
+  lp.f_rel = q->f_rel;
+  lp.x_rel = q->x_rel;
+  lp.x_abs = q->x_abs;
+  lp.init_rel = q->initial_stepsize_rel;
+  lp.lower = 0.1;  // kOptimizationTimeLowerBound (polynomial_optimization_nonlinear.h)
+  lp.rel = seg_times_out;
+  lp.iters = ip(o_it);
+  lp.result = ip(o_res);
+  lp.pass = ip(o_pass);
+  lp.opt_status = ip(o_ost);
+  lp.J = base + o_J;
+  lp.g = base + o_g;
+  lp.Jc = base + o_Jc;
+  lp.st_g = ip(o_stg);
+  lp.st_c = ip(o_stc);
+  lp.count_next = d_count;
+  const int threads = 128;
+  int cur = 0;
+  auto set_lists = [&](int c) {
+    lp.idx = ip(o_idx[c]);
+    lp.x = base + o_x[c];
+    lp.alpha = base + o_a[c];
+    lp.dfix = base + o_f[c];
+    lp.idx_next = ip(o_idx[c ^ 1]);
+    lp.x_next = base + o_x[c ^ 1];
+    lp.alpha_next = base + o_a[c ^ 1];
+    lp.dfix_next = base + o_f[c ^ 1];
+  };
+  // the start lists the iterating rows into list 0
+  set_lists(1);
+  MTG_CUDA(h, cudaMemsetAsync(d_count, 0, sizeof(int32_t), s));
+  mtg::mel_init_kernel<<<(unsigned)((B + threads - 1) / threads), threads, 0, s>>>(lp, seg_times, d_fixed);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  int rows = 0;
+  MTG_TRY(read_count(h, d_count, s, &rows));
+  for (int k = 0; rows > 0; ++k) {
+    set_lists(cur);
+    lp.rows = rows;
+    lp.k = k;
+    const unsigned blocks = (unsigned)((rows + threads - 1) / threads);
+    MTG_CUDA(h, cudaMemsetAsync(ip(o_stg), 0, sizeof(int32_t) * size_t(rows) * (K + 1), s));
+    MTG_CUDA(h, cudaMemsetAsync(ip(o_stc), 0, sizeof(int32_t) * size_t(rows) * kL, s));
+    MTG_TRY(launch_mellinger(h, p, topo, rows, lp.x, lp.dfix, base + o_J, base + o_g, s, slot, ip(o_stg)));
+    if (k == 0) {
+      mtg::mel_alpha0_kernel<<<blocks, threads, 0, s>>>(lp, base + o_a[cur]);
+      MTG_CUDA(h, cudaGetLastError());
+      h->launches++;
+    }
+    // K = 1: every gradient is zero (getCostAndGradientMellinger), so every row stops with SUCCESS: no candidates
+    if (p->K > 1) MTG_TRY(launch_line_search(h, p, topo, lp, base + o_Jc, ip(o_stc), s, slot));
+    MTG_CUDA(h, cudaMemsetAsync(d_count, 0, sizeof(int32_t), s));
+    mtg::mel_update_kernel<<<blocks, threads, 0, s>>>(lp);
+    MTG_CUDA(h, cudaGetLastError());
+    h->launches++;
+    MTG_TRY(read_count(h, d_count, s, &rows));
+    cur ^= 1;
+  }
+  if (relative_times)
+    MTG_CUDA(h, cudaMemcpyAsync(relative_times, seg_times_out, sizeof(double) * nB * K, cudaMemcpyDeviceToDevice, s));
+  MTG_TRY(launch_scale_with_violation(h, p, topo, B, seg_times_out, d_fixed, v_max, a_max, coeffs, seg_times_out,
+                                      within_range, maxima, ip(o_sst), s, slot, ip(o_pass)));
+  if (cost) MTG_TRY(launch_cost(h, p, B, seg_times_out, coeffs, cost, s));
+  const int64_t fb = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
+  mtg::mel_finish_kernel<<<(unsigned)fb, threads, 0, s>>>(B, ip(o_it), ip(o_res), ip(o_ost), ip(o_sst), iterations,
+                                                          result, status);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  return arena_release(h, ar, s);
+}
+
+int mtg_optimize_time_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                          const double* d_fixed, const mtg_mellinger_params* params, double v_max,
+                                          double a_max, double* coeffs, double* seg_times_out, double* relative_times,
+                                          double* cost, int32_t* iterations, int32_t* result, int32_t* within_range,
+                                          double* maxima, int32_t* status, void* stream) {
+  return run_problem_entry(
+      h, valid_optimize(p, B, params, v_max, a_max, seg_times, d_fixed, coeffs, seg_times_out), p, B,
+      [&](CachedTopology* topo) {
+        return launch_optimize_mellinger(h, p, topo, B, seg_times, d_fixed, params, v_max, a_max, coeffs,
+                                         seg_times_out, relative_times, cost, iterations, result, within_range, maxima,
+                                         status, (cudaStream_t)stream, mtg_handle::kPipe);
       });
 }
 
@@ -2256,6 +2463,34 @@ int mtg_scale_times_with_violation_batch_host_f64(mtg_handle* h, const mtg_probl
         return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
           return launch_scale_with_violation(h, p, topo, nb, d[0], d[1], v_max, a_max, d[2], d[0], d[3], d[4], d[5], s,
                                              slot);
+        });
+      });
+}
+
+int mtg_optimize_time_mellinger_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                               const double* d_fixed, const mtg_mellinger_params* params, double v_max,
+                                               double a_max, double* coeffs, double* seg_times_out,
+                                               double* relative_times, double* cost, int32_t* iterations,
+                                               int32_t* result, int32_t* within_range, double* maxima,
+                                               int32_t* status) {
+  return run_problem_entry(
+      h, valid_optimize(p, B, params, v_max, a_max, seg_times, d_fixed, coeffs, seg_times_out), p, B,
+      [&](CachedTopology* topo) {
+        const size_t K = p->K, D = p->D, N = p->N;
+        // the times go in from seg_times and come back, optimised and stretched in place, into seg_times_out
+        const HostBuf bufs[] = {{seg_times, seg_times_out, K * 8},
+                                {d_fixed, nullptr, D * topo->layout.n_fixed * 8},
+                                {nullptr, coeffs, K * D * N * 8},
+                                {nullptr, relative_times, K * 8},
+                                {nullptr, cost, 8},
+                                {nullptr, iterations, 4},
+                                {nullptr, result, 4},
+                                {nullptr, within_range, 4},
+                                {nullptr, maxima, 16},
+                                {nullptr, status, 4}};
+        return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+          return launch_optimize_mellinger(h, p, topo, nb, d[0], d[1], params, v_max, a_max, d[2], d[0], d[3], d[4],
+                                           d[5], d[6], d[7], d[8], d[9], s, slot);
         });
       });
 }

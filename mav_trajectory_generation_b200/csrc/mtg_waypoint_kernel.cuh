@@ -45,9 +45,17 @@ struct WaypointParams {
   // read waypoints [B][K+1][D] instead of (times, dfix), compute the segment times with
   // estimateSegmentTimesNfabian (reference src/vertex.cpp:255-272) and use zero start/end derivatives
   // (Vertex::makeStartOrEnd, src/vertex.cpp:147-153).
-  const double* __restrict__ positions;
+  // The line-search instantiation of the cost-only mode (below) reads its step and gradient pointers in the places of
+  // the fused inputs' pointers, which it never reads: the parameter block of every kernel keeps its size.
+  union {
+    const double* __restrict__ positions;
+    const double* __restrict__ ls_grad;   // [rows][K]
+  };
   double v_max, a_max, magic;
-  double* __restrict__ times_out;     // [B][K] or null
+  union {
+    double* __restrict__ times_out;     // [B][K] or null
+    const double* __restrict__ ls_alpha;  // [rows]
+  };
   // cost-only mode (SURVEY.md 8f-2, the nonlinear optimiser's inner loop): no coefficients are written; the
   // kernel returns computeCost() of every problem.  With mel_k1 = K+1 the batch is the Mellinger expansion
   // (reference impl/polynomial_optimization_nonlinear_impl.h:286-364) generated on the fly: problem q belongs to
@@ -56,12 +64,24 @@ struct WaypointParams {
   double* __restrict__ cost;          // [B] or null
   int mel_k1;
   double mel_inc, mel_lower;
+  // cost-only mode, line-search instantiation (the Mellinger outer loop's candidates): problem q is candidate
+  // j = q % kLineSearchSteps of row q / kLineSearchSteps, at line_search_time(x, g, line_search_step(alpha, j),
+  // mel_lower) per segment, where x = `times`, g = ls_grad and alpha = ls_alpha are the UNEXPANDED rows.
 };
 
 __device__ __forceinline__ double mellinger_time(double t, int i, int n, double inc, double corr, double lower) {
   if (n < 0) return t;
   const double v = (i == n) ? t + inc : t - corr;
   return v > lower ? v : lower;  // std::max(kOptimizationTimeLowerBound, t)
+}
+
+// Step sizes tried per row and iteration by the Mellinger outer loop: alpha * 2^(1 - j), j = 0..kLineSearchSteps-1
+constexpr int kLineSearchSteps = 8;
+__device__ __forceinline__ double line_search_step(double alpha, int j) { return __dmul_rn(alpha, ldexp(1.0, 1 - j)); }
+// max(lower, fl(x - fl(step * g))): two roundings (no FMA), the same max form as mellinger_time
+__device__ __forceinline__ double line_search_time(double x, double g, double step, double lower) {
+  const double v = __dsub_rn(x, __dmul_rn(step, g));
+  return v > lower ? v : lower;
 }
 
 // t = distance / v_max * 2 * (1 + magic * v_max / a_max * exp(-distance / v_max * 2)), evaluated in the

@@ -54,6 +54,12 @@ void packFixed(const Topology& topo, const Vertex::Vector& vertices, double* d_f
 bool sameTopology(const Topology& topo, const Vertex::Vector& vertices);
 void unpackSegments(const Topology& topo, const double* coeffs, const double* times, Segment::Vector* segments);
 
+// The stopping rules of the Mellinger outer loop (mtg_mellinger_params; NonlinearOptimizationParameters' defaults)
+struct MellingerParameters {
+  double f_abs = -1.0, f_rel = 0.05, x_rel = -1.0, x_abs = -1.0, initial_stepsize_rel = 0.1;
+  int max_iterations = 3000;
+};
+
 class LinearCore {
  public:
   LinearCore(int N, size_t dimension);
@@ -67,6 +73,12 @@ class LinearCore {
   void getM(Eigen::MatrixXd* M) const;
   void getMpinv(Eigen::MatrixXd* M_pinv) const;
   void getR(Eigen::MatrixXd* R) const;
+  // mtg_optimize_time_mellinger_batch_f64 on this one problem: segment_times_ and the segments take the optimised,
+  // stretched result.  Returns false when the call fails; *result gets the MTG_OPTIMIZE_RESULT_* code.
+  bool optimizeTimeMellinger(const MellingerParameters& params, double v_max, double a_max, int* result,
+                             int* iterations, std::vector<double>* relative_times);
+  // mtg_scale_times_with_violation_batch_f64 on this one problem, in place
+  bool scaleSegmentTimesWithViolation(double v_max, double a_max);
 
   int N_;
   size_t dimension_;
@@ -122,6 +134,12 @@ class BatchCore {
   // PolynomialOptimizationNonLinear::scaleSegmentTimesWithViolation: solve at times_, stretch times_, re-solve into
   // coeffs_ with d_fixed_; status_ receives the OR of the three steps' status bits
   bool scaleSegmentTimesWithViolation(double v_max, double a_max, std::vector<uint8_t>* within_range);
+  // PolynomialOptimizationNonLinear::optimize() with kMellingerOuterLoop (mtg_optimize_time_mellinger_batch_f64):
+  // times_ and coeffs_ take the optimised, stretched result in place, status_ the entry's status bits.  result,
+  // iterations: [B]; relative_times: [B][K], the times before the stretch; all three nullable.
+  bool optimizeTimeMellingerOuterLoop(const MellingerParameters& params, double v_max, double a_max,
+                                      std::vector<int>* result, std::vector<int>* iterations,
+                                      std::vector<double>* relative_times);
   // which reference checker checkInputFeasibility runs
   enum class InputChecker { kAnalytic, kRecursive, kSampling };
   // FeasibilityAnalytic, FeasibilityRecursive or FeasibilitySampling ::checkInputFeasibilityTrajectory of the current

@@ -105,6 +105,16 @@ class BatchPolynomialOptimization {
   bool scaleSegmentTimesWithViolation(double v_max, double a_max, std::vector<uint8_t>* within_range = nullptr) {
     return core_.scaleSegmentTimesWithViolation(v_max, a_max, within_range);
   }
+  // PolynomialOptimizationNonLinear::optimize() with kMellingerOuterLoop (reference
+  // impl/polynomial_optimization_nonlinear_impl.h:171-259) for every problem, as mtg_optimize_time_mellinger_batch_f64
+  // defines the descent: segmentTimes() and coefficients() take the optimised, stretched result in place, status()
+  // the status bits.  result (MTG_OPTIMIZE_RESULT_*, the nlopt_result values), iterations and relative_times (the
+  // times before the stretch, [B][K]) are nullable.  v_max / a_max: +inf for no limit.
+  bool optimizeTimeMellingerOuterLoop(const b200::MellingerParameters& params, double v_max, double a_max,
+                                      std::vector<int>* result = nullptr, std::vector<int>* iterations = nullptr,
+                                      std::vector<double>* relative_times = nullptr) {
+    return core_.optimizeTimeMellingerOuterLoop(params, v_max, a_max, result, iterations, relative_times);
+  }
   // FeasibilityAnalytic::checkInputFeasibilityTrajectory (reference mav_trajectory_generation_ros/src/
   // feasibility_analytic.cpp, feasibility_base.cpp) of every trajectory at its current coefficients, on the GPU:
   // result[b], and segment[b] = the first segment that is not feasible (-1 when the row is feasible or has a segment

@@ -27,6 +27,9 @@
 
 namespace mav_trajectory_generation {
 
+template <int _N>
+class PolynomialOptimizationNonLinear;
+
 template <int _N = 10>
 class PolynomialOptimization {
   static_assert(_N % 2 == 0, "The number of coefficients has to be even.");
@@ -186,6 +189,8 @@ class PolynomialOptimization {
   int getLastStatus() const { return core_.last_status_; }
 
  private:
+  template <int>
+  friend class PolynomialOptimizationNonLinear;  // runs the time optimiser on this problem's core
   b200::LinearCore core_;
 };
 

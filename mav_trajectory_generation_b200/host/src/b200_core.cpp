@@ -63,6 +63,16 @@ struct HandleLock {
   HandleLock() { lockHandle(); }
   ~HandleLock() { unlockHandle(); }
 };
+mtg_mellinger_params toParams(const MellingerParameters& q) {
+  mtg_mellinger_params p;
+  p.f_abs = q.f_abs;
+  p.f_rel = q.f_rel;
+  p.x_rel = q.x_rel;
+  p.x_abs = q.x_abs;
+  p.initial_stepsize_rel = q.initial_stepsize_rel;
+  p.max_iterations = q.max_iterations;
+  return p;
+}
 }  // namespace
 
 void hostMappingMatrix(int N, double T, double* A) {
@@ -301,6 +311,59 @@ bool LinearCore::solveLinear() {
     free_constraints_compact_[d] = Eigen::VectorXd::Zero(topo_.n_free);
     for (int c = 0; c < topo_.n_free; ++c) free_constraints_compact_[d][c] = d_free[size_t(d) * topo_.n_free + c];
   }
+  unpack(coeffs);
+  return true;
+}
+
+bool LinearCore::optimizeTimeMellinger(const MellingerParameters& params, double v_max, double a_max, int* result,
+                                       int* iterations, std::vector<double>* relative_times) {
+  CHECK(topo_.r >= 0 && topo_.r <= N_ / 2 - 1);
+  const int D = topo_.D;
+  std::vector<double> d_fixed(size_t(D) * topo_.n_fixed), coeffs(size_t(topo_.K) * D * N_), rel(topo_.K);
+  for (int d = 0; d < D; ++d)
+    for (int c = 0; c < topo_.n_fixed; ++c) d_fixed[size_t(d) * topo_.n_fixed + c] = fixed_constraints_compact_[d][c];
+  const mtg_mellinger_params prm = toParams(params);
+  int32_t res = 0, it = 0, status = 0;
+  mtg_problem p = {N_, topo_.r, topo_.K, D, topo_.mask.data()};
+  {
+    HandleLock lock;
+    mtg_handle* h = defaultHandle();
+    const int rc = mtg_optimize_time_mellinger_batch_host_f64(h, &p, 1, segment_times_.data(), d_fixed.data(), &prm,
+                                                              v_max, a_max, coeffs.data(), segment_times_.data(),
+                                                              rel.data(), nullptr, &it, &res, nullptr, nullptr,
+                                                              &status);
+    if (rc != MTG_OK) {
+      LOG(ERROR) << "mtg_optimize_time_mellinger_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+      return false;
+    }
+  }
+  last_status_ = status;
+  if (result) *result = res;
+  if (iterations) *iterations = it;
+  if (relative_times) *relative_times = rel;
+  unpack(coeffs);
+  return true;
+}
+
+bool LinearCore::scaleSegmentTimesWithViolation(double v_max, double a_max) {
+  const int D = topo_.D;
+  std::vector<double> d_fixed(size_t(D) * topo_.n_fixed), coeffs(size_t(topo_.K) * D * N_);
+  for (int d = 0; d < D; ++d)
+    for (int c = 0; c < topo_.n_fixed; ++c) d_fixed[size_t(d) * topo_.n_fixed + c] = fixed_constraints_compact_[d][c];
+  int32_t status = 0;
+  mtg_problem p = {N_, topo_.r, topo_.K, D, topo_.mask.data()};
+  {
+    HandleLock lock;
+    mtg_handle* h = defaultHandle();
+    const int rc = mtg_scale_times_with_violation_batch_host_f64(h, &p, 1, segment_times_.data(), d_fixed.data(), v_max,
+                                                                 a_max, coeffs.data(), segment_times_.data(), nullptr,
+                                                                 nullptr, &status);
+    if (rc != MTG_OK) {
+      LOG(ERROR) << "mtg_scale_times_with_violation_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+      return false;
+    }
+  }
+  last_status_ = status;
   unpack(coeffs);
   return true;
 }
@@ -705,6 +768,28 @@ bool BatchCore::scaleSegmentTimesWithViolation(double v_max, double a_max, std::
     return false;
   }
   copyWithinRange(within, within_range);
+  return true;
+}
+
+bool BatchCore::optimizeTimeMellingerOuterLoop(const MellingerParameters& params, double v_max, double a_max,
+                                               std::vector<int>* result, std::vector<int>* iterations,
+                                               std::vector<double>* relative_times) {
+  CHECK_GT(B_, 0u) << "setup first";
+  std::vector<int32_t> res(B_, 0), it(B_, 0);
+  if (relative_times) relative_times->assign(B_ * size_t(topo_.K), 0.0);
+  const mtg_mellinger_params prm = toParams(params);
+  mtg_problem p = {N_, topo_.r, topo_.K, topo_.D, topo_.mask.data()};
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_optimize_time_mellinger_batch_host_f64(
+      h, &p, static_cast<int64_t>(B_), times_, d_fixed_, &prm, v_max, a_max, coeffs_, times_,
+      relative_times ? relative_times->data() : nullptr, nullptr, it.data(), res.data(), nullptr, nullptr, status_);
+  if (rc != MTG_OK) {
+    LOG(ERROR) << "mtg_optimize_time_mellinger_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+    return false;
+  }
+  if (result) result->assign(res.begin(), res.end());
+  if (iterations) iterations->assign(it.begin(), it.end());
   return true;
 }
 
