@@ -4,12 +4,14 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <initializer_list>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/mtg_b200.h"
@@ -410,6 +412,59 @@ int set_carveout(mtg_handle* h, const void* fn, int percent) {
   return MTG_OK;
 }
 
+// ---- launches: every kernel of the library goes through launch_kernel() -------------------------------------------
+// Blocks of `per_block` items for `work` items, at most `per_sm` resident or grid-strided blocks per SM.
+int64_t capped_grid(const mtg_handle* h, int64_t work, int64_t per_block, int per_sm) {
+  return std::min<int64_t>((work + per_block - 1) / per_block, int64_t(per_sm) * h->sm_count);
+}
+
+// fn<<<grid, block, smem, s>>>(args...), its launch error checked and the launch counted (mtg_launch_count).  A launch
+// with dynamic shared memory first raises fn's limit to `smem` (ensure_dyn_smem); one without makes no attribute call.
+template <class... P, class... A>
+int launch_kernel(mtg_handle* h, void (*fn)(P...), int64_t grid, int block, size_t smem, cudaStream_t s, A&&... args) {
+  if (smem > 0) MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
+  fn<<<(unsigned)grid, block, smem, s>>>(std::forward<A>(args)...);
+  MTG_CUDA(h, cudaGetLastError());
+  h->launches++;
+  return MTG_OK;
+}
+
+// The segment-parallel kernels (extrema, time scaling, input feasibility, half planes): kExtremaThreads threads per
+// block in rows of K threads, one trajectory per row, with `row_smem` bytes of dynamic shared memory per row.  When
+// the rows of a block need more shared memory than a block may have, `entry` fails with "<entry>: <what> too large".
+template <class Params>
+int launch_segment_parallel(mtg_handle* h, void (*fn)(Params, int), const Params& prm, int K, int64_t B,
+                            size_t row_smem, const char* entry, const char* what, cudaStream_t s) {
+  const int tpb = std::max(1, mtg::kExtremaThreads / K);
+  const size_t smem = size_t(tpb) * row_smem;
+  if (smem > h->smem_optin) {
+    h->error = std::string(entry) + ": " + what + " too large";
+    return MTG_ERR_BAD_ARG;
+  }
+  return launch_kernel(h, fn, capped_grid(h, B, tpb, 16), mtg::kExtremaThreads, smem, s, prm, tpb);
+}
+
+// ---- kernel tables: one instantiation per order N -----------------------------------------------------------------
+// The (N, A) of one instantiation; A is the second template parameter where a kernel has one (the flat-state
+// attitude case, the masked kernel's dimension group).
+template <int N_, int A_>
+struct Inst {
+  static constexpr int N = N_, A = A_;
+};
+template <int N0, int STEP, int A0, int NA, class Pick, size_t... I>
+auto kernel_table(Pick pick, std::index_sequence<I...>) {
+  return std::array{pick(Inst<N0 + STEP * int(I / NA), A0 + int(I % NA)>{})...};
+}
+// The kernel `pick(Inst<n, a>{})` from a table, built on first use, of one instantiation per N in {N0, N0 + STEP, ...,
+// N1} and A in [A0, A1].  Takes arguments in those ranges.
+template <int N0, int N1, int STEP = 1, int A0 = 0, int A1 = 0, class Pick>
+auto kernel_by_n(Pick pick, int n, int a = A0) {
+  constexpr int NA = A1 - A0 + 1;
+  static const auto table =
+      kernel_table<N0, STEP, A0, NA>(pick, std::make_index_sequence<((N1 - N0) / STEP + 1) * NA>{});
+  return table[size_t((n - N0) / STEP * NA + (a - A0))];
+}
+
 struct DeviceGuard {
   int prev = -1;
   explicit DeviceGuard(int dev) {
@@ -613,7 +668,7 @@ int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, in
       pl->fn = (const void*)e.k3_pair;
       pl->threads = 64;
       pl->smem = smem;
-      pl->blocks = std::min<int64_t>((B + 15) / 16, int64_t(ctas) * h->sm_count);
+      pl->blocks = capped_grid(h, B, 16, ctas);
       pl->chunk = C;
       if (nmax > C) pl->park_bytes = size_t(nmax - C) * e.k3_park * size_t(pl->blocks) * 64 * sizeof(double);
       pl->carveout = carveout;
@@ -626,7 +681,7 @@ int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, in
   pl->fn = (const void*)e.k3[best_i];
   pl->threads = 32 * W;
   pl->smem = best_smem;
-  pl->blocks = std::min<int64_t>((B + 16 * W - 1) / (16 * W), int64_t(best_ctas) * h->sm_count);
+  pl->blocks = capped_grid(h, B, 16 * W, best_ctas);
   if (npark > 0) pl->park_bytes = size_t(npark) * e.k3_park * size_t(pl->blocks) * pl->threads * sizeof(double);
   pl->carveout = best_carveout;
   return MTG_OK;
@@ -687,7 +742,7 @@ int plan_waypoint(mtg_handle* h, const mtg_problem* p, const Layout& L, const Wa
         if (!f) return MTG_ERR_CUDA;
         if (65536 / (std::max(f->regs, 1) * mtg::kTmemThreads) >= ctas) pl->fn = fe;
       }
-      pl->blocks = std::min<int64_t>((B + 63) / 64, int64_t(ctas) * h->sm_count);
+      pl->blocks = capped_grid(h, B, 64, ctas);
       const int64_t tiles_per_warp = (B / 16) / std::max<int64_t>(1, pl->blocks * 4);
       pl->tile_counter = h->dynamic_tiles == 1 || (h->dynamic_tiles == 0 && tiles_per_warp >= 8 && K > kV4MaxK);
       return MTG_OK;
@@ -707,7 +762,7 @@ int plan_waypoint(mtg_handle* h, const mtg_problem* p, const Layout& L, const Wa
       pl->fn = fn;
       pl->threads = mtg::kTmemThreads;
       pl->smem = smem;
-      pl->blocks = per_tile ? tiles : std::min<int64_t>(tiles, int64_t(ctas) * h->sm_count);
+      pl->blocks = per_tile ? tiles : capped_grid(h, B, 64, ctas);
       pl->tile_counter = !per_tile && (h->dynamic_tiles == 1 || (h->dynamic_tiles == 0 && tiles_per_warp >= 16));
       return MTG_OK;
     }
@@ -752,45 +807,38 @@ int launch_waypoint(mtg_handle* h, const mtg_problem* p, const WaypointPlan& pl,
     held = &h->scratch[slot];
     MTG_TRY(arena_acquire(h, *held, pl.park_bytes, stream));
   }
+  // raised before the carveout and the tensor map (launch_kernel() then finds it raised)
   MTG_TRY(ensure_dyn_smem(h, pl.fn, pl.smem));
   if (pl.carveout >= 0) MTG_TRY(set_carveout(h, pl.fn, pl.carveout));
   const CUtensorMap* tmap = nullptr;
   if (pl.family != Family::Sweep) MTG_TRY(coeff_tmap(h, prm.coeffs, prm.B, p, p->D * p->N, &tmap));
-  const unsigned grid = (unsigned)pl.blocks;
+  const int64_t grid = pl.blocks;
+  const int block = pl.threads;
   switch (pl.family) {
     case Family::Sweep:
-      ((SweepKernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm);
+      MTG_TRY(launch_kernel(h, (SweepKernel)pl.fn, grid, block, pl.smem, stream, prm));
       break;
     case Family::Tmem:
-      ((TmemKernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm, *tmap);
+      MTG_TRY(launch_kernel(h, (TmemKernel)pl.fn, grid, block, pl.smem, stream, prm, *tmap));
       break;
     case Family::V4:
-      ((V4Kernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm, mtg::TmemLaunchV4{counter}, *tmap);
+      MTG_TRY(launch_kernel(h, (V4Kernel)pl.fn, grid, block, pl.smem, stream, prm, mtg::TmemLaunchV4{counter}, *tmap));
       break;
-    case Family::V5:
-      ((V5Kernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm, mtg::TmemLaunchV5{pl.n_buffers, counter}, *tmap);
+    case Family::V5: {
+      const mtg::TmemLaunchV5 v5{pl.n_buffers, counter};
+      MTG_TRY(launch_kernel(h, (V5Kernel)pl.fn, grid, block, pl.smem, stream, prm, v5, *tmap));
       break;
+    }
     case Family::Chunked: {
       const mtg::ChunkedLaunch cl{pl.chunk, pl.park_bytes > 0 ? held->p : nullptr, pl.evict_first};
-      ((ChunkedKernel)pl.fn)<<<grid, pl.threads, pl.smem, stream>>>(prm, cl, *tmap);
+      MTG_TRY(launch_kernel(h, (ChunkedKernel)pl.fn, grid, block, pl.smem, stream, prm, cl, *tmap));
       break;
     }
   }
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
   return held ? arena_release(h, *held, stream) : MTG_OK;
 }
 
 // ---- K4: masked block-tridiagonal kernel, any mask; N in {2..12}, dimension groups of 1..4
-typedef void (*MaskedKernel)(const mtg::MaskedParams, const CUtensorMap);
-#define MTG_MASKED_ROW(N_)                                                                                  \
-  {                                                                                                         \
-    mtg::masked_block_kernel<N_, 1>, mtg::masked_block_kernel<N_, 2>, mtg::masked_block_kernel<N_, 3>,     \
-        mtg::masked_block_kernel<N_, 4>                                                                     \
-  }
-const MaskedKernel kMaskedKernels[6][4] = {MTG_MASKED_ROW(2), MTG_MASKED_ROW(4),  MTG_MASKED_ROW(6),
-                                           MTG_MASKED_ROW(8), MTG_MASKED_ROW(10), MTG_MASKED_ROW(12)};
-
 int launch_masked(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B, const double* times,
                   const double* dfix, double* coeffs, double* dfree, int32_t* status, cudaStream_t stream, int slot) {
   const Layout& L = topo->layout;
@@ -813,23 +861,22 @@ int launch_masked(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int
   for (int d0 = 0; d0 < p->D;) {
     const int rem = p->D - d0;
     const int dg = rem > 4 ? (rem == 5 ? 3 : 4) : rem;  // 5 = 3 + 2 rather than 4 + 1
-    MaskedKernel fn = kMaskedKernels[p->N / 2 - 1][dg - 1];
+    const auto fn = kernel_by_n<2, MTG_MAX_N, 2, 1, 4>(
+        [](auto k) { return mtg::masked_block_kernel<decltype(k)::N, decltype(k)::A>; }, p->N, dg);
     const int kslots = hh * (hh + 1) / 2 + hh * dg;
     const size_t smem = size_t(4) * 32 * dg * p->N * sizeof(double);  // staging tiles of the four warps
-    MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
+    MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));  // before the occupancy query
     int per_sm = 0;
     MTG_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)fn, 128, smem));
     per_sm = std::max(per_sm, 1);
-    const int64_t blocks = std::min<int64_t>((B + 127) / 128, int64_t(per_sm) * h->sm_count);
+    const int64_t blocks = capped_grid(h, B, 128, per_sm);
     const size_t bytes = size_t(p->K + 1) * kslots * size_t(blocks) * 128 * sizeof(double);
     MTG_TRY(arena_acquire(h, ar, bytes, stream));
     prm.lifo = ar.p;
     prm.d0 = d0;
     const CUtensorMap* tmap = nullptr;
     MTG_TRY(coeff_tmap(h, coeffs, B, p, dg * p->N, &tmap));
-    fn<<<(unsigned)blocks, 128, smem, stream>>>(prm, *tmap);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
+    MTG_TRY(launch_kernel(h, fn, blocks, 128, smem, stream, prm, *tmap));
     MTG_TRY(arena_release(h, ar, stream));
     d0 += dg;
   }
@@ -865,13 +912,9 @@ int launch_cost_fused(mtg_handle* h, const mtg_problem* p, CachedTopology* topo,
   prm.mel_lower = lower;
   prm.ls_grad = ls_grad;
   prm.ls_alpha = ls_alpha;
-  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
   CUtensorMap tmap;
   std::memset(&tmap, 0, sizeof(tmap));  // unused by the cost-only instantiations
-  fn<<<(unsigned)((nx + 63) / 64), mtg::kTmemThreads, smem, stream>>>(prm, tmap);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
+  return launch_kernel(h, fn, (nx + 63) / 64, mtg::kTmemThreads, smem, stream, prm, tmap);
 }
 
 int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B, const double* times,
@@ -929,22 +972,15 @@ int launch_solve(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int6
   int64_t blocks = (B + threads - 1) / threads;
   const int64_t max_blocks = int64_t(h->sm_count) * 8;
   if (blocks > max_blocks) blocks = max_blocks;
-  if (kind == MTG_KERNEL_NOFREE) {
-    mtg::backsub_kernel<<<(unsigned)blocks, threads, 0, stream>>>(prm);
-  } else {
-    const size_t per_thread = size_t(L.n_free) * (L.bw + 1 + p->D);
-    const size_t bytes = per_thread * size_t(blocks) * threads * sizeof(double);
-    mtg_handle::Arena& ar = h->scratch[slot];
-    MTG_TRY(arena_acquire(h, ar, bytes, stream));
-    prm.scratch = ar.p;
-    prm.scratch_stride = blocks * threads;
-    mtg::generic_solve_kernel<<<(unsigned)blocks, threads, 0, stream>>>(prm);
-    MTG_CUDA(h, cudaGetLastError());
-    MTG_TRY(arena_release(h, ar, stream));
-  }
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
+  if (kind == MTG_KERNEL_NOFREE) return launch_kernel(h, mtg::backsub_kernel, blocks, threads, 0, stream, prm);
+  const size_t per_thread = size_t(L.n_free) * (L.bw + 1 + p->D);
+  const size_t bytes = per_thread * size_t(blocks) * threads * sizeof(double);
+  mtg_handle::Arena& ar = h->scratch[slot];
+  MTG_TRY(arena_acquire(h, ar, bytes, stream));
+  prm.scratch = ar.p;
+  prm.scratch_stride = blocks * threads;
+  MTG_TRY(launch_kernel(h, mtg::generic_solve_kernel, blocks, threads, 0, stream, prm));
+  return arena_release(h, ar, stream);
 }
 
 int ensure_pipe(mtg_handle* h, int i, size_t bytes) {
@@ -1081,29 +1117,6 @@ int stage_host(mtg_handle* h, int64_t B, Staging staging, const HostBuf (&bufs)[
   return MTG_OK;
 }
 
-// ---- flat-state kernel tables -------------------------------------------------------------------------------------
-int flat_attitude(int32_t D) { return D == 4 ? mtg::kAttYaw : D == 6 ? mtg::kAttRotationVector : mtg::kAttNone; }
-
-// kernel `Kern<N, ATT>` of every N in [1, 12] and attitude case, indexed [ATT][N - 1]
-template <template <int, int> class Kern, class Fn>
-Fn flat_state_kernel(int32_t N, int32_t D) {
-  static const Fn kTable[3][MTG_MAX_N] = {
-#define MTG_FLAT_ROW(A)                                                                                              \
-  {Kern<1, A>::fn, Kern<2, A>::fn, Kern<3, A>::fn, Kern<4, A>::fn,   Kern<5, A>::fn,  Kern<6, A>::fn,                \
-   Kern<7, A>::fn, Kern<8, A>::fn, Kern<9, A>::fn, Kern<10, A>::fn, Kern<11, A>::fn, Kern<12, A>::fn}
-      MTG_FLAT_ROW(mtg::kAttNone), MTG_FLAT_ROW(mtg::kAttYaw), MTG_FLAT_ROW(mtg::kAttRotationVector)};
-#undef MTG_FLAT_ROW
-  return kTable[flat_attitude(D)][N - 1];
-}
-template <int N, int ATT>
-struct FlatRangeKernel {
-  static constexpr void (*fn)(const mtg::RangeParams) = mtg::flat_state_range_kernel<N, ATT>;
-};
-template <int N, int ATT>
-struct FlatAtTimeKernel {
-  static constexpr void (*fn)(const mtg::FlatAtTimeParams) = mtg::flat_state_at_time_kernel<N, ATT>;
-};
-
 }  // namespace
 
 extern "C" {
@@ -1238,7 +1251,9 @@ int mtg_problem_layout(const mtg_problem* p, mtg_layout* out, int32_t* slot_col)
 // ---- the compute entry points ------------------------------------------------------------------------------------
 // Each kind has one argument check, shared by its device entry and its host twin, and one launcher, which takes
 // checked arguments and launches on `s` (with the arenas of pipeline slot `slot` where it uses any).  A device entry
-// is run_entry() around its launcher; a host entry is run_entry() around stage_host() around the same launcher.
+// is run_entry() around its launcher; a host entry is run_entry() around stage_host() around the same launcher.  Each
+// launcher starts its kernels with launch_kernel(), sized by capped_grid() (the segment-parallel ones through
+// launch_segment_parallel()), and picks an order's instantiation with kernel_by_n().
 
 // the entries of one constraint problem with three arrays that every row needs (solve, setFreeConstraints,
 // computeCost, the Mellinger gradient)
@@ -1302,11 +1317,7 @@ static int launch_nfabian(mtg_handle* h, const mtg_problem* p, CachedTopology* t
   pk.magic = magic;
   pk.times = t_buf;
   pk.dfix = f_buf;
-  const int threads = 128;
-  const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
-  mtg::nfabian_pack_kernel<<<(unsigned)blocks, threads, 0, s>>>(pk);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
+  MTG_TRY(launch_kernel(h, mtg::nfabian_pack_kernel, capped_grid(h, B, 128, 16), 128, 0, s, pk));
   MTG_TRY(launch_solve(h, p, topo, B, t_buf, f_buf, nullptr, coeffs, nullptr, status, s, false, nullptr, slot));
   return arena_release(h, ar, s);  // the solve was the last reader of the packed inputs
 }
@@ -1358,12 +1369,7 @@ static int launch_cost(mtg_handle* h, const mtg_problem* p, int64_t B, const dou
   CostFn fn = mtg::cost_kernel<0, 0>;
   for (const auto& e : kComputeCostKernels)
     if (e.N == p->N && e.r == p->r) fn = e.fn;
-  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
-  int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
-  fn<<<(unsigned)blocks, threads, smem, s>>>(prm, tpb);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
+  return launch_kernel(h, fn, capped_grid(h, B, tpb, 16), threads, smem, s, prm, tpb);
 }
 
 int mtg_compute_cost_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
@@ -1396,19 +1402,9 @@ int mtg_evaluate_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64
     }
     const int threads = std::max(32, std::min(256, int((40 * 1024) / (D * 8)) / 32 * 32));
     const size_t smem = size_t(threads) * D * sizeof(double);
-    typedef void (*EvalFn)(const mtg::EvalParams);
-    static const EvalFn kEval[MTG_MAX_N] = {
-        mtg::evaluate_kernel<1>, mtg::evaluate_kernel<2>,  mtg::evaluate_kernel<3>,  mtg::evaluate_kernel<4>,
-        mtg::evaluate_kernel<5>, mtg::evaluate_kernel<6>,  mtg::evaluate_kernel<7>,  mtg::evaluate_kernel<8>,
-        mtg::evaluate_kernel<9>, mtg::evaluate_kernel<10>, mtg::evaluate_kernel<11>, mtg::evaluate_kernel<12>};
-    const EvalFn fn = kEval[N - 1];
-    MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
-    const int64_t total = B * int64_t(n_samples);
-    const int64_t blocks = std::min<int64_t>((total + threads - 1) / threads, int64_t(h->sm_count) * 32);
-    fn<<<(unsigned)blocks, threads, smem, (cudaStream_t)stream>>>(ep);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
-    return MTG_OK;
+    const auto fn = kernel_by_n<1, MTG_MAX_N>([](auto k) { return mtg::evaluate_kernel<decltype(k)::N>; }, N);
+    return launch_kernel(h, fn, capped_grid(h, B * int64_t(n_samples), threads, 32), threads, smem,
+                         (cudaStream_t)stream, ep);
   });
 }
 
@@ -1424,14 +1420,22 @@ static bool valid_range(int32_t N, int32_t K, int32_t D, int64_t B, double dt, i
   return valid_rows(B, {seg_times, coeffs, n_samples}) && (B == 0 || max_samples == 0 || out);
 }
 
+// range_walk_kernel over the rows of `rp`: each sample's segment and local time, into rp.t_local and rp.seg_idx in
+// pipeline slot `slot`'s pack arena, which this acquires.  The caller evaluates the samples and releases the arena.
+static int walk_range(mtg_handle* h, mtg::RangeParams& rp, cudaStream_t s, int slot) {
+  const size_t ns = size_t(rp.B) * size_t(std::max(rp.max_samples, 1));
+  mtg_handle::Arena& ar = h->pack[slot];
+  const size_t o_idx = align_doubles(ns);  // t_local first (doubles), then seg_idx (int32)
+  MTG_TRY(arena_acquire(h, ar, (o_idx + align_doubles((ns + 1) / 2)) * 8, s));
+  rp.t_local = ar.p;
+  rp.seg_idx = reinterpret_cast<int*>(ar.p + o_idx);
+  return launch_kernel(h, mtg::range_walk_kernel, capped_grid(h, rp.B, 128, 16), 128, 0, s, rp);
+}
+
 static int launch_range(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                         const double* coeffs, double t_start, double t_end, double dt, int32_t n_derivs,
                         const int32_t* derivs, int32_t max_samples, double* out, int32_t* n_samples,
                         double* sampling_times, cudaStream_t s, int slot) {
-  const size_t ns = size_t(B) * size_t(std::max(max_samples, 1));
-  mtg_handle::Arena& ar = h->pack[slot];
-  const size_t o_idx = align_doubles(ns);  // t_local first (doubles), then seg_idx (int32)
-  MTG_TRY(arena_acquire(h, ar, (o_idx + align_doubles((ns + 1) / 2)) * 8, s));
   mtg::RangeParams rp;
   rp.N = N;
   rp.K = K;
@@ -1445,20 +1449,13 @@ static int launch_range(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t 
   rp.dt = dt;
   rp.times = seg_times;
   rp.coeffs = coeffs;
-  rp.t_local = ar.p;
-  rp.seg_idx = reinterpret_cast<int*>(ar.p + o_idx);
   rp.n_samples = n_samples;
   rp.sampling_times = sampling_times;
   rp.out = out;
   rp.range_rule = mtg::kRangePlain;
   rp.time_ns = nullptr;
-  {
-    const int threads = 128;
-    const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
-    mtg::range_walk_kernel<<<(unsigned)blocks, threads, 0, s>>>(rp);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
-  }
+  MTG_TRY(walk_range(h, rp, s, slot));
+  mtg_handle::Arena& ar = h->pack[slot];
   if (max_samples > 0) {
     // block size: the output tile (threads * n_derivs * D doubles) stays under 40 KB of shared memory
     const int rec = n_derivs * D;
@@ -1469,18 +1466,8 @@ static int launch_range(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t 
     }
     const int threads = std::max(32, std::min(256, int((40 * 1024) / (rec * 8)) / 32 * 32));
     const size_t smem = size_t(threads) * rec * sizeof(double);
-    typedef void (*RangeEval)(const mtg::RangeParams);
-    static const RangeEval kRangeEval[MTG_MAX_N] = {
-        mtg::range_eval_kernel<1>, mtg::range_eval_kernel<2>,  mtg::range_eval_kernel<3>,  mtg::range_eval_kernel<4>,
-        mtg::range_eval_kernel<5>, mtg::range_eval_kernel<6>,  mtg::range_eval_kernel<7>,  mtg::range_eval_kernel<8>,
-        mtg::range_eval_kernel<9>, mtg::range_eval_kernel<10>, mtg::range_eval_kernel<11>, mtg::range_eval_kernel<12>};
-    const RangeEval fn = kRangeEval[N - 1];
-    MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
-    const int64_t total = B * int64_t(max_samples);
-    const int64_t blocks = std::min<int64_t>((total + threads - 1) / threads, int64_t(h->sm_count) * 32);
-    fn<<<(unsigned)blocks, threads, smem, s>>>(rp);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
+    const auto fn = kernel_by_n<1, MTG_MAX_N>([](auto k) { return mtg::range_eval_kernel<decltype(k)::N>; }, N);
+    MTG_TRY(launch_kernel(h, fn, capped_grid(h, B * int64_t(max_samples), threads, 32), threads, smem, s, rp));
   }
   return arena_release(h, ar, s);
 }
@@ -1498,9 +1485,7 @@ int mtg_evaluate_range_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D,
 }
 
 // ---- flat-state samplers ------------------------------------------------------------------------------------------
-static int64_t flat_state_blocks(mtg_handle* h, int64_t records) {
-  return std::min<int64_t>((records + mtg::kFlatStateThreads - 1) / mtg::kFlatStateThreads, int64_t(h->sm_count) * 16);
-}
+static int flat_attitude(int32_t D) { return D == 4 ? mtg::kAttYaw : D == 6 ? mtg::kAttRotationVector : mtg::kAttNone; }
 
 static bool valid_flat_range(int32_t N, int32_t K, int32_t D, int64_t B, double dt, int32_t max_samples, const double* seg_times,
                              const double* coeffs, const double* states, const int32_t* n_samples) {
@@ -1513,10 +1498,6 @@ static int launch_flat_range(mtg_handle* h, int32_t N, int32_t K, int32_t D, int
                              const double* coeffs, double min_time, double max_time, double dt, int32_t whole,
                              int32_t max_samples, double* states, int64_t* time_ns, int32_t* n_samples, cudaStream_t s,
                              int slot) {
-  const size_t ns = size_t(B) * size_t(std::max(max_samples, 1));
-  mtg_handle::Arena& ar = h->pack[slot];
-  const size_t o_idx = align_doubles(ns);  // t_local first (doubles), then seg_idx (int32)
-  MTG_TRY(arena_acquire(h, ar, (o_idx + align_doubles((ns + 1) / 2)) * 8, s));
   mtg::RangeParams rp = {};
   rp.N = N;
   rp.K = K;
@@ -1528,28 +1509,19 @@ static int launch_flat_range(mtg_handle* h, int32_t N, int32_t K, int32_t D, int
   rp.dt = dt;
   rp.times = seg_times;
   rp.coeffs = coeffs;
-  rp.t_local = ar.p;
-  rp.seg_idx = reinterpret_cast<int*>(ar.p + o_idx);
   rp.n_samples = n_samples;
   rp.sampling_times = nullptr;
   rp.out = states;
   rp.range_rule = whole ? mtg::kRangeWhole : mtg::kRangeChecked;
   rp.time_ns = reinterpret_cast<long long*>(time_ns);
-  {
-    const int threads = 128;
-    const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
-    mtg::range_walk_kernel<<<(unsigned)blocks, threads, 0, s>>>(rp);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
-  }
+  MTG_TRY(walk_range(h, rp, s, slot));
   if (max_samples > 0) {
-    typedef void (*Fn)(const mtg::RangeParams);
-    const Fn fn = flat_state_kernel<FlatRangeKernel, Fn>(N, D);
-    fn<<<(unsigned)flat_state_blocks(h, B * int64_t(max_samples)), mtg::kFlatStateThreads, 0, s>>>(rp);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
+    const auto fn = kernel_by_n<1, MTG_MAX_N, 1, mtg::kAttNone, mtg::kAttRotationVector>(
+        [](auto k) { return mtg::flat_state_range_kernel<decltype(k)::N, decltype(k)::A>; }, N, flat_attitude(D));
+    const int threads = mtg::kFlatStateThreads;
+    MTG_TRY(launch_kernel(h, fn, capped_grid(h, B * int64_t(max_samples), threads, 16), threads, 0, s, rp));
   }
-  return arena_release(h, ar, s);
+  return arena_release(h, h->pack[slot], s);
 }
 
 int mtg_sample_flat_states_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
@@ -1576,12 +1548,10 @@ static int launch_flat_at_time(mtg_handle* h, int32_t N, int32_t K, int32_t D, i
   prm.states = states;
   prm.time_ns = reinterpret_cast<long long*>(time_ns);
   prm.ok = ok;
-  typedef void (*Fn)(const mtg::FlatAtTimeParams);
-  const Fn fn = flat_state_kernel<FlatAtTimeKernel, Fn>(N, D);
-  fn<<<(unsigned)flat_state_blocks(h, B), mtg::kFlatStateThreads, 0, s>>>(prm);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
+  const auto fn = kernel_by_n<1, MTG_MAX_N, 1, mtg::kAttNone, mtg::kAttRotationVector>(
+      [](auto k) { return mtg::flat_state_at_time_kernel<decltype(k)::N, decltype(k)::A>; }, N, flat_attitude(D));
+  const int threads = mtg::kFlatStateThreads;
+  return launch_kernel(h, fn, capped_grid(h, B, threads, 16), threads, 0, s, prm);
 }
 
 static bool valid_flat_at_time(int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times, const double* coeffs,
@@ -1612,11 +1582,8 @@ static int launch_mellinger(mtg_handle* h, const mtg_problem* p, CachedTopology*
     const int rc =
         launch_cost_fused(h, p, topo, B * int64_t(K + 1), seg_times, d_fixed, ar.p, int(K + 1), 0.1, 0.1, s, status_x);
     if (rc == MTG_OK) {
-      const int threads = 128;
-      const int64_t gb = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
-      mtg::mellinger_gradient_kernel<<<(unsigned)gb, threads, 0, s>>>(B, p->K, ar.p, cost, grad, 0.1);
-      MTG_CUDA(h, cudaGetLastError());
-      h->launches++;
+      MTG_TRY(launch_kernel(h, mtg::mellinger_gradient_kernel, capped_grid(h, B, 128, 16), 128, 0, s, B, p->K, ar.p,
+                            cost, grad, 0.1));
       return arena_release(h, ar, s);
     }
     if (rc != MTG_ERR_ALLOC) return rc;
@@ -1645,19 +1612,12 @@ static int launch_mellinger(mtg_handle* h, const mtg_problem* p, CachedTopology*
     mp.dfix_x = f_x;
     mp.increment = 0.1;  // reference: increment_time (nonlinear_impl.h:310)
     mp.lower = 0.1;      // kOptimizationTimeLowerBound (polynomial_optimization_nonlinear.h:31)
-    const int threads = 128;
-    const int64_t blocks = std::min<int64_t>((nx + threads - 1) / threads, int64_t(h->sm_count) * 16);
-    mtg::mellinger_expand_kernel<<<(unsigned)blocks, threads, 0, s>>>(mp);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
+    MTG_TRY(launch_kernel(h, mtg::mellinger_expand_kernel, capped_grid(h, nx, 128, 16), 128, 0, s, mp));
     MTG_TRY(launch_solve(h, p, topo, nx, t_x, f_x, nullptr, c_x, nullptr,
                          status_x ? status_x + b0 * int64_t(K + 1) : nullptr, s, false, nullptr, slot));
     MTG_TRY(launch_cost(h, p, nx, t_x, c_x, j_x, s));
-    const int64_t gb = std::min<int64_t>((nb + threads - 1) / threads, int64_t(h->sm_count) * 16);
-    mtg::mellinger_gradient_kernel<<<(unsigned)gb, threads, 0, s>>>(nb, p->K, j_x, cost ? cost + b0 : nullptr,
-                                                                  grad + b0 * K, mp.increment);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
+    MTG_TRY(launch_kernel(h, mtg::mellinger_gradient_kernel, capped_grid(h, nb, 128, 16), 128, 0, s, nb, p->K, j_x,
+                          cost ? cost + b0 : nullptr, grad + b0 * K, mp.increment));
   }
   return arena_release(h, ar, s);
 }
@@ -1695,23 +1655,9 @@ static int launch_max_magnitude(mtg_handle* h, int32_t N, int32_t K, int32_t D, 
   ep.time = time;
   ep.segment = segment;
   ep.status = status;
-  const int tpb = std::max(1, mtg::kExtremaThreads / K);
-  const size_t smem = size_t(2) * tpb * K * n_derivs * sizeof(double);
-  if (smem > h->smem_optin) {
-    h->error = "mtg_max_magnitude_batch_f64: K * n_derivs too large";
-    return MTG_ERR_BAD_ARG;
-  }
-  typedef void (*ExtremaFn)(const mtg::ExtremaParams, const int);
-  static const ExtremaFn kExtrema[MTG_MAX_N / 2] = {mtg::max_magnitude_kernel<2>, mtg::max_magnitude_kernel<4>,
-                                                    mtg::max_magnitude_kernel<6>, mtg::max_magnitude_kernel<8>,
-                                                    mtg::max_magnitude_kernel<10>, mtg::max_magnitude_kernel<12>};
-  const ExtremaFn fn = kExtrema[N / 2 - 1];
-  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
-  const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
-  fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(ep, tpb);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
+  const auto fn = kernel_by_n<2, MTG_MAX_N, 2>([](auto k) { return mtg::max_magnitude_kernel<decltype(k)::N>; }, N);
+  return launch_segment_parallel(h, fn, ep, K, B, size_t(2) * K * n_derivs * sizeof(double),
+                                 "mtg_max_magnitude_batch_f64", "K * n_derivs", s);
 }
 
 int mtg_max_magnitude_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
@@ -1781,11 +1727,7 @@ static int launch_time_objective(mtg_handle* h, const mtg_problem* p, CachedTopo
   op.objective = objective;
   op.terms = terms;
   op.status = status;
-  const int threads = 128;
-  const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
-  mtg::time_objective_kernel<<<(unsigned)blocks, threads, 0, s>>>(op);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
+  MTG_TRY(launch_kernel(h, mtg::time_objective_kernel, capped_grid(h, B, 128, 16), 128, 0, s, op));
   return arena_release(h, ar, s);
 }
 
@@ -1828,23 +1770,10 @@ static int launch_scale_to_constraints(mtg_handle* h, int32_t N, int32_t K, int3
   sp.within = within_range;
   sp.maxima = maxima;
   sp.status = status;
-  const int tpb = std::max(1, mtg::kExtremaThreads / K);
-  const size_t smem = size_t(2) * tpb * K * sizeof(double) + size_t(tpb) * (sizeof(double) + sizeof(int));
-  if (smem > h->smem_optin) {
-    h->error = "mtg_scale_to_constraints_batch_f64: K too large";
-    return MTG_ERR_BAD_ARG;
-  }
-  typedef void (*ScaleFn)(const mtg::ScaleParams, const int);
-  static const ScaleFn kScale[MTG_MAX_N / 2 - 1] = {
-      mtg::scale_to_constraints_kernel<4>, mtg::scale_to_constraints_kernel<6>, mtg::scale_to_constraints_kernel<8>,
-      mtg::scale_to_constraints_kernel<10>, mtg::scale_to_constraints_kernel<12>};
-  const ScaleFn fn = kScale[N / 2 - 2];
-  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
-  const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
-  fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(sp, tpb);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
+  const auto fn =
+      kernel_by_n<4, MTG_MAX_N, 2>([](auto k) { return mtg::scale_to_constraints_kernel<decltype(k)::N>; }, N);
+  return launch_segment_parallel(h, fn, sp, K, B, size_t(2) * K * sizeof(double) + sizeof(double) + sizeof(int),
+                                 "mtg_scale_to_constraints_batch_f64", "K", s);
 }
 
 int mtg_scale_to_constraints_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
@@ -1879,22 +1808,16 @@ static int launch_scale_with_violation(mtg_handle* h, const mtg_problem* p, Cach
   // nonlinear_impl.h:366-406: the solve at the given times (trajectory_.scaleSegmentTimesToMeetConstraints acts on
   // the solved trajectory), the stretch in place on coeffs, then solveLinear() at the stretched times
   MTG_TRY(launch_solve(h, p, topo, B, seg_times, d_fixed, nullptr, coeffs, nullptr, st_solve, s, false, nullptr, slot));
-  const int threads = 128;
-  const int64_t blocks = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
-  if (pass) {  // rows with a non-zero pass[] are not stretched (the scaling passes failed solves through)
-    mtg::or_status_kernel<<<(unsigned)blocks, threads, 0, s>>>(B, pass, st_solve);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
-  }
+  const int64_t blocks = capped_grid(h, B, 128, 16);
+  if (pass)  // rows with a non-zero pass[] are not stretched (the scaling passes failed solves through)
+    MTG_TRY(launch_kernel(h, mtg::or_status_kernel, blocks, 128, 0, s, B, pass, st_solve));
   MTG_TRY(launch_scale_to_constraints(h, p->N, p->K, p->D, B, seg_times, coeffs, v_max, a_max, seg_times_out, coeffs,
                                       st_solve, within_range, maxima, st_scale, s));
   MTG_TRY(launch_solve(h, p, topo, B, seg_times_out, d_fixed, nullptr, coeffs, nullptr, st_resolve, s, false, nullptr,
                        slot));
   if (status) {
     MTG_CUDA(h, cudaMemcpyAsync(status, st_scale, sizeof(int32_t) * size_t(B), cudaMemcpyDeviceToDevice, s));
-    mtg::or_status_kernel<<<(unsigned)blocks, threads, 0, s>>>(B, st_resolve, status);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
+    MTG_TRY(launch_kernel(h, mtg::or_status_kernel, blocks, 128, 0, s, B, st_resolve, status));
   }
   return arena_release(h, ar, s);
 }
@@ -1951,11 +1874,8 @@ static int launch_line_search(mtg_handle* h, const mtg_problem* p, CachedTopolog
     cp.g = lp.g + r0 * K;
     cp.alpha = lp.alpha + r0;
     cp.dfix = lp.dfix + r0 * dnf;
-    const int threads = 128;
-    const int64_t blocks = std::min<int64_t>((nx + threads - 1) / threads, int64_t(h->sm_count) * 16);
-    mtg::line_search_expand_kernel<<<(unsigned)blocks, threads, 0, s>>>(cp, ar.p, ar.p + o_f);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
+    MTG_TRY(launch_kernel(h, mtg::line_search_expand_kernel, capped_grid(h, nx, 128, 16), 128, 0, s, cp, ar.p,
+                          ar.p + o_f));
     MTG_TRY(launch_solve(h, p, topo, nx, ar.p, ar.p + o_f, nullptr, ar.p + o_c, nullptr, st_c + r0 * kL, s, false,
                          nullptr, slot));
     MTG_TRY(launch_cost(h, p, nx, ar.p, ar.p + o_c, Jc + r0 * kL, s));
@@ -2038,30 +1958,22 @@ static int launch_optimize_mellinger(mtg_handle* h, const mtg_problem* p, Cached
   // the start lists the iterating rows into list 0
   set_lists(1);
   MTG_CUDA(h, cudaMemsetAsync(d_count, 0, sizeof(int32_t), s));
-  mtg::mel_init_kernel<<<(unsigned)((B + threads - 1) / threads), threads, 0, s>>>(lp, seg_times, d_fixed);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
+  MTG_TRY(launch_kernel(h, mtg::mel_init_kernel, (B + threads - 1) / threads, threads, 0, s, lp, seg_times, d_fixed));
   int rows = 0;
   MTG_TRY(read_count(h, d_count, s, &rows));
   for (int k = 0; rows > 0; ++k) {
     set_lists(cur);
     lp.rows = rows;
     lp.k = k;
-    const unsigned blocks = (unsigned)((rows + threads - 1) / threads);
+    const int blocks = (rows + threads - 1) / threads;
     MTG_CUDA(h, cudaMemsetAsync(ip(o_stg), 0, sizeof(int32_t) * size_t(rows) * (K + 1), s));
     MTG_CUDA(h, cudaMemsetAsync(ip(o_stc), 0, sizeof(int32_t) * size_t(rows) * kL, s));
     MTG_TRY(launch_mellinger(h, p, topo, rows, lp.x, lp.dfix, base + o_J, base + o_g, s, slot, ip(o_stg)));
-    if (k == 0) {
-      mtg::mel_alpha0_kernel<<<blocks, threads, 0, s>>>(lp, base + o_a[cur]);
-      MTG_CUDA(h, cudaGetLastError());
-      h->launches++;
-    }
+    if (k == 0) MTG_TRY(launch_kernel(h, mtg::mel_alpha0_kernel, blocks, threads, 0, s, lp, base + o_a[cur]));
     // K = 1: every gradient is zero (getCostAndGradientMellinger), so every row stops with SUCCESS: no candidates
     if (p->K > 1) MTG_TRY(launch_line_search(h, p, topo, lp, base + o_Jc, ip(o_stc), s, slot));
     MTG_CUDA(h, cudaMemsetAsync(d_count, 0, sizeof(int32_t), s));
-    mtg::mel_update_kernel<<<blocks, threads, 0, s>>>(lp);
-    MTG_CUDA(h, cudaGetLastError());
-    h->launches++;
+    MTG_TRY(launch_kernel(h, mtg::mel_update_kernel, blocks, threads, 0, s, lp));
     MTG_TRY(read_count(h, d_count, s, &rows));
     cur ^= 1;
   }
@@ -2070,11 +1982,8 @@ static int launch_optimize_mellinger(mtg_handle* h, const mtg_problem* p, Cached
   MTG_TRY(launch_scale_with_violation(h, p, topo, B, seg_times_out, d_fixed, v_max, a_max, coeffs, seg_times_out,
                                       within_range, maxima, ip(o_sst), s, slot, ip(o_pass)));
   if (cost) MTG_TRY(launch_cost(h, p, B, seg_times_out, coeffs, cost, s));
-  const int64_t fb = std::min<int64_t>((B + threads - 1) / threads, int64_t(h->sm_count) * 16);
-  mtg::mel_finish_kernel<<<(unsigned)fb, threads, 0, s>>>(B, ip(o_it), ip(o_res), ip(o_ost), ip(o_sst), iterations,
-                                                          result, status);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
+  MTG_TRY(launch_kernel(h, mtg::mel_finish_kernel, capped_grid(h, B, threads, 16), threads, 0, s, B, ip(o_it),
+                        ip(o_res), ip(o_ost), ip(o_sst), iterations, result, status));
   return arena_release(h, ar, s);
 }
 
@@ -2123,10 +2032,11 @@ static bool valid_sampling(int32_t N, int32_t K, int32_t D, int64_t B, const dou
 enum class FeasKind { Analytic, Recursive, Sampling };
 
 // Analytic: input_feasibility_kernel; Recursive: input_feasibility_recursive_kernel; Sampling:
-// input_feasibility_sampling_kernel (a warp per segment) at sampling_interval
-static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
-                                    const double* coeffs, const mtg_input_constraints* ic, int32_t* result,
-                                    int32_t* segment, int32_t* status, cudaStream_t s,
+// input_feasibility_sampling_kernel (a warp per segment) at sampling_interval.  `entry` names the public entry point
+// in the error of a K too large.
+static int launch_input_feasibility(mtg_handle* h, const char* entry, int32_t N, int32_t K, int32_t D, int64_t B,
+                                    const double* seg_times, const double* coeffs, const mtg_input_constraints* ic,
+                                    int32_t* result, int32_t* segment, int32_t* status, cudaStream_t s,
                                     FeasKind kind = FeasKind::Analytic, double sampling_interval = 0.0) {
   mtg::FeasParams fp;
   fp.K = K;
@@ -2147,43 +2057,23 @@ static int launch_input_feasibility(mtg_handle* h, int32_t N, int32_t K, int32_t
   fp.result = result;
   fp.segment = segment;
   fp.status = status;
-  const int tpb = std::max(1, mtg::kExtremaThreads / K);
-  const size_t smem = size_t(tpb) * K * sizeof(int);
-  if (smem > h->smem_optin) {
-    h->error = kind == FeasKind::Recursive  ? "mtg_input_feasibility_recursive_batch_f64: K too large"
-               : kind == FeasKind::Sampling ? "mtg_input_feasibility_sampling_batch_f64: K too large"
-                                            : "mtg_input_feasibility_batch_f64: K too large";
-    return MTG_ERR_BAD_ARG;
-  }
-  typedef void (*FeasFn)(const mtg::FeasParams, const int);
-  static const FeasFn kFeas[MTG_MAX_N / 2 - 1] = {
-      mtg::input_feasibility_kernel<4>, mtg::input_feasibility_kernel<6>, mtg::input_feasibility_kernel<8>,
-      mtg::input_feasibility_kernel<10>, mtg::input_feasibility_kernel<12>};
-  static const FeasFn kFeasRec[MTG_MAX_N / 2 - 1] = {
-      mtg::input_feasibility_recursive_kernel<4>, mtg::input_feasibility_recursive_kernel<6>,
-      mtg::input_feasibility_recursive_kernel<8>, mtg::input_feasibility_recursive_kernel<10>,
-      mtg::input_feasibility_recursive_kernel<12>};
-  static const FeasFn kFeasSampling[MTG_MAX_N / 2 - 1] = {
-      mtg::input_feasibility_sampling_kernel<4>, mtg::input_feasibility_sampling_kernel<6>,
-      mtg::input_feasibility_sampling_kernel<8>, mtg::input_feasibility_sampling_kernel<10>,
-      mtg::input_feasibility_sampling_kernel<12>};
-  const FeasFn fn = (kind == FeasKind::Recursive  ? kFeasRec
-                     : kind == FeasKind::Sampling ? kFeasSampling
-                                                  : kFeas)[N / 2 - 2];
-  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
-  const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
-  fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(fp, tpb);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
+  const auto fn = kernel_by_n<4, MTG_MAX_N, 2, 0, 2>(
+      [](auto k) {
+        constexpr int n = decltype(k)::N;
+        if constexpr (decltype(k)::A == int(FeasKind::Recursive)) return mtg::input_feasibility_recursive_kernel<n>;
+        else if constexpr (decltype(k)::A == int(FeasKind::Sampling)) return mtg::input_feasibility_sampling_kernel<n>;
+        else return mtg::input_feasibility_kernel<n>;
+      },
+      N, int(kind));
+  return launch_segment_parallel(h, fn, fp, K, B, size_t(K) * sizeof(int), entry, "K", s);
 }
 
 int mtg_input_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B, const double* seg_times,
                                     const double* coeffs, const mtg_input_constraints* constraints, int32_t* result,
                                     int32_t* segment, int32_t* status, void* stream) {
   return run_entry(h, valid_feasibility(N, K, D, B, seg_times, coeffs, constraints, result), B, [&] {
-    return launch_input_feasibility(h, N, K, D, B, seg_times, coeffs, constraints, result, segment, status,
-                                    (cudaStream_t)stream);
+    return launch_input_feasibility(h, "mtg_input_feasibility_batch_f64", N, K, D, B, seg_times, coeffs, constraints,
+                                    result, segment, status, (cudaStream_t)stream);
   });
 }
 
@@ -2193,8 +2083,8 @@ int mtg_input_feasibility_recursive_batch_f64(mtg_handle* h, int32_t N, int32_t 
                                               const mtg_input_constraints* constraints, int32_t* result,
                                               int32_t* segment, int32_t* status, void* stream) {
   return run_entry(h, valid_feasibility(N, K, D, B, seg_times, coeffs, constraints, result), B, [&] {
-    return launch_input_feasibility(h, N, K, D, B, seg_times, coeffs, constraints, result, segment, status,
-                                    (cudaStream_t)stream, FeasKind::Recursive);
+    return launch_input_feasibility(h, "mtg_input_feasibility_recursive_batch_f64", N, K, D, B, seg_times, coeffs,
+                                    constraints, result, segment, status, (cudaStream_t)stream, FeasKind::Recursive);
   });
 }
 
@@ -2204,8 +2094,9 @@ int mtg_input_feasibility_sampling_batch_f64(mtg_handle* h, int32_t N, int32_t K
                                              const mtg_input_constraints* constraints, double sampling_interval,
                                              int32_t* result, int32_t* segment, int32_t* status, void* stream) {
   return run_entry(h, valid_sampling(N, K, D, B, seg_times, coeffs, constraints, sampling_interval, result), B, [&] {
-    return launch_input_feasibility(h, N, K, D, B, seg_times, coeffs, constraints, result, segment, status,
-                                    (cudaStream_t)stream, FeasKind::Sampling, sampling_interval);
+    return launch_input_feasibility(h, "mtg_input_feasibility_sampling_batch_f64", N, K, D, B, seg_times, coeffs,
+                                    constraints, result, segment, status, (cudaStream_t)stream, FeasKind::Sampling,
+                                    sampling_interval);
   });
 }
 
@@ -2247,23 +2138,9 @@ static int launch_half_plane(mtg_handle* h, int32_t N, int32_t K, int32_t D, int
       hp.planes[p][d] = p < n_planes ? planes[p].point[d] : 0.0;
       hp.planes[p][3 + d] = p < n_planes ? planes[p].normal[d] : 0.0;
     }
-  const int tpb = std::max(1, mtg::kExtremaThreads / K);
-  const size_t smem = size_t(tpb) * K * sizeof(int);
-  if (smem > h->smem_optin) {
-    h->error = "mtg_half_plane_feasibility_batch_f64: K too large";
-    return MTG_ERR_BAD_ARG;
-  }
-  typedef void (*HalfPlaneFn)(const mtg::HalfPlaneParams, const int);
-  static const HalfPlaneFn kHalfPlane[MTG_MAX_N / 2] = {mtg::half_plane_kernel<2>,  mtg::half_plane_kernel<4>,
-                                                        mtg::half_plane_kernel<6>,  mtg::half_plane_kernel<8>,
-                                                        mtg::half_plane_kernel<10>, mtg::half_plane_kernel<12>};
-  const HalfPlaneFn fn = kHalfPlane[N / 2 - 1];
-  MTG_TRY(ensure_dyn_smem(h, (const void*)fn, smem));
-  const int64_t blocks = std::min<int64_t>((B + tpb - 1) / tpb, int64_t(h->sm_count) * 16);
-  fn<<<(unsigned)blocks, mtg::kExtremaThreads, smem, s>>>(hp, tpb);
-  MTG_CUDA(h, cudaGetLastError());
-  h->launches++;
-  return MTG_OK;
+  const auto fn = kernel_by_n<2, MTG_MAX_N, 2>([](auto k) { return mtg::half_plane_kernel<decltype(k)::N>; }, N);
+  return launch_segment_parallel(h, fn, hp, K, B, size_t(K) * sizeof(int), "mtg_half_plane_feasibility_batch_f64", "K",
+                                 s);
 }
 
 int mtg_half_plane_feasibility_batch_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
@@ -2506,7 +2383,8 @@ int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, in
                             {nullptr, segment, 4},
                             {nullptr, status, 4}};
     return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
-      return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s);
+      return launch_input_feasibility(h, "mtg_input_feasibility_batch_f64", N, K, D, nb, d[0], d[1], constraints, d[2],
+                                      d[3], d[4], s);
     });
   });
 }
@@ -2522,8 +2400,8 @@ int mtg_input_feasibility_recursive_batch_host_f64(mtg_handle* h, int32_t N, int
                             {nullptr, segment, 4},
                             {nullptr, status, 4}};
     return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
-      return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s,
-                                      FeasKind::Recursive);
+      return launch_input_feasibility(h, "mtg_input_feasibility_recursive_batch_f64", N, K, D, nb, d[0], d[1],
+                                      constraints, d[2], d[3], d[4], s, FeasKind::Recursive);
     });
   });
 }
@@ -2539,8 +2417,8 @@ int mtg_input_feasibility_sampling_batch_host_f64(mtg_handle* h, int32_t N, int3
                             {nullptr, segment, 4},
                             {nullptr, status, 4}};
     return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int) {
-      return launch_input_feasibility(h, N, K, D, nb, d[0], d[1], constraints, d[2], d[3], d[4], s,
-                                      FeasKind::Sampling, sampling_interval);
+      return launch_input_feasibility(h, "mtg_input_feasibility_sampling_batch_f64", N, K, D, nb, d[0], d[1],
+                                      constraints, d[2], d[3], d[4], s, FeasKind::Sampling, sampling_interval);
     });
   });
 }
