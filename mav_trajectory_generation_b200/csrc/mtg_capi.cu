@@ -225,7 +225,7 @@ struct WaypointEntry {
   size_t (*k3_smem[2])(int C);    // with C resident blocks per lane
   int k3_park;                    // doubles per thread of one vertex block that K3 parks in global memory
   ChunkedKernel k3_pair;          // K3 in warp pairs (one tile's inward sweep beside the last tile's outward one)
-  size_t (*k3_pair_smem)(int C);
+  size_t (*k3_pair_smem)(int C, int K, int nf);  // with C resident blocks per lane and its tile input buffer
   // null where the shape has no such instantiation
   SweepKernel v1;                 // one thread per trajectory (cross-checks and profiles)
   size_t (*v1_smem)(int K);
@@ -595,7 +595,7 @@ struct WaypointPlan {
 // K3: the chunked twisted kernel -- any K, fixed on-chip footprint; the vertex blocks beyond the C resident ones
 // are parked in global memory.
 // With `pairs` (the default route), the paired form takes the solve where it fits: see below.
-int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, int64_t B, bool pairs,
+int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, int64_t B, int nf, bool pairs,
                  WaypointPlan* pl) {
   const int nmax = (p->K + 1) / 2 - 1;
   // Auto: one-warp CTAs (shared memory then comes in 31-52 KB steps instead of 124-206 KB ones), no L2 hints, at
@@ -646,13 +646,16 @@ int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, in
   // The paired form (twisted_chunked_pair_kernel): 64-thread CTAs that run one tile's inward sweep beside the last
   // tile's outward sweep on one tile's resident blocks.  Auto: while every block of a lane fits in shared memory
   // (nmax <= kPairMaxBlocks, K <= 16), C = nmax -- nothing parked -- at kAutoPairs pairs per SM.  Measured with
-  // tools/k3_sweep.py on an H100 80GB HBM3 at N = 10, D = 3, 700 W power limit (ms per solve, spread of the round
-  // medians <= 0.03 ms), against the one-warp auto plan above (K = 16: 2.59, K = 50: 3.09, K = 100: 3.08 in the
-  // same runs), at 2 / 3 / 4 pairs per SM:
-  //   K = 16:  C = 5: 2.43 / 2.74 / 3.06   C = 6: 2.31 / 2.44   C = 7: 2.20 / 2.36
-  //   K = 50:  C = 4: 3.30 / 3.16 / 3.58   C = 5: 3.20 / 3.12 / 3.52
-  //   K = 100: C = 4: 3.28 / 3.13 / 3.55   C = 5: 3.23 / 3.10 / 3.51
-  // More pairs lose the L1 they take, and with blocks parked the pairs do not beat the one-warp plan.  Forced,
+  // tools/k3_sweep.py on an H100 80GB HBM3 at N = 10, D = 3, 700 W power limit, SM clock 1980 MHz (ms per solve,
+  // spread of the round medians <= 0.02 ms but one 0.34), with the inputs in tile buffers filled by bulk copies, at
+  // 2 / 3 / 4 pairs per SM where they fit:
+  //   K = 8  (1 048 576): C = 3: 1.128 / 1.111 / 1.148
+  //   K = 12 (1 048 576): C = 3: 1.808 / 1.975 / 2.134   C = 5: 1.593 / 1.662
+  //   K = 16 (1 048 576): C = 3: 2.720 / 3.134 / 3.397   C = 5: 2.340 / 2.567   C = 7: 2.054 / 2.183
+  // A third pair loses even though the inputs no longer pass through L1 (only at K = 8 is it 1.5 % ahead, within
+  // twice the spread).  Before the tile buffers (per-lane cp.async gathers through L1), K = 16 ran C = 7 at 2.20 / 2.36
+  // and, with blocks parked, K = 50 and K = 100 at 3.1-3.3 ms against 3.09 and 3.08 for the one-warp plan, which
+  // keeps those K.  Forced,
   // CHUNK_BLOCKS sets C and CTAS_PER_SM caps the warps per SM (pairs = CTAS_PER_SM / 2) at any K.  The pairs need an
   // inward sweep (K >= 3); CHUNK_WARPS or L2_HINTS select the one-warp form.
   constexpr int kPairMaxBlocks = 7;
@@ -660,7 +663,7 @@ int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, in
   const bool forced = h->chunk_blocks > 0 || h->ctas_per_sm > 0;
   if (pairs && h->chunk_warps == 0 && h->l2_hints == 0 && nmax >= 1 && (forced || nmax <= kPairMaxBlocks)) {
     const int C = h->chunk_blocks > 0 || nmax > kPairMaxBlocks ? best_C : nmax;
-    const size_t smem = e.k3_pair_smem(C);
+    const size_t smem = e.k3_pair_smem(C, p->K, nf);
     const int cap = h->ctas_per_sm > 0 ? h->ctas_per_sm / 2 : kAutoPairs;
     int ctas = 0, carveout = 0;
     if (cap >= 1) MTG_TRY(chunked_residency(h, (const void*)e.k3_pair, smem, cap, 64, &ctas, &carveout));
@@ -714,7 +717,7 @@ int plan_waypoint(mtg_handle* h, const mtg_problem* p, const Layout& L, const Wa
   const int V = h->waypoint_variant, K = p->K;
   const int64_t B = prm.B;
   if (!a16(prm.coeffs)) return MTG_ERR_ALLOC;
-  if (V == 5 && !fused) return plan_chunked(h, p, e, B, false, pl);
+  if (V == 5 && !fused) return plan_chunked(h, p, e, B, prm.n_fixed, false, pl);
   const bool inputs_a16 = fused ? a16(prm.positions) : a16(prm.times) && a16(prm.dfix);
   if ((V == 6 || (V == 0 && h->tma_inputs != 0)) && B % 16 == 0 && inputs_a16 && e.v5) {
     const void* fn = (const void*)(fused ? e.v5_fused : e.v5);
@@ -773,7 +776,7 @@ int plan_waypoint(mtg_handle* h, const mtg_problem* p, const Layout& L, const Wa
     const size_t smem = e.v3_smem(K);
     bool fits = false;
     MTG_TRY(v3_fits(h, (const void*)e.v3, smem, &fits));
-    if (!fits) return fused ? MTG_ERR_ALLOC : plan_chunked(h, p, e, B, V == 0, pl);
+    if (!fits) return fused ? MTG_ERR_ALLOC : plan_chunked(h, p, e, B, prm.n_fixed, V == 0, pl);
     pl->family = Family::Tmem;
     pl->fn = (const void*)(fused ? e.v3_fused : e.v3);
     pl->blocks = (B + 63) / 64;

@@ -368,37 +368,59 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
 // tile's parity: (v-1) % C on even tiles, (n-v) % C on odd ones.  Parked blocks stay the outer ones of each tile
 // (the refill distance stays C-1 steps) and the parking area has one half per parity.
 //
-// Handshakes (mbarriers, one arrival per lane):
-//   freed[s]  outward -> inward: the slot s has been read for the last time in this tile
-//   ready     inward -> outward: the middle vertex is done and the handoff (starting ed of each lane) written
+// Inputs: the inward warp reads everything from a tile input buffer that holds the tile's seg_times[16][K] and
+// d_fixed[16][D][n_fixed] exactly as they lie in global memory.  A whole tile with 16-byte aligned inputs arrives by
+// two cp.async.bulk copies (which bypass L1, so the pairs do not compete with their own input lines for it); the
+// ragged last tile, or unaligned inputs, fill the same layout with per-lane 8-byte cp.async copies, rows past B
+// repeating row B-1.  The buffer is refilled with the next tile once the inward sweep has read its last input, so
+// the copy lands while the middle vertex is solved.  Before that refill the inward warp copies what the outward
+// warp's final segment reads (x0, u0, T0 of own vertex 0) into END.
+//
+// Handshakes (mbarriers):
+//   freed[s]  outward -> inward, one arrival per lane: the slot s has been read for the last time in this tile; the
+//             slot of vertex 1, popped last, is released only after the final segment has read END, so that END is
+//             free when the inward warp fills it after step n (which waits for that slot)
+//   ready     inward -> outward, one arrival per lane: the middle vertex is done and the handoff (starting ed of each
+//             lane) and END written
+//   full      the tile buffer holds the next tile: transaction count of the bulk copies (one arrival), or the
+//             per-lane copies tracked by cp.async.mbarrier.arrive (one arrival once every lane has issued them)
 // Neither side can run two phases ahead of the other: tile j's inward step n waits for tile j-1's last pop, which
 // follows that tile's wait on `ready` and the landing of all its refills; this needs n >= 1 (K >= 3).
 // tests/test_k3_pair_schedule.py walks this schedule on the host.
+//
+// RD does not enter the paired form (it has no input ring): it is the ring depth of the one-warp instantiations
+// built beside it, kept in the name so that each registry row has one paired kernel of a fixed name.
 template <int N, int D, int RD>
 struct ChunkedPairLayout {
   static constexpr int h = N / 2;
   static constexpr int m = h - 1;
   static constexpr int kSlots = sweep_state_slots<N, D, true>();
   static constexpr int kPark = kSlots + 1;
-  static constexpr int kPro = 2 * D + m * D + 1;     // x0, x1, u0[m], T0
-  static constexpr int kRing = RD * (1 + D);         // inward warp's input ring
   static constexpr int kEnd = D + m * D + 1;         // outward warp: x0, u0[m], T0 of the final segment
   static constexpr int kHand = h * D;                // handoff: the starting ed of the outward sweep
-  static constexpr int kMaxChunk = 31;               // mbarriers: freed[C], ready
-  static constexpr size_t kBarBytes = 8 * (kMaxChunk + 1);
+  static constexpr int kMaxChunk = 30;               // mbarriers: freed[C], ready, full
+  static constexpr size_t kBarBytes = 8 * (kMaxChunk + 2);
   static constexpr size_t stage_bytes = tmem_stage_bytes<N, D, 32>();  // the outward warp's staging tile
-  static constexpr int pro = kRing;
-  static constexpr int end = pro + kPro;
+  static constexpr size_t tile_offset = stage_bytes + kBarBytes;      // 16-byte aligned: the bulk copies land here
+  static_assert(tile_offset % 16 == 0, "tile input buffer alignment");
+  // doubles of the tile input buffer: seg_times[16][K], then d_fixed[16][D][nf] (both multiples of 16 bytes)
+  __host__ __device__ static constexpr size_t tile_doubles(int K, int nf) { return size_t(16) * K + size_t(16) * D * nf; }
+  static constexpr int end = 0;
   static constexpr int hand = end + kEnd;
   static constexpr int times = hand + kHand;         // then C slot times, then C blocks
   __host__ __device__ static constexpr size_t region(int C) { return size_t(times) + C; }
-  __host__ __device__ static constexpr size_t bytes(int C) {
-    return stage_bytes + kBarBytes + tmem_slot_bytes(region(C) + size_t(C) * kSlots, 32);
+  __host__ __device__ static constexpr size_t bytes(int C, int K, int nf) {
+    return tile_offset + tile_doubles(K, nf) * 8 + tmem_slot_bytes(region(C) + size_t(C) * kSlots, 32);
   }
 };
 
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// the mbarrier's current phase also waits for every cp.async this thread has issued so far (its pending count is
+// raised by one now and lowered when they have landed)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
+  asm volatile("cp.async.mbarrier.arrive.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
 // bulk::mbar_wait with the loop in C++, so that one kernel can wait at several places
 __device__ __forceinline__ void mbar_wait_parity(uint32_t bar, uint32_t parity) {
@@ -423,8 +445,6 @@ __global__ void __launch_bounds__(64, 4)
   using Lay = ChunkedPairLayout<N, D, RD>;
   constexpr int kSlots = Lay::kSlots;
   constexpr int kPark = Lay::kPark;
-  constexpr int kPro = Lay::kPro;
-  static_assert(RD >= 2, "ring depth");
   using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
   using S = sweep::Sweep<N, D, G>;
@@ -442,12 +462,14 @@ __global__ void __launch_bounds__(64, 4)
   const int npark = n - C;
 
   double2* stage = reinterpret_cast<double2*>(smem_raw);
-  const uint32_t bar0 = smem_u32(smem_raw + Lay::stage_bytes);  // freed[s] at bar0 + 8 s, ready at bar0 + 8 C
+  // freed[s] at bar0 + 8 s, ready at bar0 + 8 C, full at bar0 + 8 (C + 1)
+  const uint32_t bar0 = smem_u32(smem_raw + Lay::stage_bytes);
   const uint32_t ready = bar0 + 8u * uint32_t(C);
-  double* base = reinterpret_cast<double*>(smem_raw + Lay::stage_bytes + Lay::kBarBytes) + lane;
+  const uint32_t full = ready + 8u;
+  const int tile_t = 16 * K, tile_f = 16 * D * nf;
+  double* tile = reinterpret_cast<double*>(smem_raw + Lay::tile_offset);
+  double* base = tile + tile_t + tile_f + lane;
   auto SL = [&](int slot) -> double* { return base + size_t(slot) * 32; };
-  auto PF = [&](int buf, int slot) -> double* { return SL(buf * (1 + D) + slot); };
-  auto PRO = [&](int slot) -> double* { return SL(Lay::pro + slot); };
   auto END = [&](int slot) -> double* { return SL(Lay::end + slot); };
   auto HAND = [&](int slot) -> double* { return SL(Lay::hand + slot); };
   auto HT = [&](int b) -> double* { return SL(Lay::times + b); };
@@ -457,6 +479,7 @@ __global__ void __launch_bounds__(64, 4)
 
   if (threadIdx.x == 0) {
     for (int s = 0; s <= C; ++s) bulk::mbar_init(bar0 + 8u * uint32_t(s), 32);
+    bulk::mbar_init(full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -470,88 +493,84 @@ __global__ void __launch_bounds__(64, 4)
   auto PK = [&](long long j, int b, int slot) -> double* {
     return cl.ckpt + ((long long)b * kPark + slot) * gthreads + ((long long)blockIdx.x * 64 + (j & 1) * 32 + lane);
   };
-
-  struct Ptrs {
-    const double* tt;
-    const double* fx;
+  // this lane's trajectory in warp tile w (past B: row B-1, whose results are not stored)
+  struct Row {
     long long traj;
     bool valid;
   };
-  auto tile_ptrs = [&](long long w) -> Ptrs {
-    Ptrs p;
-    p.traj = w * 16 + (lane >> 1);
-    p.valid = p.traj < prm.B;
-    if (!p.valid) p.traj = prm.B - 1;
-    p.tt = prm.times + p.traj * K;
-    p.fx = prm.dfix + p.traj * (long long)D * nf;
-    return p;
+  auto row_of = [&](long long w) -> Row {
+    Row r;
+    r.traj = w * 16 + (lane >> 1);
+    r.valid = r.traj < prm.B;
+    if (!r.valid) r.traj = prm.B - 1;
+    return r;
   };
-  auto xaddr = [&](const Ptrs& p, int v, int d) -> const double* { return p.fx + d * nf + fr.pidx(v); };
   const int np = (K - 1) * m;
 
   if (inward) {
     // ================================================================ warp 0: prologue, inward sweep, middle
-    auto pro_issue = [&](const Ptrs& p) {
-#pragma unroll
-      for (int d = 0; d < D; ++d) {
-        cp_async8_stream(PRO(d), xaddr(p, 0, d), cl.evict_first);
-        cp_async8_stream(PRO(D + d), xaddr(p, 1, d), cl.evict_first);
-#pragma unroll
-        for (int b = 0; b < m; ++b) cp_async8_stream(PRO(2 * D + b * D + d), p.fx + d * nf + e0 + b, cl.evict_first);
+    const bool inputs_a16 = ((reinterpret_cast<uintptr_t>(prm.times) | reinterpret_cast<uintptr_t>(prm.dfix)) & 15u) == 0;
+    // warp tile w -> the tile buffer, completing the current phase of `full`
+    auto fill = [&](long long w) {
+      const double* gt = prm.times + w * tile_t;
+      const double* gf = prm.dfix + w * (long long)tile_f;
+      // the reads of the last tile (generic proxy) before the writes of the bulk copies (async proxy)
+      fence_proxy_async();
+      __syncwarp();
+      if (inputs_a16 && (w + 1) * 16 <= prm.B) {  // warp-uniform
+        if (lane == 0) {
+          bulk::mbar_expect_tx(full, uint32_t(tile_t + tile_f) * 8u);
+          bulk::copy_g2s(smem_u32(tile), gt, uint32_t(tile_t) * 8u, full);
+          bulk::copy_g2s(smem_u32(tile + tile_t), gf, uint32_t(tile_f) * 8u, full);
+        }
+      } else {
+        // element i of the buffer is element i of the tile's inputs; in rows past B, the same column of row B-1
+        const int rows = int(prm.B - w * 16 < 16 ? prm.B - w * 16 : 16);
+        const int last_t = rows * K - K, last_f = (rows - 1) * D * nf;
+        for (int i = lane; i < tile_t; i += 32) cp_async8(tile + i, gt + (i < rows * K ? i : last_t + i % K));
+        for (int i = lane; i < tile_f; i += 32)
+          cp_async8(tile + tile_t + i, gf + (i < rows * D * nf ? i : last_f + i % (D * nf)));
+        cp_async_mbar_arrive(full);
+        __syncwarp();  // every lane's pending count is raised before the phase can complete
+        if (lane == 0) mbar_arrive(full);
       }
-      cp_async8_stream(PRO(kPro - 1), p.tt + fr.seg(0), cl.evict_first);
     };
-    auto ring_issue = [&](const Ptrs& p, int v) {
-      const int j = v < K ? v : K - 1;
-      const int vn = v + 1 <= K ? v + 1 : K;
-      const int buf = v % RD;
-      cp_async8_stream(PF(buf, 0), p.tt + fr.seg(j), cl.evict_first);
-#pragma unroll
-      for (int d = 0; d < D; ++d) cp_async8_stream(PF(buf, 1 + d), xaddr(p, vn, d), cl.evict_first);
-    };
+    const double* __restrict__ tT = tile + (lane >> 1) * K;
+    const double* __restrict__ tF = tile + tile_t + (lane >> 1) * D * nf;
+    auto in_x = [&](int v, int d) -> double { return tF[d * nf + fr.pidx(v)]; };  // position of own vertex v
+    auto in_u0 = [&](int b, int d) -> double { return tF[d * nf + e0 + b]; };     // fixed end derivative b+1, raw
 
     long long wt = blockIdx.x;
-    if (wt < n_wtiles) {
-      pro_issue(tile_ptrs(wt));
-      cp_async_commit();
-    }
+    if (wt < n_wtiles) fill(wt);
     for (long long j = 0; wt < n_wtiles; wt += wt_stride, ++j) {
-      const Ptrs P = tile_ptrs(wt);
-#pragma unroll
-      for (int q = 1; q < RD; ++q) {
-        if (q <= nh) ring_issue(P, q);
-        cp_async_commit();
-      }
-      cp_async_wait_group<RD - 1>();
+      const Row P = row_of(wt);
+      mbar_wait_parity(full, uint32_t(j & 1));
 
       int stat = 0;
       double Wp[m][m], yp[m][D], Cee[m][m], cps[m], cpe[m], xm[D], xc[D];
       {
 #pragma unroll
         for (int d = 0; d < D; ++d) {
-          xm[d] = *PRO(d);
-          xc[d] = *PRO(D + d);
+          xm[d] = in_x(0, d);
+          xc[d] = in_x(1, d);
         }
-        const double T0 = *PRO(kPro - 1);
+        const double T0 = tT[fr.seg(0)];
         if (bad_segment_time(T0)) stat |= kStatusBadTime;
         const double iT0 = fast_rcp(T0);
         double pw[N - 1];
         segment_powers<N, R>(T0, iT0, pw);
         S::end_blocks(pw, Cee, cps, cpe);
-        S::carry_fold(pw, [&](int b, int d) { return fr.sgn(b) * *PRO(2 * D + b * D + d); }, Wp, yp);
+        S::carry_fold(pw, [&](int b, int d) { return fr.sgn(b) * in_u0(b, d); }, Wp, yp);
       }
 
       for (int v = 1; v <= n; ++v) {
         double sv[kSlots];
         double T;
         if (v <= nh) {
-          cp_async_wait_group<RD - 2>();
           double xn[D];
 #pragma unroll
-          for (int d = 0; d < D; ++d) xn[d] = *PF(v % RD, 1 + d);
-          T = *PF(v % RD, 0);
-          if (v + RD - 1 <= nh) ring_issue(P, v + RD - 1);
-          cp_async_commit();
+          for (int d = 0; d < D; ++d) xn[d] = in_x(v + 1, d);
+          T = tT[fr.seg(v)];
           if (bad_segment_time(T)) stat |= kStatusBadTime;
           const double iT = fast_rcp(T);
           double pw[N - 1];
@@ -581,11 +600,17 @@ __global__ void __launch_bounds__(64, 4)
           for (int i = 0; i < kSlots; ++i) *SP(b, i) = sv[i];
         }
       }
-      // the prologue region is this warp's own: the next tile's inputs land during the middle vertex
-      if (wt + wt_stride < n_wtiles) {
-        pro_issue(tile_ptrs(wt + wt_stride));
-        cp_async_commit();
+      // the last tile's final segment has read END (step n waited for the slot released after it): the final
+      // segment's inputs of this tile go there, then the buffer takes the next tile, which lands during the middle
+      // vertex
+#pragma unroll
+      for (int d = 0; d < D; ++d) {
+        *END(d) = in_x(0, d);
+#pragma unroll
+        for (int b = 0; b < m; ++b) *END(D + b * D + d) = in_u0(b, d);
       }
+      *END(Lay::kEnd - 1) = tT[fr.seg(0)];
+      if (wt + wt_stride < n_wtiles) fill(wt + wt_stride);
 
       double um[m][D];
       S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
@@ -616,18 +641,9 @@ __global__ void __launch_bounds__(64, 4)
 
   long long j = 0;
   for (long long wt = blockIdx.x; wt < n_wtiles; wt += wt_stride, ++j) {
-    const Ptrs P = tile_ptrs(wt);
+    const Row P = row_of(wt);
     const long long traj0 = wt * 16;
     const bool valid = P.valid;
-    // what the final segment reads besides ed, many steps ahead of its use
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-      cp_async8_stream(END(d), xaddr(P, 0, d), cl.evict_first);
-#pragma unroll
-      for (int b = 0; b < m; ++b) cp_async8_stream(END(D + b * D + d), P.fx + d * nf + e0 + b, cl.evict_first);
-    }
-    cp_async8_stream(END(Lay::kEnd - 1), P.tt + fr.seg(0), cl.evict_first);
-    cp_async_commit();
 
     double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + P.traj * (long long)D * np : nullptr;
     auto store_free = [&](int v_own, const double (&u)[h][D]) {
@@ -662,8 +678,8 @@ __global__ void __launch_bounds__(64, 4)
 #pragma unroll
         for (int i = 0; i < kSlots; ++i) cp_async8(SP(b, i), PK(j, v - C - 1, i));
         cp_async8(HT(b), PK(j, v - C - 1, kSlots));
-      } else {
-        mbar_arrive(bar0 + 8u * uint32_t(b));  // the slot is the next tile's
+      } else if (v > 1) {
+        mbar_arrive(bar0 + 8u * uint32_t(b));  // the slot is the next tile's (vertex 1's: after the final segment)
       }
       cp_async_commit();
       double tE[m][D];
@@ -687,7 +703,6 @@ __global__ void __launch_bounds__(64, 4)
     }
     {  // own segment 0: the fixed end vertex
       double sd[h][D];
-      cp_async_wait_group<0>();
 #pragma unroll
       for (int d = 0; d < D; ++d) {
         sd[0][d] = *END(d);
@@ -695,6 +710,7 @@ __global__ void __launch_bounds__(64, 4)
         for (int b = 0; b < m; ++b) sd[1 + b][d] = fr.sgn(b) * *END(D + b * D + d);
       }
       const double T = *END(Lay::kEnd - 1);
+      mbar_arrive(bar0 + 8u * uint32_t(slot_of(1, j)));  // vertex 1's slot and END are the next tile's
       const double iT = fast_rcp(T);
       __syncwarp();
       out.emit(0, 0, T, iT, sd, ed, traj0);

@@ -1,6 +1,6 @@
 """Forced-configuration sweep of the chunked kernel K3 (developer tool, not the benchmark).
 
-Times K3 (N = 10, r = 4, D = 3) at K = 8, 16, 50 and 100 over
+Times K3 (N = 10, r = 4, D = 3) at K = 8, 12, 16, 50 and 100 over
   * C: vertex blocks per lane kept in shared memory (--cs, default 2 to 6),
   * warps per SM, from 4 up to the most that fit, as one-warp CTAs (W = 1) and as four-warp CTAs (W = 4),
   * pairs per SM of the paired form (W = 2: twisted_chunked_pair_kernel, which the default route launches), from 2
@@ -29,25 +29,26 @@ import mav_trajectory_generation_b200 as m  # noqa: E402
 from quick_bench import synth  # noqa: E402
 
 N, R, D = 10, 4, 3
-BATCH = {8: 1048576, 16: 1048576, 50: 246272, 100: 113664}
+BATCH = {8: 1048576, 12: 1048576, 16: 1048576, 50: 246272, 100: 113664}
 SMEM_PER_SM = 228 * 1024  # H100; every CTA also reserves 1 KB
 MAX_WARPS_BY_REGS = 8     # K3 at N = 10, D = 3 uses 248-250 registers per thread
 
 
-def k3_smem(C, W):
+def k3_smem(C, W, K):
     """Dynamic shared memory of K3 at N = 10, D = 3 (ChunkedLayout<10, 3, 3, W>::bytes, ring depth 3; W = 2:
     ChunkedPairLayout<10, 3, 3>::bytes)"""
     h, slots = N // 2, 25
     pro = 2 * D + (h - 1) * D + 1
-    if W == 2:  # ring, prologue, final-segment inputs, handoff, times, blocks; one staging tile; mbarriers
-        region = 3 * (1 + D) + pro + (D + (h - 1) * D + 1) + h * D + C
-        return 32 * (D * h * 16) + 256 + 32 * 8 * (region + C * slots)
+    if W == 2:  # one staging tile; mbarriers; tile input buffer; final-segment inputs, handoff, times, blocks
+        tile = 8 * 16 * (K + D * (2 * h + K - 1))
+        region = (D + (h - 1) * D + 1) + h * D + C
+        return 32 * (D * h * 16) + 256 + tile + 32 * 8 * (region + C * slots)
     region = 3 * (1 + D) + C + D + 1
     return 32 * W * (D * h * 16 + 8 * (region + max(C * slots, pro)))
 
 
-def max_warps(C, W):
-    return min(MAX_WARPS_BY_REGS, SMEM_PER_SM // (k3_smem(C, W) + 1024) * W)
+def max_warps(C, W, K):
+    return min(MAX_WARPS_BY_REGS, SMEM_PER_SM // (k3_smem(C, W, K) + 1024) * W)
 
 
 def configs(K, cs, ws, hint_modes):
@@ -58,13 +59,13 @@ def configs(K, cs, ws, hint_modes):
             continue
         for hints in hint_modes:
             if 1 in ws:
-                for w in range(4, max_warps(C, 1) + 1):
+                for w in range(4, max_warps(C, 1, K) + 1):
                     out.append(dict(C=C, W=1, warps=w, hints=hints))
             if 4 in ws:
-                for w in range(4, max_warps(C, 4) + 1, 4):
+                for w in range(4, max_warps(C, 4, K) + 1, 4):
                     out.append(dict(C=C, W=4, warps=w, hints=hints))
         if 2 in ws:  # the paired form runs without hints
-            for w in range(4, max_warps(C, 2) + 1, 2):
+            for w in range(4, max_warps(C, 2, K) + 1, 2):
                 out.append(dict(C=C, W=2, warps=w, hints=0))
     return out
 
