@@ -1,6 +1,7 @@
 // mtg_sweep.cuh -- the per-vertex arithmetic of the waypoint (block-tridiagonal) sweep, written once for every kernel
-// that runs it (v1 one-thread, v2 twisted, v3, v4, v5 and the chunked kernel K3) and the Hermite-form emission of the
-// twisted TMA kernels and the masked kernel.
+// that runs it (v1 one-thread, v2 twisted, v3, v4, v5 and the chunked kernel K3), the tile steps built from it that
+// v4, v5 and K3 share (Tile), the d_free writer of v2-v5 and K3 (FreeStore) and the Hermite-form emission of
+// the twisted TMA kernels and the masked kernel.
 //
 // Mathematics: see mtg_waypoint_kernel.cuh; twisted frames and index maps: mtg_twisted_kernel.cuh.  Each piece fixes
 // one operation order; the kernels only choose where they call it.  Two differences between kernels are deliberate
@@ -9,8 +10,9 @@
 //     carry with an exact power-of-two scaling (v4, v5, K3): carry_bcar / carry_fold and the two overloads of
 //     assemble() and middle().  The fold form starts the right-hand side with -cps*xm, which is not
 //     fma(-cps, xm, 0.0): the latter can flip the sign of a zero.
-//   * where the outward step's E u product is computed: couple() before the activity test in v4 and K3 (K3 runs
-//     at the register limit), inside it in v5; uncouple_from() interleaves it with the solve per dimension (v1-v3).
+//   * where the outward step's E u product is computed: Tile::outward_couple() before the activity test in v4 and K3
+//     (K3 runs at the register limit), inside it in v5; uncouple_from() interleaves it with the solve per dimension
+//     (v1-v3).
 // v1 sweeps the whole trajectory in one thread: it folds the far end's fixed derivatives u_K into the last
 // right-hand side between assemble() and factor(), and its last outward step has no coupling term.
 #pragma once
@@ -24,6 +26,19 @@ namespace mtg {
 template <int N, int D, bool kPos = false>
 __host__ __device__ constexpr int sweep_state_slots() {
   return (N / 2 - 1) * (N / 2) / 2 + (N / 2 - 1) * D + (kPos ? D : 0);
+}
+
+// pw[e] = T^(1-2R+e), e = 0..2m.
+template <int N, int R>
+__device__ __forceinline__ void segment_powers(double T, double invT, double (&pw)[N - 1]) {
+  constexpr int m = N / 2 - 1;
+  if constexpr (R == 0) {
+    pw[0] = T;
+  } else {
+    pw[0] = pow_int<2 * R - 1>(invT);
+  }
+#pragma unroll
+  for (int e = 1; e <= 2 * m; ++e) pw[e] = pw[e - 1] * T;
 }
 
 namespace sweep {
@@ -43,6 +58,33 @@ struct Frame {
   __device__ __forceinline__ double sgn(int idx) const { return (half && !(idx & 1)) ? -1.0 : 1.0; }
   // first fixed end-derivative slot of own-frame vertex 0
   __device__ __forceinline__ int e0() const { return half ? N / 2 + K : 1; }
+};
+
+// writer of one trajectory's free derivatives into d_free [B][D][(K-1)*m], in getFreeConstraints order; writes
+// nothing when d_free is null or the lane's row lies past B
+template <int N, int D>
+struct FreeStore {
+  static constexpr int h = N / 2;
+  static constexpr int m = h - 1;
+  const Frame<N>& fr;
+  int np;
+  double* df;
+  bool valid;
+  __device__ __forceinline__ FreeStore(double* dfree, long long traj, bool valid_, const Frame<N>& fr_)
+      : fr(fr_),
+        np((fr_.K - 1) * m),
+        df(dfree != nullptr ? dfree + traj * (long long)D * np : nullptr),
+        valid(valid_) {}
+  // derivatives 1..m of own-frame vertex v_own: u[1 + j][d], own-frame sign
+  __device__ __forceinline__ void operator()(int v_own, const double (&u)[h][D]) const {
+    if (df != nullptr && valid) {
+      const int vo = fr.vert(v_own);
+#pragma unroll
+      for (int d = 0; d < D; ++d)
+#pragma unroll
+        for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
+    }
+  }
 };
 
 template <int N, int D, class G>
@@ -426,6 +468,102 @@ struct Sweep {
         um[j][d] = s * inv[j];
       }
     }
+  }
+};
+
+// The tile steps of the carry-fold kernels v4, v5 and the one-warp K3, whose results the tests hold bitwise equal:
+// every step fixes its operation order once for all three.  The steps do no memory traffic: inputs arrive as
+// values or accessors, state blocks leave and return as register arrays, and the kernels place the loads, stores
+// and handshakes around the calls.  What the sweep towards the middle carries from one step to the next is the status
+// stat, the (W, y) carry Wp / yp, the end blocks Cee / cps / cpe of the segment stepped over last and the positions
+// xm / xc of the previous and the current vertex.  (They stay separate arrays of the kernel: gathered into one
+// struct, they change the machine code of v5.)
+template <int N, int R, int D>
+struct Tile {
+  using S = Sweep<N, D, H1Imm<N, R>>;
+  static constexpr int h = N / 2;
+  static constexpr int m = h - 1;
+
+  // own segment 0 of time T0, from own vertex 0 (fixed derivatives u0(b, d), own-frame sign) to vertex 1
+  template <class U0>
+  static __device__ __forceinline__ void first_segment(double T0, const U0& u0, int& stat, double (&Wp)[m][m],
+                                                       double (&yp)[m][D], double (&Cee)[m][m], double (&cps)[m],
+                                                       double (&cpe)[m]) {
+    stat = 0;
+    if (bad_segment_time(T0)) stat |= kStatusBadTime;
+    const double iT0 = fast_rcp(T0);
+    double pw[N - 1];
+    segment_powers<N, R>(T0, iT0, pw);
+    S::end_blocks(pw, Cee, cps, cpe);
+    S::carry_fold(pw, u0, Wp, yp);
+  }
+  // eliminates the current vertex over own segment v (time T, next vertex at xn): its state block -> sv, with the
+  // vertex position when sv has room for it
+  template <int SL>
+  static __device__ __forceinline__ void inward_step(double T, const double (&xn)[D], int& stat, double (&Wp)[m][m],
+                                                     double (&yp)[m][D], double (&Cee)[m][m], double (&cps)[m],
+                                                     double (&cpe)[m], double (&xm)[D], double (&xc)[D],
+                                                     double (&sv)[SL]) {
+    if (bad_segment_time(T)) stat |= kStatusBadTime;
+    const double iT = fast_rcp(T);
+    double pw[N - 1];
+    segment_powers<N, R>(T, iT, pw);
+    double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
+    S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
+    S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
+    S::pack(L, inv, yp, xc, sv);
+    S::end_blocks(pw, Cee, cps, cpe);
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+      xm[d] = xc[d];
+      xc[d] = xn[d];
+    }
+  }
+  // the middle vertex, where both halves meet (stat becomes the trajectory's status): ed = [x; u] of the middle
+  // vertex, the end derivatives of the first outward step
+  static __device__ __forceinline__ void meet(int& stat, const double (&Wp)[m][m], const double (&yp)[m][D],
+                                              const double (&Cee)[m][m], const double (&cps)[m],
+                                              const double (&cpe)[m], const double (&xm)[D], const double (&xc)[D],
+                                              double (&ed)[h][D]) {
+    double um[m][D];
+    S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+      ed[0][d] = xc[d];
+#pragma unroll
+      for (int j = 0; j < m; ++j) ed[1 + j][d] = um[j][d];
+    }
+  }
+
+  // outward step over own segment v (time T), coupling: tE = E_v u_{v+1}; returns 1/T
+  static __device__ __forceinline__ double outward_couple(double T, const double (&ed)[h][D], double (&tE)[m][D]) {
+    const double iT = fast_rcp(T);
+    double pw[N - 1];
+    segment_powers<N, R>(T, iT, pw);
+    S::couple(pw, ed, tE);
+    return iT;
+  }
+  // outward step, solve: sd = [x_v; u_v] from the vertex's state block sv, with the position x_v held in sv
+  template <int SL>
+  static __device__ __forceinline__ void outward_solve(const double (&sv)[SL], const double (&tE)[m][D],
+                                                       double (&sd)[h][D]) {
+    double xv[D];
+#pragma unroll
+    for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
+    S::back_substitute(sv, tE, xv, sd);
+  }
+  // ... or given as xv
+  template <int SL>
+  static __device__ __forceinline__ void outward_solve(const double (&sv)[SL], const double (&tE)[m][D],
+                                                       const double (&xv)[D], double (&sd)[h][D]) {
+    S::back_substitute(sv, tE, xv, sd);
+  }
+  // the vertex just solved becomes the end vertex of the next outward step
+  static __device__ __forceinline__ void advance(double (&ed)[h][D], const double (&sd)[h][D]) {
+#pragma unroll
+    for (int d = 0; d < D; ++d)
+#pragma unroll
+      for (int k = 0; k < h; ++k) ed[k][d] = sd[k][d];
   }
 };
 

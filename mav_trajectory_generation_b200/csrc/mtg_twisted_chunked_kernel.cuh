@@ -82,9 +82,8 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
   constexpr int kPro = Lay::kPro;
   constexpr int kThreads = Lay::kThreads;
   static_assert(RD >= 2, "ring depth");
-  using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
-  using S = sweep::Sweep<N, D, G>;
+  using Tile = sweep::Tile<N, R, D>;
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = W == 1 ? int(threadIdx.x) : int(threadIdx.x & 31);
@@ -181,7 +180,7 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
     }
     cp_async_wait_group<RD - 1>();
 
-    int stat = 0;
+    int stat;
     double Wp[m][m], yp[m][D], Cee[m][m], cps[m], cpe[m], xm[D], xc[D];
     {
 #pragma unroll
@@ -192,13 +191,8 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
       }
       const double T0 = *PRO(kPro - 1);
       stash[size_t(D) * kThreads] = T0;
-      if (bad_segment_time(T0)) stat |= kStatusBadTime;
-      const double iT0 = fast_rcp(T0);
-      double pw[N - 1];
-      segment_powers<N, R>(T0, iT0, pw);
-      S::end_blocks(pw, Cee, cps, cpe);
-      // initial carry from the fixed end derivatives (exact 2^+-600 scaling)
-      S::carry_fold(pw, [&](int b, int d) { return fr.sgn(b) * *PRO(2 * D + b * D + d); }, Wp, yp);
+      Tile::first_segment(T0, [&](int b, int d) { return fr.sgn(b) * *PRO(2 * D + b * D + d); }, stat, Wp, yp, Cee,
+                          cps, cpe);
     }
 
     // ---------------------------------------------------------------- sweep towards the middle
@@ -213,21 +207,7 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
         T = *PF(v % RD, 0);
         if (v + RD - 1 <= nh) ring_issue(P, v + RD - 1);  // nothing is left in flight after the last own step
         cp_async_commit();
-        if (bad_segment_time(T)) stat |= kStatusBadTime;
-        const double iT = fast_rcp(T);
-        double pw[N - 1];
-        segment_powers<N, R>(T, iT, pw);
-
-        double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
-        S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
-        S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
-        S::pack(L, inv, yp, xc, sv);
-        S::end_blocks(pw, Cee, cps, cpe);
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          xm[d] = xc[d];
-          xc[d] = xn[d];
-        }
+        Tile::inward_step(T, xn, stat, Wp, yp, Cee, cps, cpe, xm, xc, sv);
       }
       __syncwarp();
       if (v <= npark) {  // warp-uniform; every lane is active here (v < n <= nh + 1)
@@ -244,30 +224,12 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
     __syncwarp();
 
     // ---------------------------------------------------------------- middle vertex: both halves meet
-    double um[m][D];
-    S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
+    double ed[h][D];
+    Tile::meet(stat, Wp, yp, Cee, cps, cpe, xm, xc, ed);
     if (valid && half == 0 && prm.status != nullptr) prm.status[P.traj] = stat;
 
     // ---------------------------------------------------------------- outward back-substitution
-    const int np = (K - 1) * m;
-    double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + P.traj * (long long)D * np : nullptr;
-    auto store_free = [&](int v_own, const double (&u)[h][D]) {
-      if (df != nullptr && valid) {
-        const int vo = fr.vert(v_own);
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
-      }
-    };
-
-    double ed[h][D];
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-      ed[0][d] = xc[d];
-#pragma unroll
-      for (int j = 0; j < m; ++j) ed[1 + j][d] = um[j][d];
-    }
+    const sweep::FreeStore<N, D> store_free(prm.dfree, P.traj, valid, fr);
     if (half == 0) store_free(nh + 1, ed);
 
     // The ring is idle during the outward sweep: the fixed end derivatives needed by the final emission are
@@ -295,20 +257,14 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
       if (v <= npark) cp_async_wait_at_most(C - 1);
       const bool act = v <= nh;
       const double T = act ? *HT(b) : 1.0;
-      const double iT = fast_rcp(T);
-      double pw[N - 1];
-      segment_powers<N, R>(T, iT, pw);
+      double tE[m][D];  // E_v u_{v+1} (before the activity test: this kernel runs at the register limit)
+      const double iT = Tile::outward_couple(T, ed, tE);
       double sv[kSlots];
 #pragma unroll
       for (int i = 0; i < kSlots; ++i) sv[i] = *SP(b, i);
-      double tE[m][D];  // E_v u_{v+1} (before the activity test: this kernel runs at the register limit)
-      S::couple(pw, ed, tE);
       double sd[h][D];
       if (act) {
-        double xv[D];
-#pragma unroll
-        for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
-        S::back_substitute(sv, tE, xv, sd);
+        Tile::outward_solve(sv, tE, sd);
         store_free(v, sd);
       }
       if (v - C >= 1) {  // warp-uniform: the freed slot takes parked block v-C
@@ -319,12 +275,7 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
       cp_async_commit();
       __syncwarp();
       out.emit(v, v, T, iT, sd, ed, traj0);
-      if (act) {
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int k = 0; k < h; ++k) ed[k][d] = sd[k][d];
-      }
+      if (act) Tile::advance(ed, sd);
     }
     if (n > 0) issue_next_pro();  // the state region is dead only now
     {  // own segment 0: the fixed end vertex

@@ -130,17 +130,7 @@ __global__ void __launch_bounds__(32) twisted_solve_kernel(const WaypointParams 
 
   // ---------------------------------------------------------------- outward back-substitution
   double* __restrict__ out = prm.coeffs + traj * (long long)K * D * N;
-  const int np = (K - 1) * m;
-  double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + traj * (long long)D * np : nullptr;
-  auto store_free = [&](int v_own, const double (&u)[h][D]) {  // u[1+j][d]: own-frame derivatives
-    if (df != nullptr && valid) {
-      const int vo = fr.vert(v_own);
-#pragma unroll
-      for (int d = 0; d < D; ++d)
-#pragma unroll
-        for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
-    }
-  };
+  const sweep::FreeStore<N, D> store_free(prm.dfree, traj, valid, fr);
   // emit own-frame segment j (start derivatives sd at own vertex j, end derivatives ed at j+1).
   // For the reversed half the ORIGINAL segment starts at own vertex j+1: start = J ed, end = J sd.
   // The swap is a select per value (no divergent code path); J is folded into the time powers.

@@ -218,17 +218,7 @@
   if (valid && half == 0 && prm.status != nullptr) prm.status[traj] = stat;
 
   // ---------------------------------------------------------------- outward back-substitution
-  const int np = (K - 1) * m;
-  double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + traj * (long long)D * np : nullptr;
-  auto store_free = [&](int v_own, const double (&u)[h][D]) {
-    if (df != nullptr && valid) {
-      const int vo = fr.vert(v_own);
-#pragma unroll
-      for (int d = 0; d < D; ++d)
-#pragma unroll
-        for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
-    }
-  };
+  const sweep::FreeStore<N, D> store_free(prm.dfree, traj, valid, fr);
 
   double ed[h][D];
 #pragma unroll

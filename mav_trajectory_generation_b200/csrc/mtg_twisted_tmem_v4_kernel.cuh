@@ -60,9 +60,8 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
   static_assert(RD >= 2, "ring depth");
-  using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
-  using S = sweep::Sweep<N, D, G>;
+  using Tile = sweep::Tile<N, R, D>;
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -170,7 +169,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     }
     cp_async_wait_group<RD - 1>();
 
-    int stat = 0;
+    int stat;
     double Wp[m][m], yp[m][D], Cee[m][m], cps[m], cpe[m], xm[D], xc[D];
     {
       double T0;
@@ -185,13 +184,10 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       } else {
         T0 = *PRO(kPro - 1);
       }
-      if (bad_segment_time(T0)) stat |= kStatusBadTime;
+      Tile::first_segment(
+          T0, [&](int b, int d) { return FUSED ? 0.0 : fr.sgn(b) * *PRO(2 * D + b * D + d); }, stat, Wp, yp, Cee,
+          cps, cpe);
       HT(0) = T0;
-      const double iT0 = fast_rcp(T0);
-      double pw[N - 1];
-      segment_powers<N, R>(T0, iT0, pw);
-      S::end_blocks(pw, Cee, cps, cpe);
-      S::carry_fold(pw, [&](int b, int d) { return FUSED ? 0.0 : fr.sgn(b) * *PRO(2 * D + b * D + d); }, Wp, yp);
     }
 
     // ---------------------------------------------------------------- sweep towards the middle
@@ -211,21 +207,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         HT(v) = T;
         if (v + RD - 1 <= nh) ring_issue(P, v + RD - 1);  // nothing is left in flight after the last own step
         cp_async_commit();
-        if (bad_segment_time(T)) stat |= kStatusBadTime;
-        const double iT = fast_rcp(T);
-        double pw[N - 1];
-        segment_powers<N, R>(T, iT, pw);
-
-        double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
-        S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
-        S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
-        S::pack(L, inv, yp, xc, sv);
-        S::end_blocks(pw, Cee, cps, cpe);
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          xm[d] = xc[d];
-          xc[d] = xn[d];
-        }
+        Tile::inward_step(T, xn, stat, Wp, yp, Cee, cps, cpe, xm, xc, sv);
       }
       __syncwarp();
 #pragma unroll
@@ -234,30 +216,12 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     __syncwarp();
 
     // ---------------------------------------------------------------- middle vertex
-    double um[m][D];
-    S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
+    double ed[h][D];
+    Tile::meet(stat, Wp, yp, Cee, cps, cpe, xm, xc, ed);
     if (valid && half == 0 && prm.status != nullptr) prm.status[P.traj] = stat;
 
     // ---------------------------------------------------------------- outward back-substitution
-    const int np = (K - 1) * m;
-    double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + P.traj * (long long)D * np : nullptr;
-    auto store_free = [&](int v_own, const double (&u)[h][D]) {
-      if (df != nullptr && valid) {
-        const int vo = fr.vert(v_own);
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
-      }
-    };
-
-    double ed[h][D];
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-      ed[0][d] = xc[d];
-#pragma unroll
-      for (int j = 0; j < m; ++j) ed[1 + j][d] = um[j][d];
-    }
+    const sweep::FreeStore<N, D> store_free(prm.dfree, P.traj, valid, fr);
     if (half == 0) store_free(nh + 1, ed);
 
     // The ring is idle during the outward sweep: the fixed end derivatives needed by the final emission are
@@ -287,33 +251,22 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     for (int v = nmax; v >= 1; --v) {
       const bool act = v <= nh;
       const double T = act ? HT(v) : 1.0;
-      const double iT = fast_rcp(T);
-      double pw[N - 1];
-      segment_powers<N, R>(T, iT, pw);
+      double tE[m][D];
+      const double iT = Tile::outward_couple(T, ed, tE);
       double sv[kSlots];
 #pragma unroll
       for (int i = 0; i < kSlots; ++i) sv[i] = SP(v - 1, i);
-      double tE[m][D];
-      S::couple(pw, ed, tE);
       double sd[h][D];
       if (act) {
-        double xv[D];
-#pragma unroll
-        for (int d = 0; d < D; ++d) xv[d] = S::position(sv, d);
         if constexpr (FUSED) {
           if (tout != nullptr && valid) tout[fr.seg(v)] = T;
         }
-        S::back_substitute(sv, tE, xv, sd);
+        Tile::outward_solve(sv, tE, sd);
         store_free(v, sd);
       }
       __syncwarp();
       out.emit(v, v, T, iT, sd, ed, traj0);
-      if (act) {
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int k = 0; k < h; ++k) ed[k][d] = sd[k][d];
-      }
+      if (act) Tile::advance(ed, sd);
     }
     if (nmax > 0) issue_next_pro();  // the state region is dead only now
     {

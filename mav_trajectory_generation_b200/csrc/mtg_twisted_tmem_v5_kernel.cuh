@@ -100,9 +100,8 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
   constexpr int kSlots = Lay::kSlots;
   constexpr unsigned kFull = 0xffffffffu;
   constexpr int kWarps = kTmemThreads / 32;
-  using G = H1Imm<N, R>;
   using AI = A1InvImm<N>;
-  using S = sweep::Sweep<N, D, G>;
+  using Tile = sweep::Tile<N, R, D>;
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -207,7 +206,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     const long long traj0 = wt * 16;
     const long long traj = traj0 + tl_row;
 
-    int stat = 0;
+    int stat;
     double Wp[m][m], yp[m][D], Cee[m][m], cps[m], cpe[m], xm[D], xc[D];
     {
 #pragma unroll
@@ -222,12 +221,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
       } else {
         T0 = in_T(0);
       }
-      if (bad_segment_time(T0)) stat |= kStatusBadTime;
-      const double iT0 = fast_rcp(T0);
-      double pw[N - 1];
-      segment_powers<N, R>(T0, iT0, pw);
-      S::end_blocks(pw, Cee, cps, cpe);
-      S::carry_fold(pw, in_u0, Wp, yp);
+      Tile::first_segment(T0, in_u0, stat, Wp, yp, Cee, cps, cpe);
     }
 
     // ---------------------------------------------------------------- sweep towards the middle
@@ -244,21 +238,7 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         } else {
           T = in_T(v);
         }
-        if (bad_segment_time(T)) stat |= kStatusBadTime;
-        const double iT = fast_rcp(T);
-        double pw[N - 1];
-        segment_powers<N, R>(T, iT, pw);
-
-        double Dp[m][m], E[m][m], bb[m][D], L[m][m], inv[m];
-        S::assemble(pw, Cee, cps, cpe, Wp, yp, xm, xc, xn, Dp, E, bb);
-        S::factor(Dp, E, bb, L, inv, Wp, yp, stat);
-        S::pack(L, inv, yp, nullptr, sv);
-        S::end_blocks(pw, Cee, cps, cpe);
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          xm[d] = xc[d];
-          xc[d] = xn[d];
-        }
+        Tile::inward_step(T, xn, stat, Wp, yp, Cee, cps, cpe, xm, xc, sv);
       }
       __syncwarp();
 #pragma unroll
@@ -267,30 +247,12 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
     __syncwarp();
 
     // ---------------------------------------------------------------- middle vertex
-    double um[m][D];
-    S::middle(Cee, cps, cpe, Wp, yp, xm, xc, um, stat);
+    double ed[h][D];
+    Tile::meet(stat, Wp, yp, Cee, cps, cpe, xm, xc, ed);
     if (half == 0 && prm.status != nullptr) prm.status[traj] = stat;
 
     // ---------------------------------------------------------------- outward back-substitution
-    const int np = (K - 1) * m;
-    double* __restrict__ df = prm.dfree != nullptr ? prm.dfree + traj * (long long)D * np : nullptr;
-    auto store_free = [&](int v_own, const double (&u)[h][D]) {
-      if (df != nullptr) {
-        const int vo = fr.vert(v_own);
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int j = 0; j < m; ++j) df[d * np + (vo - 1) * m + j] = fr.sgn(j) * u[1 + j][d];
-      }
-    };
-
-    double ed[h][D];
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-      ed[0][d] = xc[d];
-#pragma unroll
-      for (int j = 0; j < m; ++j) ed[1 + j][d] = um[j][d];
-    }
+    const sweep::FreeStore<N, D> store_free(prm.dfree, traj, true, fr);
     if (half == 0) store_free(nh + 1, ed);
 
     constexpr int kStash0 = EARLY * kSlots;  // state slots of the blocks >= EARLY: popped when the sweep reaches vertex EARLY
@@ -338,22 +300,14 @@ __global__ void __launch_bounds__(kTmemThreads, MINB)
         if constexpr (FUSED) {
           if (prm.times_out != nullptr) prm.times_out[traj * K + fr.seg(v)] = T;
         }
-        iT = fast_rcp(T);
-        double pw[N - 1];
-        segment_powers<N, R>(T, iT, pw);
         double tE[m][D];
-        S::couple(pw, ed, tE);
-        S::back_substitute(sv, tE, xv, sd);
+        iT = Tile::outward_couple(T, ed, tE);
+        Tile::outward_solve(sv, tE, xv, sd);
         store_free(v, sd);
       }
       __syncwarp();
       out.emit(v, v, T, iT, sd, ed, traj0);
-      if (act) {
-#pragma unroll
-        for (int d = 0; d < D; ++d)
-#pragma unroll
-          for (int k = 0; k < h; ++k) ed[k][d] = sd[k][d];
-      }
+      if (act) Tile::advance(ed, sd);
     }
     {
       double sd[h][D];

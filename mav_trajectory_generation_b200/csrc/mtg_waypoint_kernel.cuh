@@ -102,19 +102,6 @@ __device__ __forceinline__ double nfabian_time(const double (&a)[D], const doubl
   return __dmul_rn(lead, fac);
 }
 
-// pw[e] = T^(1-2R+e), e = 0..2m.
-template <int N, int R>
-__device__ __forceinline__ void segment_powers(double T, double invT, double (&pw)[N - 1]) {
-  constexpr int m = N / 2 - 1;
-  if constexpr (R == 0) {
-    pw[0] = T;
-  } else {
-    pw[0] = pow_int<2 * R - 1>(invT);
-  }
-#pragma unroll
-  for (int e = 1; e <= 2 * m; ++e) pw[e] = pw[e - 1] * T;
-}
-
 // Emit the N coefficients of every dimension of one segment.
 //   sd[k][d], ed[k][d]: derivative k (0..m) at the segment start / end.
 // p_j = T^-j * sum_s A1inv[j][s] * T^(s mod h) * d_s ; for j < h this is d_j / j! exactly as the
