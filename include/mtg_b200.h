@@ -261,7 +261,7 @@ int mtg_scale_times_with_violation_batch_f64(mtg_handle* h, const mtg_problem* p
                                              double* seg_times_out, int32_t* within_range, double* maxima,
                                              int32_t* status, void* stream);
 
-/* Result codes of mtg_optimize_time_mellinger_batch_f64: the public nlopt_result values, so that callers of the
+/* Result codes of mtg_optimize_time_mellinger_batch_f64 and mtg_optimize_time_batch_f64: the public nlopt_result values, so that callers of the
  * reference read stopping reasons as before. */
 #define MTG_OPTIMIZE_RESULT_FAILURE (-1)
 #define MTG_OPTIMIZE_RESULT_ROUNDOFF_LIMITED (-4)
@@ -316,6 +316,47 @@ int mtg_optimize_time_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
                                           double a_max, double* coeffs, double* seg_times_out, double* relative_times,
                                           double* cost, int32_t* iterations, int32_t* result, int32_t* within_range,
                                           double* maxima, int32_t* status, void* stream);
+
+/* PolynomialOptimizationNonLinear::optimize() with kSquaredTime or kRichterTime (optimizeTime(), impl/
+ * polynomial_optimization_nonlinear_impl.h:132-168) for B trajectories: the K segment times minimise the objective of
+ * mtg_time_objective_batch_f64 (d_free == NULL) with the caller's `obj`, bounded below by 0.1 s.  obj->time_cost picks
+ * the method (0 kSquaredTime, 1 kRichterTime).  The reference drives the search with NLopt's LN_BOBYQA; this entry
+ * defines its own derivative-free compass search, per row, with x = the K segment times, l = 0.1, f(x) = that
+ * objective, and e counting objective evaluations (OptimizationInfo::n_iterations):
+ *   1. Start.  A segment time <= 0 or non-finite: FAILURE, status MTG_STATUS_BAD_TIME, times unchanged, e = 0.  A time
+ *      in (0, 0.1): FAILURE, not iterated, e = 1 (the Mellinger entry's decision).  Otherwise f_0 = f(x_0), e = 1; a
+ *      start solve reporting MTG_STATUS_NOT_SPD gives FAILURE.
+ *   2. Steps.  delta_i = fl(rho * x_0,i), rho = initial_stepsize_rel (<= 0: 0.1), NLopt's initial_step as the
+ *      reference sets it (:139-147).
+ *   3. Poll, only if max_iterations < 0 or e + 2K <= max_iterations (else stop: MAXEVAL_REACHED).  Candidate j = 2i
+ *      has y_i = fl(x_i + delta_i), j = 2i + 1 has y_i = max(l, fl(x_i - delta_i)) (`v > l ? v : l`, no FMA); every
+ *      other coordinate equals x.  All 2K are evaluated: e += 2K.
+ *   4. Accept.  j* = the candidate with the smallest objective, the lowest j on a tie.  f(y_j*) < f(x) (strict; a NaN
+ *      never wins): x = y_j*, f = f(y_j*), delta unchanged.  Otherwise every delta_i = delta_i / 2.  Any candidate
+ *      solve reporting MTG_STATUS_NOT_SPD ends the row: FAILURE, keeps x, status bit set.
+ *   5. Stop, tested in this order after each poll.  After an accepted poll: |df| <= f_rel * |f_new| (f_rel >= 0) or
+ *      <= f_abs (f_abs >= 0): FTOL_REACHED; else, when x_rel >= 0 or x_abs >= 0, every |dx_i| <= x_rel * |x_i| or
+ *      <= x_abs: XTOL_REACHED.  After a failed poll: when x_rel >= 0 or x_abs >= 0, every halved delta_i <= x_rel *
+ *      |x_i| or <= x_abs: XTOL_REACHED; else, every candidate of the next poll equal to x bit for bit:
+ *      ROUNDOFF_LIMITED.  Otherwise the next poll (step 3).
+ * The objective strictly decreases over finitely many fp64 points and delta reaches rounding after about 55 halvings,
+ * so every row stops even without tolerances.  params: the fields of mtg_mellinger_params are read as NLopt reads
+ * NonlinearOptimizationParameters; max_iterations counts OBJECTIVE EVALUATIONS (NLopt's maxeval), not gradient
+ * evaluations as in mtg_optimize_time_mellinger_batch_f64.
+ * Outputs: seg_times_out [B][K] the BEST point the search found (may be seg_times; the reference leaves its problem at
+ * the last point NLopt evaluated, which need not be the best); coeffs [B][K][D][N] the solve at it; objective [B] and
+ * terms [B][3] as mtg_time_objective_batch_f64 there; evaluations [B] e; result [B] MTG_OPTIMIZE_RESULT_*; status [B]
+ * the objective's status bits at the returned times, with MTG_STATUS_NOT_SPD when a candidate's solve failed.  No
+ * scaleSegmentTimesWithViolation follows (optimizeTime() does not call it).  Everything after seg_times_out is
+ * nullable.  A row's result does not depend on the other rows of the batch.  Like the Mellinger entry this one WAITS
+ * on `stream` once per poll to read the number of rows still iterating.  Refused (MTG_ERR_BAD_ARG, no launch): what
+ * mtg_time_objective_batch_f64 refuses, a null params, and params with every tolerance negative and
+ * max_iterations < 0. */
+int mtg_optimize_time_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                const double* d_fixed, const mtg_time_objective* obj,
+                                const mtg_mellinger_params* params, double* coeffs, double* seg_times_out,
+                                double* objective, double* terms, int32_t* evaluations, int32_t* result,
+                                int32_t* status, void* stream);
 
 /* FeasibilityAnalytic::checkInputFeasibility per segment and checkInputFeasibilityTrajectory per trajectory (reference
  * mav_trajectory_generation_ros/src/feasibility_analytic.cpp, feasibility_base.cpp).  result[b] is an MTG_FEAS_* code
@@ -548,6 +589,11 @@ int mtg_optimize_time_mellinger_batch_host_f64(mtg_handle* h, const mtg_problem*
                                                double* relative_times, double* cost, int32_t* iterations,
                                                int32_t* result, int32_t* within_range, double* maxima,
                                                int32_t* status);
+int mtg_optimize_time_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                     const double* d_fixed, const mtg_time_objective* obj,
+                                     const mtg_mellinger_params* params, double* coeffs, double* seg_times_out,
+                                     double* objective, double* terms, int32_t* evaluations, int32_t* result,
+                                     int32_t* status);
 
 int mtg_input_feasibility_batch_host_f64(mtg_handle* h, int32_t N, int32_t K, int32_t D, int64_t B,
                                          const double* seg_times, const double* coeffs,

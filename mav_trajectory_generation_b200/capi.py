@@ -44,7 +44,7 @@ EXPORTED_SYMBOLS = [
     "mtg_input_feasibility_sampling_batch_host_f64", "mtg_sample_flat_states_batch_f64",
     "mtg_sample_flat_state_at_time_batch_f64", "mtg_sample_flat_states_batch_host_f64",
     "mtg_sample_flat_state_at_time_batch_host_f64", "mtg_optimize_time_mellinger_batch_f64",
-    "mtg_optimize_time_mellinger_batch_host_f64",
+    "mtg_optimize_time_mellinger_batch_host_f64", "mtg_optimize_time_batch_f64", "mtg_optimize_time_batch_host_f64",
 ]
 # mav_msgs::EigenTrajectoryPoint as one record of MTG_FLAT_STATE_DOUBLES doubles: the slice of each field
 FLAT_STATE_DOUBLES = 25
@@ -308,6 +308,9 @@ def load():
                                                         C.POINTER(MtgMellingerParams), dbl, dbl, dp, dp, dp, dp, dp,
                                                         dp, dp, dp, dp, vp]
     L.mtg_optimize_time_mellinger_batch_host_f64.argtypes = L.mtg_optimize_time_mellinger_batch_f64.argtypes[:-1]
+    L.mtg_optimize_time_batch_f64.argtypes = [vp, C.POINTER(MtgProblem), i64, dp, dp, C.POINTER(MtgTimeObjective),
+                                              C.POINTER(MtgMellingerParams), dp, dp, dp, dp, dp, dp, dp, vp]
+    L.mtg_optimize_time_batch_host_f64.argtypes = L.mtg_optimize_time_batch_f64.argtypes[:-1]
     for name in EXPORTED_SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export what the header declares
     _lib = L
@@ -633,6 +636,36 @@ class Solver:
     _MELLINGER_OUTPUTS = ("coeffs", "seg_times", "relative_times", "cost", "iterations", "result", "within_range",
                           "maxima", "status")
 
+    def optimize_time(self, prob, seg_times, d_fixed, constraints=(), time_cost=TIME_COST_SQUARED, params=None,
+                      time_penalty=500.0, soft_constraint_weight=100.0, maximum_cost=1e12, seg_times_out=None,
+                      stream=None):
+        """Batched PolynomialOptimizationNonLinear::optimize() with kSquaredTime (time_cost TIME_COST_SQUARED) or
+        kRichterTime (TIME_COST_RICHTER), as the compass search of mtg_b200.h: -> dict of coeffs [B][K][D][N],
+        seg_times [B][K] (the best point), objective [B], terms [B][3], evaluations [B], result [B]
+        (OPTIMIZE_RESULT_*), status [B].  constraints: soft [(derivative, max_value), ...]; params: a mellinger_params()
+        whose max_iterations counts objective evaluations.  Waits on the stream once per poll."""
+        import torch
+        B = seg_times.shape[0]
+        dev = seg_times.device
+        if params is None:
+            params = mellinger_params()
+        obj = time_objective_params(time_cost, time_penalty, soft_constraint_weight, maximum_cost, constraints)
+        out = dict(coeffs=torch.empty((B, prob.K, prob.D, prob.N), dtype=torch.float64, device=dev),
+                   seg_times=seg_times_out if seg_times_out is not None else torch.empty_like(seg_times),
+                   objective=torch.empty((B,), dtype=torch.float64, device=dev),
+                   terms=torch.empty((B, 3), dtype=torch.float64, device=dev),
+                   evaluations=torch.empty((B,), dtype=torch.int32, device=dev),
+                   result=torch.empty((B,), dtype=torch.int32, device=dev),
+                   status=torch.empty((B,), dtype=torch.int32, device=dev))
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.mtg_optimize_time_batch_f64(
+            self.h, C.byref(prob.c), B, seg_times.data_ptr(), d_fixed.data_ptr(), C.byref(obj), C.byref(params),
+            *[out[k].data_ptr() for k in self._OPTIMIZE_TIME_OUTPUTS], s)
+        self._check(rc, "mtg_optimize_time_batch_f64")
+        return out
+
+    _OPTIMIZE_TIME_OUTPUTS = ("coeffs", "seg_times", "objective", "terms", "evaluations", "result", "status")
+
     def check_input_feasibility(self, seg_times, coeffs, limits, min_section_time=0.05, gravity=GRAVITY, stream=None):
         """Batched FeasibilityAnalytic::checkInputFeasibilityTrajectory: (result [B], segment [B], status [B]), int32.
         limits: {name: value} over INPUT_LIMITS (absent name = no limit; default_input_limits() gives the reference's
@@ -839,6 +872,26 @@ class Solver:
             self.h, C.byref(prob.c), B, seg_times.ctypes.data, d_fixed.ctypes.data, C.byref(params), float(v_max),
             float(a_max), *[out[k].ctypes.data for k in self._MELLINGER_OUTPUTS])
         self._check(rc, "mtg_optimize_time_mellinger_batch_host_f64")
+        return out
+
+    def optimize_time_host(self, prob, seg_times, d_fixed, constraints=(), time_cost=TIME_COST_SQUARED, params=None,
+                           time_penalty=500.0, soft_constraint_weight=100.0, maximum_cost=1e12):
+        """optimize_time on host numpy arrays (one copy in, the search, one copy out): a dict of numpy arrays with
+        the same keys."""
+        B, K = seg_times.shape
+        if params is None:
+            params = mellinger_params()
+        obj = time_objective_params(time_cost, time_penalty, soft_constraint_weight, maximum_cost, constraints)
+        seg_times = np.ascontiguousarray(seg_times, dtype=np.float64)
+        d_fixed = np.ascontiguousarray(d_fixed, dtype=np.float64)
+        f8, i4 = np.float64, np.int32
+        out = dict(coeffs=np.empty((B, K, prob.D, prob.N), f8), seg_times=np.empty((B, K), f8),
+                   objective=np.empty(B, f8), terms=np.empty((B, 3), f8), evaluations=np.empty(B, i4),
+                   result=np.empty(B, i4), status=np.empty(B, i4))
+        rc = self.lib.mtg_optimize_time_batch_host_f64(
+            self.h, C.byref(prob.c), B, seg_times.ctypes.data, d_fixed.ctypes.data, C.byref(obj), C.byref(params),
+            *[out[k].ctypes.data for k in self._OPTIMIZE_TIME_OUTPUTS])
+        self._check(rc, "mtg_optimize_time_batch_host_f64")
         return out
 
     def scale_times_with_violation_host(self, prob, seg_times, d_fixed, v_max, a_max, coeffs, seg_times_out,

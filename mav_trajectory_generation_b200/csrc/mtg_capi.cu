@@ -21,6 +21,7 @@
 #include "mtg_generic_kernel.cuh"
 #include "mtg_half_plane_kernel.cuh"
 #include "mtg_mellinger_loop_kernel.cuh"
+#include "mtg_time_search_kernel.cuh"
 #include "mtg_twisted_kernel.cuh"
 #include "mtg_twisted_tmem_kernel.cuh"
 #include "mtg_twisted_tmem_v4_kernel.cuh"
@@ -85,7 +86,8 @@ struct mtg_handle {
   Arena pack[kPipe + 1];     // times + d_fixed produced by nfabian_pack_kernel; Mellinger expansion
   Arena counters[kPipe + 1]; // dynamic tile counter of the persistent kernels (event-ordered like the scratch arenas: two
                              // launches of one slot on different caller streams must not share a live counter)
-  Arena optim[kPipe + 1];    // Mellinger outer loop: compact row lists and per-row state across its iterations
+  Arena optim[kPipe + 1];    // Mellinger outer loop and compass search: compact row lists and per-row state across
+                             // their iterations; the compass search's candidate chunk too (up to kTimeSearchBudget)
   int* pinned_count = nullptr;        // the outer loop's active-row count, read back once per iteration
   cudaEvent_t count_ev = nullptr;
   // What is known about each kernel function launched so far, queried or set once per function so that a repeated
@@ -2004,6 +2006,132 @@ int mtg_optimize_time_mellinger_batch_f64(mtg_handle* h, const mtg_problem* p, i
       });
 }
 
+// ---- the compass search on the segment times (optimize() with kSquaredTime / kRichterTime) -------------------------
+// Device memory for one poll's candidates (times, d_fixed, coefficients, objective, status): larger batches are
+// evaluated in chunks of at most this many bytes (DESIGN.md section 3f).
+constexpr size_t kTimeSearchBudget = size_t(512) << 20;
+
+static bool valid_optimize_time(const mtg_problem* p, int64_t B, const mtg_time_objective* obj,
+                                const mtg_mellinger_params* q, const double* seg_times, const double* d_fixed,
+                                const double* coeffs, const double* seg_times_out) {
+  return valid_objective(p, B, obj, seg_times, d_fixed, coeffs, seg_times_out) && valid_mellinger_params(q);
+}
+
+static int launch_optimize_time(mtg_handle* h, const mtg_problem* p, CachedTopology* topo, int64_t B,
+                                const double* seg_times, const double* d_fixed, const mtg_time_objective* obj,
+                                const mtg_mellinger_params* q, double* coeffs, double* seg_times_out,
+                                double* objective, double* terms, int32_t* evaluations, int32_t* result,
+                                int32_t* status, cudaStream_t s, int slot) {
+  const size_t K = p->K, D = p->D, N = p->N, C = 2 * K, dnf = D * topo->layout.n_fixed, nB = size_t(B);
+  // candidates per chunk: a multiple of 16 (8 rows), so that the expanded batch keeps the TMA-input route
+  const size_t per_x = (K + dnf + K * D * N + 1) * 8 + 4;
+  size_t chunk = std::max<size_t>(8, kTimeSearchBudget / (per_x * C) / 8 * 8);
+  chunk = std::min(chunk, nB);
+  const size_t nx = chunk * C, ni = (nB + 1) / 2;
+  // arena (optim; launch_time_objective takes pack): [B] f0, [2] lists of ([B] idx, [B][K] x, [B][K] delta, [B] f,
+  // [B][dnf] d_fixed), [B] evals, result, opt_status, st0, st_final, the count, then one chunk's candidates
+  size_t off = 0;
+  auto take = [&](size_t doubles) {
+    const size_t o = off;
+    off += align_doubles(doubles);
+    return o;
+  };
+  const size_t o_f0 = take(nB), o_idx[2] = {take(ni), take(ni)}, o_x[2] = {take(nB * K), take(nB * K)},
+               o_d[2] = {take(nB * K), take(nB * K)}, o_f[2] = {take(nB), take(nB)},
+               o_df[2] = {take(nB * dnf), take(nB * dnf)}, o_ev = take(ni), o_res = take(ni), o_ost = take(ni),
+               o_st0 = take(ni), o_stf = take(ni), o_cnt = take(1), o_tx = take(nx * K), o_fx = take(nx * dnf),
+               o_cx = take(nx * K * D * N), o_fc = take(nx), o_stc = take((nx + 1) / 2);
+  mtg_handle::Arena& ar = h->optim[slot];
+  MTG_TRY(arena_acquire(h, ar, off * 8, s));
+  double* base = ar.p;
+  auto ip = [&](size_t o) { return reinterpret_cast<int32_t*>(base + o); };
+  int32_t* d_count = ip(o_cnt);
+
+  mtg::TimeSearchParams tp{};
+  tp.K = p->K;
+  tp.dnf = int(dnf);
+  tp.B = B;
+  tp.max_iterations = q->max_iterations;
+  tp.f_abs = q->f_abs;
+  tp.f_rel = q->f_rel;
+  tp.x_rel = q->x_rel;
+  tp.x_abs = q->x_abs;
+  tp.init_rel = q->initial_stepsize_rel;
+  tp.lower = 0.1;  // kOptimizationTimeLowerBound (polynomial_optimization_nonlinear.h)
+  tp.x_out = seg_times_out;
+  tp.evals_out = ip(o_ev);
+  tp.result = ip(o_res);
+  tp.opt_status = ip(o_ost);
+  tp.count_next = d_count;
+  const int threads = 128;
+  auto set_lists = [&](int c) {
+    tp.idx = ip(o_idx[c]);
+    tp.x = base + o_x[c];
+    tp.delta = base + o_d[c];
+    tp.f = base + o_f[c];
+    tp.dfix = base + o_df[c];
+    tp.idx_next = ip(o_idx[c ^ 1]);
+    tp.x_next = base + o_x[c ^ 1];
+    tp.delta_next = base + o_d[c ^ 1];
+    tp.f_next = base + o_f[c ^ 1];
+    tp.dfix_next = base + o_df[c ^ 1];
+  };
+  // f(x0) for every row (coeffs is scratch until the final evaluation), then the start lists the iterating rows
+  // into list 0
+  MTG_TRY(launch_time_objective(h, p, topo, B, seg_times, d_fixed, nullptr, obj, coeffs, base + o_f0, nullptr,
+                                ip(o_st0), s, slot));
+  set_lists(1);
+  MTG_CUDA(h, cudaMemsetAsync(d_count, 0, sizeof(int32_t), s));
+  MTG_TRY(launch_kernel(h, mtg::ts_init_kernel, (B + threads - 1) / threads, threads, 0, s, tp, seg_times,
+                        base + o_f0, ip(o_st0), d_fixed));
+  int rows = 0;
+  MTG_TRY(read_count(h, d_count, s, &rows));
+  int cur = 0;
+  for (int polls = 1; rows > 0; ++polls) {
+    set_lists(cur);
+    tp.evals = 1 + int(C) * polls;
+    MTG_CUDA(h, cudaMemsetAsync(d_count, 0, sizeof(int32_t), s));
+    for (int64_t r0 = 0; r0 < rows; r0 += int64_t(chunk)) {
+      const int64_t nr = std::min<int64_t>(int64_t(chunk), rows - r0), ncx = nr * int64_t(C);
+      mtg::TimeSearchParams cp = tp;
+      cp.rows = int(nr);
+      cp.idx = tp.idx + r0;
+      cp.x = tp.x + r0 * K;
+      cp.delta = tp.delta + r0 * K;
+      cp.f = tp.f + r0;
+      cp.dfix = tp.dfix + r0 * dnf;
+      cp.fc = base + o_fc;
+      cp.st_c = ip(o_stc);
+      MTG_TRY(launch_kernel(h, mtg::ts_expand_kernel, capped_grid(h, ncx, threads, 16), threads, 0, s, cp,
+                            base + o_tx, base + o_fx));
+      MTG_TRY(launch_time_objective(h, p, topo, ncx, base + o_tx, base + o_fx, nullptr, obj, base + o_cx, base + o_fc,
+                                    nullptr, ip(o_stc), s, slot));
+      MTG_TRY(launch_kernel(h, mtg::ts_decide_kernel, (nr + threads - 1) / threads, threads, 0, s, cp));
+    }
+    MTG_TRY(read_count(h, d_count, s, &rows));
+    cur ^= 1;
+  }
+  // the returned point's solve, objective and terms
+  MTG_TRY(launch_time_objective(h, p, topo, B, seg_times_out, d_fixed, nullptr, obj, coeffs,
+                                objective ? objective : base + o_f0, terms, ip(o_stf), s, slot));
+  MTG_TRY(launch_kernel(h, mtg::ts_finish_kernel, capped_grid(h, B, threads, 16), threads, 0, s, B, ip(o_ev),
+                        ip(o_res), ip(o_ost), ip(o_stf), evaluations, result, status));
+  return arena_release(h, ar, s);
+}
+
+int mtg_optimize_time_batch_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                const double* d_fixed, const mtg_time_objective* obj,
+                                const mtg_mellinger_params* params, double* coeffs, double* seg_times_out,
+                                double* objective, double* terms, int32_t* evaluations, int32_t* result,
+                                int32_t* status, void* stream) {
+  return run_problem_entry(
+      h, valid_optimize_time(p, B, obj, params, seg_times, d_fixed, coeffs, seg_times_out), p, B,
+      [&](CachedTopology* topo) {
+        return launch_optimize_time(h, p, topo, B, seg_times, d_fixed, obj, params, coeffs, seg_times_out, objective,
+                                    terms, evaluations, result, status, (cudaStream_t)stream, mtg_handle::kPipe);
+      });
+}
+
 // Every input-feasibility entry: N even in [4, 12]; the limits are final values (the host mirror's InputConstraints
 // applies addConstraint's corrections), each present one not NaN and >= 0 (+inf never fails); gravity finite.  Any D:
 // rows with D not 3 or 4 are Indeterminable, as in the reference.
@@ -2371,6 +2499,31 @@ int mtg_optimize_time_mellinger_batch_host_f64(mtg_handle* h, const mtg_problem*
         return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
           return launch_optimize_mellinger(h, p, topo, nb, d[0], d[1], params, v_max, a_max, d[2], d[0], d[3], d[4],
                                            d[5], d[6], d[7], d[8], d[9], s, slot);
+        });
+      });
+}
+
+int mtg_optimize_time_batch_host_f64(mtg_handle* h, const mtg_problem* p, int64_t B, const double* seg_times,
+                                     const double* d_fixed, const mtg_time_objective* obj,
+                                     const mtg_mellinger_params* params, double* coeffs, double* seg_times_out,
+                                     double* objective, double* terms, int32_t* evaluations, int32_t* result,
+                                     int32_t* status) {
+  return run_problem_entry(
+      h, valid_optimize_time(p, B, obj, params, seg_times, d_fixed, coeffs, seg_times_out), p, B,
+      [&](CachedTopology* topo) {
+        const size_t K = p->K, D = p->D, N = p->N;
+        // the times go in from seg_times and come back, optimised in place, into seg_times_out
+        const HostBuf bufs[] = {{seg_times, seg_times_out, K * 8},
+                                {d_fixed, nullptr, D * topo->layout.n_fixed * 8},
+                                {nullptr, coeffs, K * D * N * 8},
+                                {nullptr, objective, 8},
+                                {nullptr, terms, 24},
+                                {nullptr, evaluations, 4},
+                                {nullptr, result, 4},
+                                {nullptr, status, 4}};
+        return stage_host(h, B, Staging::OneChunk, bufs, [&](const DevBuf* d, int64_t nb, cudaStream_t s, int slot) {
+          return launch_optimize_time(h, p, topo, nb, d[0], d[1], obj, params, d[2], d[0], d[3], d[4], d[5], d[6], d[7],
+                                      s, slot);
         });
       });
 }

@@ -140,6 +140,11 @@ class BatchCore {
   bool optimizeTimeMellingerOuterLoop(const MellingerParameters& params, double v_max, double a_max,
                                       std::vector<int>* result, std::vector<int>* iterations,
                                       std::vector<double>* relative_times);
+  // PolynomialOptimizationNonLinear::optimize() with kSquaredTime / kRichterTime (params.richter_time) as the compass
+  // search of mtg_optimize_time_batch_f64: times_ and coeffs_ take the best point and its solve in place, status_ the
+  // entry's status bits.  result, evaluations, objective: [B], nullable.
+  bool optimizeTime(const TimeObjectiveParameters& objective_params, const MellingerParameters& params,
+                    std::vector<int>* result, std::vector<int>* evaluations, std::vector<double>* objective);
   // which reference checker checkInputFeasibility runs
   enum class InputChecker { kAnalytic, kRecursive, kSampling };
   // FeasibilityAnalytic, FeasibilityRecursive or FeasibilitySampling ::checkInputFeasibilityTrajectory of the current

@@ -115,6 +115,16 @@ class BatchPolynomialOptimization {
                                       std::vector<double>* relative_times = nullptr) {
     return core_.optimizeTimeMellingerOuterLoop(params, v_max, a_max, result, iterations, relative_times);
   }
+  // PolynomialOptimizationNonLinear::optimize() with kSquaredTime or kRichterTime (objective_params.richter_time;
+  // reference optimizeTime(), impl/polynomial_optimization_nonlinear_impl.h:132-168) for every problem, as the compass
+  // search of mtg_optimize_time_batch_f64: segmentTimes() and coefficients() take the best point found and its solve in
+  // place, status() the status bits.  params.max_iterations counts objective evaluations.  result
+  // (MTG_OPTIMIZE_RESULT_*), evaluations and objective (the objective at the returned times) are nullable.
+  bool optimizeTime(const b200::TimeObjectiveParameters& objective_params, const b200::MellingerParameters& params,
+                    std::vector<int>* result = nullptr, std::vector<int>* evaluations = nullptr,
+                    std::vector<double>* objective = nullptr) {
+    return core_.optimizeTime(objective_params, params, result, evaluations, objective);
+  }
   // FeasibilityAnalytic::checkInputFeasibilityTrajectory (reference mav_trajectory_generation_ros/src/
   // feasibility_analytic.cpp, feasibility_base.cpp) of every trajectory at its current coefficients, on the GPU:
   // result[b], and segment[b] = the first segment that is not feasible (-1 when the row is feasible or has a segment

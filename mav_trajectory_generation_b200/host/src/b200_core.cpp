@@ -73,6 +73,14 @@ mtg_mellinger_params toParams(const MellingerParameters& q) {
   p.max_iterations = q.max_iterations;
   return p;
 }
+// The C-ABI objective of `params`; its constraints array is *cons, which must outlive the call it is passed to.
+mtg_time_objective toObjective(const TimeObjectiveParameters& params, std::vector<mtg_soft_constraint>* cons) {
+  CHECK_LE(params.soft_constraints.size(), 8u);
+  cons->clear();
+  for (const auto& c : params.soft_constraints) cons->push_back({c.first, c.second});
+  return {params.richter_time ? 1 : 0, params.time_penalty, params.soft_constraint_weight, params.maximum_cost,
+          static_cast<int32_t>(cons->size()), cons->data()};
+}
 }  // namespace
 
 void hostMappingMatrix(int N, double T, double* A) {
@@ -716,11 +724,8 @@ void BatchCore::computeMaximaOfMagnitude(const std::vector<int>& derivatives, st
 bool BatchCore::timeObjective(const TimeObjectiveParameters& params, const double* d_free, std::vector<double>* objective,
                               std::vector<double>* terms) {
   CHECK_GT(B_, 0u) << "setup first";
-  CHECK_LE(params.soft_constraints.size(), 8u);
   std::vector<mtg_soft_constraint> cons;
-  for (const auto& c : params.soft_constraints) cons.push_back({c.first, c.second});
-  mtg_time_objective obj = {params.richter_time ? 1 : 0, params.time_penalty, params.soft_constraint_weight,
-                            params.maximum_cost, static_cast<int32_t>(cons.size()), cons.data()};
+  const mtg_time_objective obj = toObjective(params, &cons);
   CHECK_NOTNULL(objective)->assign(B_, 0.0);
   if (terms) terms->assign(3 * B_, 0.0);
   mtg_problem p = {N_, topo_.r, topo_.K, topo_.D, topo_.mask.data()};
@@ -790,6 +795,29 @@ bool BatchCore::optimizeTimeMellingerOuterLoop(const MellingerParameters& params
   }
   if (result) result->assign(res.begin(), res.end());
   if (iterations) iterations->assign(it.begin(), it.end());
+  return true;
+}
+
+bool BatchCore::optimizeTime(const TimeObjectiveParameters& objective_params, const MellingerParameters& params,
+                             std::vector<int>* result, std::vector<int>* evaluations, std::vector<double>* objective) {
+  CHECK_GT(B_, 0u) << "setup first";
+  std::vector<mtg_soft_constraint> cons;
+  const mtg_time_objective obj = toObjective(objective_params, &cons);
+  std::vector<int32_t> res(B_, 0), ev(B_, 0);
+  if (objective) objective->assign(B_, 0.0);
+  const mtg_mellinger_params prm = toParams(params);
+  mtg_problem p = {N_, topo_.r, topo_.K, topo_.D, topo_.mask.data()};
+  HandleLock lock;
+  mtg_handle* h = defaultHandle();
+  const int rc = mtg_optimize_time_batch_host_f64(h, &p, static_cast<int64_t>(B_), times_, d_fixed_, &obj, &prm,
+                                                  coeffs_, times_, objective ? objective->data() : nullptr, nullptr,
+                                                  ev.data(), res.data(), status_);
+  if (rc != MTG_OK) {
+    LOG(ERROR) << "mtg_optimize_time_batch_host_f64 failed (rc=" << rc << "): " << mtg_last_error(h);
+    return false;
+  }
+  if (result) result->assign(res.begin(), res.end());
+  if (evaluations) evaluations->assign(ev.begin(), ev.end());
   return true;
 }
 
