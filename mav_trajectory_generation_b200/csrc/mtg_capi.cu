@@ -109,13 +109,14 @@ struct mtg_handle {
     int carveout = 0;  // cudaFuncAttributePreferredSharedMemoryCarveout for these CTAs
   };
   std::vector<ChunkedPlan> chunked_plans;
-  // last encoded coefficient tensor map (B = 1 solveLinear() calls re-use the same output buffer)
+  // last encoded coefficient tensor map of each cache slot (B = 1 solveLinear() calls re-use the same output buffer):
+  // slot 0 holds boxes of one segment or less, slot 1 the paired chunked kernel's boxes of two segments
   struct TmapKey {
     const void* base = nullptr;
     int64_t B = 0;
     int K = 0, D = 0, N = 0, box = 0;
-  } tmap_key;
-  CUtensorMap tmap_cached;
+  } tmap_key[2];
+  CUtensorMap tmap_cached[2];
   cudaStream_t streams[kPipe] = {nullptr, nullptr, nullptr};
   void* dev_buf[kPipe] = {nullptr, nullptr, nullptr};
   size_t dev_buf_bytes[kPipe] = {0, 0, 0};
@@ -217,6 +218,8 @@ typedef void (*TmemKernel)(const mtg::WaypointParams, const CUtensorMap);  // v3
 typedef void (*V4Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV4, const CUtensorMap);
 typedef void (*V5Kernel)(const mtg::WaypointParams, const mtg::TmemLaunchV5, const CUtensorMap);
 typedef void (*ChunkedKernel)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap);
+typedef void (*ChunkedPairKernel)(const mtg::WaypointParams, const mtg::ChunkedLaunch, const CUtensorMap,
+                                  const CUtensorMap);
 struct WaypointEntry {
   int N, R, D;
   SweepKernel v2;                 // two lanes per trajectory (twisted factorisation), state in shared memory
@@ -226,7 +229,7 @@ struct WaypointEntry {
   ChunkedKernel k3[2];            // K3: any K, kChunkedWarps[i] warps per CTA
   size_t (*k3_smem[2])(int C);    // with C resident blocks per lane
   int k3_park;                    // doubles per thread of one vertex block that K3 parks in global memory
-  ChunkedKernel k3_pair;          // K3 in warp pairs (one tile's inward sweep beside the last tile's outward one)
+  ChunkedPairKernel k3_pair;      // K3 in warp pairs (one tile's inward sweep beside the last tile's outward one)
   size_t (*k3_pair_smem)(int C, int K, int nf);  // with C resident blocks per lane and its tile input buffer
   // null where the shape has no such instantiation
   SweepKernel v1;                 // one thread per trajectory (cross-checks and profiles)
@@ -479,8 +482,9 @@ struct DeviceGuard {
   }
 };
 
-// coeffs as a 2-D fp64 tensor [B][K*D*N] for the TMA stores (box = 16 trajectories x `box` doubles of one segment).
-// The last encoded map is kept: repeated calls on the same output buffer encode it once.
+// coeffs as a 2-D fp64 tensor [B][K*D*N] for the TMA stores (box = 16 trajectories x `box` doubles: at most one
+// segment, or two for the paired chunked kernel).  The last encoded map of each size class is kept: repeated calls
+// on the same output buffer encode it once.
 int coeff_tmap(mtg_handle* h, double* coeffs, int64_t B, const mtg_problem* p, int box, const CUtensorMap** out) {
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -494,8 +498,10 @@ int coeff_tmap(mtg_handle* h, double* coeffs, int64_t B, const mtg_problem* p, i
       return nullptr;
     return reinterpret_cast<EncodeFn>(fp);
   }();
-  mtg_handle::TmapKey& key = h->tmap_key;
-  *out = &h->tmap_cached;
+  const int slot = box > p->D * p->N ? 1 : 0;
+  mtg_handle::TmapKey& key = h->tmap_key[slot];
+  CUtensorMap* map = &h->tmap_cached[slot];
+  *out = map;
   if (key.base == coeffs && key.B == B && key.K == p->K && key.D == p->D && key.N == p->N && key.box == box)
     return MTG_OK;
   key.base = nullptr;
@@ -508,7 +514,7 @@ int coeff_tmap(mtg_handle* h, double* coeffs, int64_t B, const mtg_problem* p, i
   const cuuint64_t strides[1] = {row * sizeof(double)};
   const cuuint32_t boxdim[2] = {cuuint32_t(box), 16u};
   const cuuint32_t estr[2] = {1u, 1u};
-  const CUresult cr = encode(&h->tmap_cached, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, coeffs, dims, strides, boxdim, estr,
+  const CUresult cr = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, coeffs, dims, strides, boxdim, estr,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                              CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (cr != CUDA_SUCCESS) {
@@ -579,7 +585,8 @@ int chunked_residency(mtg_handle* h, const void* fn, size_t smem, int cap, int t
 }
 
 // ---- waypoint launches: plan_waypoint() decides, launch_waypoint() launches -------------------
-enum class Family { Sweep, Tmem, V4, V5, Chunked };  // v1 and v2, v3, v4, v5, K3: fixes the argument list
+enum class Family { Sweep, Tmem, V4, V5, Chunked, ChunkedPair };  // v1 and v2, v3, v4, v5, K3, paired K3: fixes the
+                                                                 // argument list
 struct WaypointPlan {
   Family family = Family::Sweep;
   const void* fn = nullptr;
@@ -662,6 +669,8 @@ int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, in
   // inward sweep (K >= 3); CHUNK_WARPS or L2_HINTS select the one-warp form.
   constexpr int kPairMaxBlocks = 7;
   constexpr int kAutoPairs = 2;
+  static_assert(kPairMaxBlocks == 7 && kAutoPairs == 2 && kSmemPerSm == 228 * 1024,
+                "ChunkedPairLayout::kStorePairs is sized for two pairs per SM at C = 7");
   const bool forced = h->chunk_blocks > 0 || h->ctas_per_sm > 0;
   if (pairs && h->chunk_warps == 0 && h->l2_hints == 0 && nmax >= 1 && (forced || nmax <= kPairMaxBlocks)) {
     const int C = h->chunk_blocks > 0 || nmax > kPairMaxBlocks ? best_C : nmax;
@@ -670,6 +679,7 @@ int plan_chunked(mtg_handle* h, const mtg_problem* p, const WaypointEntry& e, in
     int ctas = 0, carveout = 0;
     if (cap >= 1) MTG_TRY(chunked_residency(h, (const void*)e.k3_pair, smem, cap, 64, &ctas, &carveout));
     if (ctas >= (forced ? 1 : kAutoPairs)) {
+      pl->family = Family::ChunkedPair;
       pl->fn = (const void*)e.k3_pair;
       pl->threads = 64;
       pl->smem = smem;
@@ -837,6 +847,13 @@ int launch_waypoint(mtg_handle* h, const mtg_problem* p, const WaypointPlan& pl,
     case Family::Chunked: {
       const mtg::ChunkedLaunch cl{pl.chunk, pl.park_bytes > 0 ? held->p : nullptr, pl.evict_first};
       MTG_TRY(launch_kernel(h, (ChunkedKernel)pl.fn, grid, block, pl.smem, stream, prm, cl, *tmap));
+      break;
+    }
+    case Family::ChunkedPair: {
+      const CUtensorMap* tmap2 = nullptr;
+      MTG_TRY(coeff_tmap(h, prm.coeffs, prm.B, p, 2 * p->D * p->N, &tmap2));
+      const mtg::ChunkedLaunch cl{pl.chunk, pl.park_bytes > 0 ? held->p : nullptr, pl.evict_first};
+      MTG_TRY(launch_kernel(h, (ChunkedPairKernel)pl.fn, grid, block, pl.smem, stream, prm, cl, *tmap, *tmap2));
       break;
     }
   }

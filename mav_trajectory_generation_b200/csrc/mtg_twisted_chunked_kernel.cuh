@@ -339,6 +339,8 @@ __global__ void __launch_bounds__(32 * W, 8 / W)
 // follows that tile's wait on `ready` and the landing of all its refills; this needs n >= 1 (K >= 3).
 // tests/test_k3_pair_schedule.py walks this schedule on the host.
 //
+// Output: TmaPairEmitter, or TmaEmitter where the staging of TmaPairEmitter does not fit (ChunkedPairLayout).
+//
 // RD does not enter the paired form (it has no input ring): it is the ring depth of the one-warp instantiations
 // built beside it, kept in the name so that each registry row has one paired kernel of a fixed name.
 template <int N, int D, int RD>
@@ -351,14 +353,23 @@ struct ChunkedPairLayout {
   static constexpr int kHand = h * D;                // handoff: the starting ed of the outward sweep
   static constexpr int kMaxChunk = 30;               // mbarriers: freed[C], ready, full
   static constexpr size_t kBarBytes = 8 * (kMaxChunk + 2);
-  static constexpr size_t stage_bytes = tmem_stage_bytes<N, D, 32>();  // the outward warp's staging tile
+  static constexpr int end = 0;
+  static constexpr int hand = end + kEnd;
+  static constexpr int times = hand + kHand;         // then C slot times, then C blocks
+  // The outward warp stores two segments per box (TmaPairEmitter) from two buffers of [half][16 rows][two segments],
+  // four times the staging of one segment per box (TmaEmitter).  It does so where two CTAs per SM still fit with that
+  // staging at K = 16 with all 7 blocks of a lane resident: the default route runs the paired form there at two pairs
+  // per SM (plan_chunked), and the wider staging must not push a shape off it.  That holds up to D*N = 32; N = 10 at
+  // D = 4 and N = 12 at D >= 3 store one segment per box.
+  static constexpr size_t kTile = tmem_stage_bytes<N, D, 32>();
+  static constexpr size_t kPairCtaAtK16 = 4 * kTile + kBarBytes + 8 * (16 * 16 + 16 * D * (2 * h + 15)) +
+                                          tmem_slot_bytes(times + 7 + 7 * kSlots, 32);
+  static constexpr bool kStorePairs = 2 * (kPairCtaAtK16 + 1024) <= 228 * 1024;
+  static constexpr size_t stage_bytes = (kStorePairs ? 4 : 1) * kTile;
   static constexpr size_t tile_offset = stage_bytes + kBarBytes;      // 16-byte aligned: the bulk copies land here
   static_assert(tile_offset % 16 == 0, "tile input buffer alignment");
   // doubles of the tile input buffer: seg_times[16][K], then d_fixed[16][D][nf] (both multiples of 16 bytes)
   __host__ __device__ static constexpr size_t tile_doubles(int K, int nf) { return size_t(16) * K + size_t(16) * D * nf; }
-  static constexpr int end = 0;
-  static constexpr int hand = end + kEnd;
-  static constexpr int times = hand + kHand;         // then C slot times, then C blocks
   __host__ __device__ static constexpr size_t region(int C) { return size_t(times) + C; }
   __host__ __device__ static constexpr size_t bytes(int C, int K, int nf) {
     return tile_offset + tile_doubles(K, nf) * 8 + tmem_slot_bytes(region(C) + size_t(C) * kSlots, 32);
@@ -386,11 +397,77 @@ __device__ __forceinline__ void mbar_wait_parity(uint32_t bar, uint32_t parity) 
         : "memory");
 }
 
+// waits until at most one bulk group of this thread is still reading shared memory
+__device__ __forceinline__ void bulk_wait_read_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
+
+// Output of the paired kernel's outward warp.  A half stores its segments in boxes of two consecutive global
+// segments (2i, 2i+1): 16 rows x 2*D*N doubles against `tmap2`.  Its pieces are 16*D*N bytes apart, so at N = 10,
+// D = 3 and even K every one starts on a 32-byte sector of the output (one segment, 240 bytes, starts every other
+// one 16 bytes into a sector, and its neighbour follows a step later).  The forward half emits ..., 3, 2 | 1, 0 and the backward half M, M+1 | ... | K-2, K-1 (M = ceil(K/2)); a
+// segment whose partner belongs to the other half (n even; M odd; K-1 even) is stored alone, 16 rows x D*N against
+// `tmap`.  Each half alternates between two staging buffers box by box, and lane `half` issues its half's stores
+// into its own bulk groups (one per box), so the first write of a box waits only until the store of the box before
+// the last one has read its buffer.
+template <int N, int D, class AI>
+struct TmaPairEmitter {
+  static constexpr int h = N / 2;
+  static constexpr int kSeg = D * h;  // double2 of one segment
+  const CUtensorMap* tmap;            // box 16 x D*N
+  const CUtensorMap* tmap2;           // box 16 x 2*D*N
+  double2* stage;                     // the warp's staging [buffer][half][16 rows][2 * kSeg]
+  int lane, K;
+  int nh;                             // this lane's half is active in sweep step v iff v <= nh
+  bool evict_first;                   // stores marked evict-first in L2
+  int nbox = 0;                       // boxes stored by this lane's half (its buffer is nbox % 2)
+  __device__ __forceinline__ void store(const CUtensorMap* map, const void* ssrc, int c0, int c1) const {
+    if (evict_first) tma_store_box_evict_first(map, ssrc, c0, c1);
+    else tma_store_box(map, ssrc, c0, c1);
+  }
+  // emit own-frame segment v (sweep step v; 0 = final) for every lane of the warp at once (convergent)
+  __device__ __forceinline__ void emit(int v, double T, double iT, const double (&sd)[h][D], const double (&ed)[h][D],
+                                       long long traj0) {
+    using HF = sweep::Hermite<N, AI>;
+    const int half = lane & 1;
+    const int g = half ? K - 1 - v : v;  // global segment
+    const bool act = v <= nh;
+    const bool next = (g & 1) != half;  // the partner g^1 is this half's segment of step v-1 (else of step v+1)
+    const bool open = act && next && v >= 1;
+    const bool close = act && !next && v + 1 <= nh;
+    double2* buf = stage + size_t((nbox & 1) * 2 + half) * 16 * (2 * kSeg);
+    double2* row = open || close ? buf + (lane >> 1) * (2 * kSeg) + (g & 1) * kSeg : buf + (lane >> 1) * kSeg;
+    double tp[h], itp[h];
+    HF::powers(T, iT, half, tp, itp);
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+      double c[N];
+      HF::template coeffs<D>(half, tp, itp, sd, ed, d, c);
+      if (d == 0) {  // a box's buffer is free once the store of the box before the last one has read it
+        if (lane == half && act && !close) bulk_wait_read_1();
+        __syncwarp();
+      }
+      if (act) {
+#pragma unroll
+        for (int q = 0; q < h; ++q) row[d * h + q] = make_double2(c[2 * q], c[2 * q + 1]);
+      }
+    }
+    fence_proxy_async();
+    __syncwarp();
+    if (act && !open) {
+      if (lane == half) {
+        if (close) store(tmap2, buf, (g & ~1) * (D * N), (int)traj0);
+        else store(tmap, buf, g * (D * N), (int)traj0);
+        bulk_commit();
+      }
+      ++nbox;
+    }
+  }
+};
+
 // 64 threads, at most 4 CTAs per SM by registers (cap 255)
 template <int N, int R, int D, int RD>
 __global__ void __launch_bounds__(64, 4)
     twisted_chunked_pair_kernel(const WaypointParams prm, const ChunkedLaunch cl,
-                                const __grid_constant__ CUtensorMap tmap) {
+                                const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap2) {
   constexpr int h = N / 2;
   constexpr int m = h - 1;
   using Lay = ChunkedPairLayout<N, D, RD>;
@@ -586,9 +663,13 @@ __global__ void __launch_bounds__(64, 4)
   }
 
   // ================================================================== warp 1: outward sweep, final segment
-  double2* my_row = stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h);
-  const int nhF = M - 1, nhB = K - M - 1;
-  const TmaEmitter<N, D, AI> out{&tmap, stage, my_row, lane, K, nhF, nhB, cl.evict_first != 0};
+  const TmaEmitter<N, D, AI> out1{&tmap, stage, stage + ((lane & 1) * 16 + (lane >> 1)) * (D * h), lane, K, M - 1,
+                                  K - M - 1, cl.evict_first != 0};
+  TmaPairEmitter<N, D, AI> out2{&tmap, &tmap2, stage, lane, K, nh, cl.evict_first != 0};
+  auto emit = [&](int v, double T, double iT, const double (&sd)[h][D], const double (&ed)[h][D], long long traj0) {
+    if constexpr (Lay::kStorePairs) out2.emit(v, T, iT, sd, ed, traj0);
+    else out1.emit(v, v, T, iT, sd, ed, traj0);
+  };
 
   long long j = 0;
   for (long long wt = blockIdx.x; wt < n_wtiles; wt += wt_stride, ++j) {
@@ -644,7 +725,7 @@ __global__ void __launch_bounds__(64, 4)
         store_free(v, sd);
       }
       __syncwarp();
-      out.emit(v, v, T, iT, sd, ed, traj0);
+      emit(v, T, iT, sd, ed, traj0);
       if (act) {
 #pragma unroll
         for (int d = 0; d < D; ++d)
@@ -664,10 +745,10 @@ __global__ void __launch_bounds__(64, 4)
       mbar_arrive(bar0 + 8u * uint32_t(slot_of(1, j)));  // vertex 1's slot and END are the next tile's
       const double iT = fast_rcp(T);
       __syncwarp();
-      out.emit(0, 0, T, iT, sd, ed, traj0);
+      emit(0, T, iT, sd, ed, traj0);
     }
   }
-  if (lane == 0) bulk_wait_all();
+  if (lane < (Lay::kStorePairs ? 2 : 1)) bulk_wait_all();  // lane `half` stores each half's pairs
 }
 
 }  // namespace mtg

@@ -39,10 +39,11 @@ def k3_smem(C, W, K):
     ChunkedPairLayout<10, 3, 3>::bytes)"""
     h, slots = N // 2, 25
     pro = 2 * D + (h - 1) * D + 1
-    if W == 2:  # one staging tile; mbarriers; tile input buffer; final-segment inputs, handoff, times, blocks
+    if W == 2:  # two staging buffers of two segments per row; mbarriers; tile input buffer; final-segment inputs,
+        # handoff, times, blocks
         tile = 8 * 16 * (K + D * (2 * h + K - 1))
         region = (D + (h - 1) * D + 1) + h * D + C
-        return 32 * (D * h * 16) + 256 + tile + 32 * 8 * (region + C * slots)
+        return 4 * 32 * (D * h * 16) + 256 + tile + 32 * 8 * (region + C * slots)
     region = 3 * (1 + D) + C + D + 1
     return 32 * W * (D * h * 16 + 8 * (region + max(C * slots, pro)))
 
